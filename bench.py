@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- throughput of the two G2Vec hot paths on B200 (BASELINE.json metric:
-"CBOW context-windows/sec and random-walk steps/sec at 1/2/4/8 B200 vs CPU ref").
+"""bench.py -- throughput of the two G2Vec hot paths on H100 (BASELINE.json metric:
+"CBOW context-windows/sec and random-walk steps/sec at 1/2/4/8 GPUs vs CPU ref").
 
     python bench.py --gpus N --steps K --warmup W          # this repo's CUDA path
     python bench.py --impl reference --gpus N ...          # the reference's own CPU implementation
+    python bench.py ... --dump-outputs DIR                 # also write what the timed path computed (DIR/<name>.npy)
 
 One "step":  CBOW  = one iteration of the reference's training loop (G2Vec.py:262-267): a full-batch
                      optimizer step over all training windows (fwd+bwd+[all-reduce]+update) plus the
@@ -18,9 +19,9 @@ line.  Workload at N=1: BASELINE configs[1] (synthetic 10k genes / 500k edges pe
 work (numRepetition = 10*N), parameters replicated, dense gradient NCCL-all-reduced once per step.
 
 Extra blocks of the same JSON line:
-  roofline       the fused fwd+bwd kernel of the headline config.  Its table + gradient (10 MB) live in the L2, so
-                 the bound is the L2 / L1TEX path, and the peak it is divided by is MEASURED in the same run:
-                 g2v_test_l2_rows reads / red.adds the same rows with the arithmetic removed.
+  roofline       the fused fwd+bwd kernel of the headline config.  Its table + gradient (10 MB) fit the L2, so
+                 the peak it is divided by is MEASURED in the same run: g2v_test_l2_rows reads / red.adds the same
+                 rows with the arithmetic removed.
   roofline_hbm   (N=1) the same kernel on BASELINE configs[4]'s table -- 200k genes x 512 = 410 MB, far beyond the
                  L2 -- on synthetic windows (SURVEY 8d: 80 distinct genes, seed 777): the single-pass kernel against
                  the measured HBM peak, and the gene-slab passes that ship for such tables (csrc/g2v_cbow_slab.cu).
@@ -32,7 +33,7 @@ Extra blocks of the same JSON line:
                  total work fixed, walkers and windows sharded over the N ranks.
 
 Timing: CUDA events on the launching stream, W warm-up steps, L2 flushed (256 MiB write) before every
-timed step, max over ranks.  CPU baseline: the UNMODIFIED reference (oracle/_ref/G2Vec.py, staged by
+timed step, max over ranks.  --steps K sets the number of timed steps of every timed block.  CPU baseline: the UNMODIFIED reference (oracle/_ref/G2Vec.py, staged by
 __graft_entry__.build(); its TF 1.x ops on oracle/tf1_shim.py) on a bounded sample, on this box's host cores.
 """
 import argparse
@@ -74,7 +75,12 @@ def parse():
     p.add_argument("--strong-workloads", nargs="*", default=["syn50k", "syn20k"])
     p.add_argument("--cpu-sample-windows", type=int, default=16384)
     p.add_argument("--cpu-walk-seconds", type=float, default=8.0)
-    return p.parse_args()
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="write the headline walk pass's and CBOW step's outputs of the last timed step as DIR/<name>.npy")
+    a = p.parse_args()
+    if a.steps < 1 or a.warmup < 0:
+        p.error("--steps must be >= 1 and --warmup >= 0")
+    return a
 
 
 def workload(name):
@@ -88,28 +94,29 @@ def workload(name):
     return gs, V, D, L, "synthetic directed ER, %d genes / %d edges per group, weights U(0.5,1)" % (V, E)
 
 
-_RUN = {"reps": None, "world": 1}
-
-
-def traffic_lookup(kernel, workload_name, need_reps=None):
-    """DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of the named kernel from the
-    committed ncu capture of this same command (profiles/traffic.json); None when no capture exists for this
-    workload / numRepetition / GPU count."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            e = json.load(f)[kernel][workload_name]
-        reps = _RUN["reps"] if need_reps is None else need_reps
-        return e["dram_bytes"] if (e.get("reps") == reps and _RUN["world"] == 1) else None
-    except Exception:
-        return None
-
-
 def peaks():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s), not measured"
+
+
+def dump_sample(n, k, seed=0):
+    """Sorted ids of a fixed, seeded sample of k of n rows (all of them when n <= k)."""
+    if n <= k:
+        return np.arange(n)
+    return np.sort(np.random.RandomState(seed).choice(n, size=k, replace=False))
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each array as out_dir/<name>.npy: integers as float64 (exact), floats as float32; 64 MB at most in all."""
+    arrays = {k: np.asarray(a) for k, a in arrays.items()}
+    arrays = {k: a.astype(np.float64) if a.dtype.kind in "iub" else a.astype(np.float32) for k, a in arrays.items()}
+    assert sum(a.nbytes for a in arrays.values()) <= 64 << 20, "--dump-outputs: more than 64 MB"
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 class ClockSampler:
@@ -216,10 +223,11 @@ def run_b200(args):
         torch.cuda.synchronize()
 
     K, W = args.steps, args.warmup
-    _RUN.update(reps=args.reps, world=world)
     flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     ev = lambda: torch.cuda.Event(enable_timing=True)
     peak, peak_src = peaks()
+    l2_bytes = torch.cuda.get_device_properties(dev).L2_cache_size
+    dumped = {}                                  # --dump-outputs: host copies of the timed path's last outputs
 
     def timed(fn, n, marks=0):
         """n steps, each: L2 flush, start event, fn(marks...), end event.  Returns per-step ms (+ inner marks)."""
@@ -239,7 +247,7 @@ def run_b200(args):
     launches0 = _capi.launch_count()
 
     # ------------------------------------------------------------------------------------------ one pipeline
-    def pipeline(wl_name, reps_total, hidden=None, want_e2e=False, want_cbow_detail=False, steps=K, warm=W):
+    def pipeline(wl_name, reps_total, hidden=None, want_e2e=False, want_dump=False, steps=K, warm=W):
         """Walks -> windows -> CBOW steps for one workload; walkers rank::world, windows of the rank's own walkers."""
         gs, V, D, L, desc = workload(wl_name)
         D = hidden or D
@@ -260,7 +268,7 @@ def run_b200(args):
         # visit-order pass first: the byte model needs to know which visits scanned their row
         timed(lambda: walk_pass(False), max(1, warm))
         barrier()
-        vt, _ = timed(lambda: walk_pass(False), min(steps, 5))
+        vt, _ = timed(lambda: walk_pass(False), steps)
         barrier()
         visits = allsum(int(sum(int(o[1].sum()) for o in outs)))
         # algorithmic bytes of one pass: per visit 4 B (node id written); per visit that scans its row
@@ -279,10 +287,15 @@ def run_b200(args):
         wt, _ = timed(walk_pass, steps)
         barrier()
         walk_launches = _capi.launch_count() - l0
+        if want_dump:                            # the last timed pass's canonical rows (seeded sample of walkers)
+            idx = torch.from_numpy(dump_sample(2 * n_walk, 4096)).to(dev)
+            dumped.update(walk_rows=all_rows[idx].cpu().numpy(), walk_lens=all_lens[idx].cpu().numpy(),
+                          walk_sample_walkers=idx.cpu().numpy())
         walk_ms = allmax(float(np.mean(wt)))
         res = {"V": V, "D": D, "L": L, "desc": desc, "walk_ms": walk_ms, "walk_visit_order_ms": allmax(float(np.mean(vt))),
                "visits": visits, "walk_launches": walk_launches, "n_walk": n_walk, "wbytes": wbytes,
-               "walk_gbs": wbytes / (float(np.mean(wt)) * 1e-3) / 1e9, "layout": graphs[0].layout}
+               "walk_gbs": wbytes / (float(np.mean(wt)) * 1e-3) / 1e9, "layout": graphs[0].layout,
+               "csr_bytes": sum(4 * len(rp) + 8 * len(col) for rp, col, _ in gs)}
 
         if want_e2e:
             qws = [g2v.graph.quantise_weights(w) for _, _, w in gs]
@@ -292,16 +305,20 @@ def run_b200(args):
                                             walker_begin=rank, walker_stride=world)
             walk_host_pass()
             barrier(); t0 = time.perf_counter()
-            for _ in range(max(1, min(steps, 3))):
+            for _ in range(steps):
                 walk_host_pass()
-            barrier(); dt = allmax((time.perf_counter() - t0) / max(1, min(steps, 3)))
+            barrier(); dt = allmax((time.perf_counter() - t0) / steps)
             csr_b = sum(4 * (len(rp)) + 8 * len(col) for rp, col, _ in gs)
             res["walk_e2e"] = {"value": visits / dt, "unit": "steps/s", "h2d_bytes_per_step": int(csr_b),
                                "d2h_bytes_per_step": int(2 * n_walk * (L + 1) * 4), "api": "g2v_walk_host (C ABI, host buffers)"}
 
         # ---- windows from the walks: set semantics of G2Vec.py:351,313 + CSR + geneFreq (csrc/g2v_paths.cu)
         grp = torch.cat([torch.zeros(n_walk, dtype=torch.uint8, device=dev), torch.ones(n_walk, dtype=torch.uint8, device=dev)])
-        rowptr, gene, label, _code = paths.build_windows(all_rows, all_lens, all_keys, grp, V)   # sort-free set pipeline
+        rowptr, gene, label, code = paths.build_windows(all_rows, all_lens, all_keys, grp, V)    # sort-free set pipeline
+        if want_dump:
+            wi = torch.from_numpy(dump_sample(int(rowptr.shape[0]) - 1, 65536)).to(dev)
+            dumped.update(windows_len=(rowptr[wi + 1] - rowptr[wi]).cpu().numpy(), windows_label=label[wi].cpu().numpy(),
+                          windows_sample=wi.cpu().numpy(), gene_freq_code=code.cpu().numpy())
         del all_rows, all_lens, all_keys, grp, outs
         N_loc = int(rowptr.shape[0]) - 1
         lens_np = np.diff(rowptr.cpu().numpy()).astype(np.int64)
@@ -312,13 +329,14 @@ def run_b200(args):
         res.update(n_tr=n_tr_tot, n_va=n_va_tot, mean_len=float(lens_np.mean()), ltr=lens_np[tr], gs=gs,
                    windows=(rowptr, gene, label), tr_d=tr_d, va_d=va_d)
 
-        def measure(algo):
+        def measure(algo, dump=False):
             model = g2v.CbowModel(rowptr, gene, label, V, D, W0, Wo0, optimizer=args.optimizer, lr=0.005, algo=algo,
                                   nvl_group=dist.group.WORLD if (world > 1 and algo == "rows") else None)
             model.prepare_csc(tr_d)                    # rank1: transposed incidence of the static training list
             slabs = model.prepare_slabs(tr_d)          # rows, table > L2: gene-slab passes
             model.prepare_slabs(va_d)
-            loop = cbow.DeviceLoop(model, ddist, tr_d, va_d, n_tr_tot, 512, False)
+            # the loop's step cap must not end the timed steps early: eager, graph and 5-step-graph blocks, and e2e
+            loop = cbow.DeviceLoop(model, ddist, tr_d, va_d, n_tr_tot, max(512, warm + steps + 16), False)
             loop.attach()
             try:
                 timed(lambda *m: loop.one(True, *m), warm, marks=3)
@@ -341,11 +359,17 @@ def run_b200(args):
                     gt, _ = timed(g_full.replay, steps)
                     barrier()
                     r["step_ms"], r["graph"] = allmax(float(np.mean(gt))), True
+                    if dump:                    # the weights train_cbow returns, after the last timed step
+                        wi = dump_sample(V, 4096) if V * D * 4 > (16 << 20) else np.arange(V)
+                        dumped.update(cbow_W_ih=model.W_ih[torch.from_numpy(wi).to(dev)].cpu().numpy(),
+                                      cbow_W_ho=model.W_ho.cpu().numpy())
+                        if len(wi) < V:
+                            dumped["cbow_W_ih_sample_rows"] = wi
                     loop.reset()
                     g_prod = loop.capture([False] * 4 + [True])
                     timed(g_prod.replay, 1)
                     barrier()
-                    pt, _ = timed(g_prod.replay, max(2, steps // 5 + 1))
+                    pt, _ = timed(g_prod.replay, -(-steps // 5))
                     barrier()
                     r["prod_ms"] = allmax(float(np.mean(pt))) / 5.0
                 except Exception as exc:                # collectives not capturable on this box: eager numbers stand
@@ -363,25 +387,24 @@ def run_b200(args):
 
     # ------------------------------------------------------------------------------------------ headline
     reps_total = args.reps * (world if args.scaling == "weak" else 1)
-    P = pipeline(args.workload, reps_total, want_e2e=not args.no_e2e)
+    want_dump = args.dump_outputs is not None and rank == 0
+    P = pipeline(args.workload, reps_total, want_e2e=not args.no_e2e, want_dump=want_dump)
     V, D, L, desc = P["V"], P["D"], P["L"], P["desc"]
     n_tr_tot, n_va_tot, ltr = P["n_tr"], P["n_va"], P["ltr"]
     rowptr, gene, label = P["windows"]
-    l2_bytes = 126e6
     walkers_total = int(allsum(2 * P["n_walk"]))
     WALK = {"metric": "random_walk_steps_per_sec", "value": P["visits"] / (P["walk_ms"] * 1e-3), "unit": "steps/s",
             "ms_per_pass": P["walk_ms"], "walkers": walkers_total, "visits_per_pass": P["visits"],
             "mode": "tuple(sorted(path)) fused into the sampler (sorted rows + 64-bit keys out); graph packed as "
                     + {1: "{col, qw} pairs (8 B per edge)", 2: "16+16-bit words (4 B per edge, two neighbours per lane)"}[P["layout"]],
             "visit_order_ms_per_pass": P["walk_visit_order_ms"],
-            "roofline": {"kernel": "walk_kernel", "bound": "issue", "achieved": P["walk_gbs"], "peak": peak,
-                         "unit": "GB/s", "frac": P["walk_gbs"] / peak,
-                         "traffic": traffic_lookup("walk", args.workload),
+            "roofline": {"kernel": "walk_kernel", "bound": "not measured", "achieved": P["walk_gbs"], "peak": peak,
+                         "unit": "GB/s", "frac": P["walk_gbs"] / peak, "peak_source": peak_src,
                          "algorithmic_bytes_per_pass": P["wbytes"],
                          "bytes_model": "4 B per visit + (8 + 8*deg) B per visit that scans its row",
-                         "note": "ncu: the CSR is L2-resident (DRAM traffic 0.1 % of the algorithmic bytes) and the kernel is "
-                                 "bound by instruction issue (75-87 % of the issue slots), not by bytes; the fraction of the HBM "
-                                 "peak is reported because SURVEY 8d defines the walk roofline that way"},
+                         "note": "the packed CSR (%.0f MB) is re-read by every walker and can stay in the L2; the fraction "
+                                 "of the HBM peak is reported because SURVEY 8d defines the walk roofline that way"
+                                 % (P["csr_bytes"] / 1e6)},
             "e2e": P.get("walk_e2e")}
     walk_launches = P["walk_launches"]
 
@@ -407,14 +430,13 @@ def run_b200(args):
         if algo == "rows":
             b = int((ltr * (8 * D + 4) + 5).sum())          # SURVEY 8d: l*(8D+4)+5 per window
             gbs = b / (r["fb_ms"] * 1e-3) / 1e9
-            resident = 2 * V * D * 4 < 0.75 * l2_bytes
+            resident = 2 * V * D * 4 <= 0.9 * l2_bytes            # g2v_cbow_slab_plan's rule
             out = {"kernel": ("cbow_slab_fwd_kernel + cbow_slab_bwd_kernel passes (%d gene slabs)" % r["n_slabs"]) if r["slabs"]
                              else "cbow_rows_kernel<%d,true> (fused gather/sum/logit/BCE/scatter-add)" % max(D // 128, 0),
                    "achieved": gbs, "unit": "GB/s", "kernel_ms": r["fb_ms"], "algorithmic_bytes_per_launch": b,
                    "bytes_model": "sum over this rank's training windows of l*(8D+4)+5; the optimizer epilogue "
                                   "(%d B) is a separate kernel" % opt_b,
-                   "hbm_peak": peak, "frac_of_hbm_peak": gbs / peak, "peak_source": peak_src,
-                   "traffic": traffic_lookup("cbow_rows_fwdbwd", args.workload)}
+                   "hbm_peak": peak, "frac_of_hbm_peak": gbs / peak, "peak_source": peak_src}
             if resident and D in (128, 256, 512) and not r["slabs"]:
                 pk = l2_rows_peak(r["model"])
                 half = float(ltr.sum()) * D * 4               # bytes gathered = bytes added
@@ -426,16 +448,14 @@ def run_b200(args):
                                      "how": "g2v_test_l2_rows on the same table and the same row ids, arithmetic removed; "
                                             "the two streams overlap, so peak = bytes / max(gather bytes / gather rate, added bytes / RED rate) "
                                             "= 2 x the RED rate here: the L2 atomic units are the ceiling"},
-                           note="W_ih + gradient (%.0f MB) are L2-resident at this config (ncu: DRAM traffic 0.5 %% of the "
-                                "algorithmic bytes, l1tex 77 %%, lts 65 %%): the bound is the L2/L1TEX path, not HBM; "
-                                "frac_of_hbm_peak is kept only for reference" % (2 * V * D * 4 / 1e6))
+                           note="W_ih + gradient (%.0f MB) fit the L2 (%.0f MB) at this config: the bound is the L2/L1TEX "
+                                "path, not HBM; frac_of_hbm_peak is kept only for reference" % (2 * V * D * 4 / 1e6, l2_bytes / 1e6))
             elif r["slabs"]:
                 out.update(bound="l2", peak=peak, frac=gbs / peak,
                            note="W_ih + gradient (%.0f MB) exceed the L2; the step runs gene slab by gene slab so that rows are "
-                                "L2-resident within a pass (forward: L2 reads; backward: L2 atomic units -- ncu l1tex 87 %%, lts "
-                                "61 %%, DRAM ~0): the algorithmic rate is divided by the measured HBM peak only for reference "
-                                "and exceeds it; the single-pass kernel on this table is 0.74 of the HBM peak (roofline_hbm)"
-                                % (2 * V * D * 4 / 1e6))
+                                "L2-resident within a pass (forward: L2 reads; backward: L2 atomic units): the algorithmic "
+                                "rate is divided by the HBM peak only for reference; roofline_hbm compares the single-pass "
+                                "kernel on a table of this kind" % (2 * V * D * 4 / 1e6))
             else:
                 out.update(bound="hbm", peak=peak, frac=gbs / peak,
                            note="W_ih + gradient (%.0f MB) exceed the L2" % (2 * V * D * 4 / 1e6))
@@ -445,13 +465,15 @@ def run_b200(args):
         gbs = b / (ms * 1e-3) / 1e9
         return {"kernel": "r1_update_kernel + r1_update_ho_kernel + r1_prepare_kernel (dense optimizer pass)",
                 "bound": "hbm", "achieved": gbs, "peak": peak, "unit": "GB/s", "frac": gbs / peak,
-                "traffic": traffic_lookup("r1_update", args.workload), "peak_source": peak_src, "kernel_ms": ms,
+                "peak_source": peak_src, "kernel_ms": ms,
                 "algorithmic_bytes_per_launch": b,
                 "bytes_model": "28*V*D (Adam: read W,m,v + write W,m,v, then re-read W for s); the window kernels "
                                "(forward + CSC segmented sum) move only %d B (16*l+9 per window) in %.3f ms"
                                % (int((ltr * 16 + 9).sum()), r["fb_ms"])}
 
-    main = P["measure"](args.algo)
+    main = P["measure"](args.algo, dump=want_dump)
+    if want_dump:
+        dump_outputs(args.dump_outputs, dumped)
     main_roofline = roofline_of(args.algo, main)
     alt = "rank1" if args.algo == "rows" else "rows"
     ALT = None
@@ -524,7 +546,7 @@ def run_b200(args):
     # ------------------------------------------------------------------------------------------ roofline_hbm
     hbm = None
     if world == 1 and not args.no_hbm:
-        hbm = roofline_hbm(args, g2v, cbow, dev, timed, peak, peak_src, K, W)
+        hbm = roofline_hbm(args, g2v, cbow, dev, timed, peak, peak_src, K, W, l2_bytes)
 
     # ------------------------------------------------------------------------------------------ parity (N>1)
     parity = None
@@ -536,7 +558,7 @@ def run_b200(args):
     if not args.no_strong and args.scaling == "weak" and args.workload == "syn10k":
         strong = {}
         for wl in args.strong_workloads:
-            S = pipeline(wl, 10, steps=max(3, K // 2), warm=2)
+            S = pipeline(wl, 10)
             r = S["measure"]("rows")
             r.pop("model"); r.pop("loop")
             strong[wl] = {"value": r["value"], "unit": UNIT, "ms_per_step": r["step_ms"], "windows_train": S["n_tr"],
@@ -610,9 +632,9 @@ def run_b200(args):
         dist.destroy_process_group()
 
 
-def roofline_hbm(args, g2v, cbow, dev, timed, peak, peak_src, K, W):
+def roofline_hbm(args, g2v, cbow, dev, timed, peak, peak_src, K, W, l2_bytes):
     """The fused CBOW kernel where it is genuinely HBM-bound: BASELINE configs[4]'s table (200k genes x 512 = 410 MB,
-    3x the L2) on synthetic windows (SURVEY 8d: 80 distinct genes uniform, labels Bernoulli(0.5), seed 777)."""
+    8x H100's L2) on synthetic windows (SURVEY 8d: 80 distinct genes uniform, labels Bernoulli(0.5), seed 777)."""
     import torch
     V, D, L = 200_000, 512, 80
     N = 2 * args.hbm_reps * V
@@ -633,8 +655,8 @@ def roofline_hbm(args, g2v, cbow, dev, timed, peak, peak_src, K, W):
         m = g2v.CbowModel(rowptr, gene, label, V, D, W0, Wo0, lr=0.005)
         m.prepare_slabs(tr)
         fn = lambda: m.fwdbwd(tr, n_tr)
-        timed(fn, max(W, 3))
-        t, _ = timed(fn, max(K, 5))
+        timed(fn, W)
+        t, _ = timed(fn, K)
         ms = float(np.mean(t))
         out[kind] = {"ms": ms, "achieved": alg / (ms * 1e-3) / 1e9, "n_slabs": getattr(m, "_n_slabs", 1)}
         del m
@@ -644,22 +666,19 @@ def roofline_hbm(args, g2v, cbow, dev, timed, peak, peak_src, K, W):
     return {"kernel": "cbow_rows_kernel<4,true> (fused gather/sum/logit/BCE/scatter-add, ONE launch per step)",
             "bound": "hbm", "achieved": sp["achieved"], "peak": peak, "unit": "GB/s", "frac": sp["achieved"] / peak,
             "kernel_ms": sp["ms"], "algorithmic_bytes_per_launch": alg, "peak_source": peak_src,
-            "traffic": traffic_lookup("cbow_rows_fwdbwd", "stress200k", need_reps=args.hbm_reps),
             "config": {"workload": "CBOW only: %d synthetic windows of %d distinct genes (seed 777), %d of them training, "
-                                   "V = %d, hidden %d: W_ih and the gradient are 410 MB each (L2: 126 MB)" % (N, L, n_tr, V, D),
-                       "l2": "256 MiB flush write before every timed launch", "steps": max(K, 5), "warmup": max(W, 3)},
-            "note": "every gathered row and every red.global.add into the gradient misses the L2 in this form: ncu of this "
-                    "command shows DRAM traffic 1.30x the algorithmic bytes (the reduction is a DRAM read-modify-write)",
+                                   "V = %d, hidden %d: W_ih and the gradient are 410 MB each (L2: %.0f MB)"
+                                   % (N, L, n_tr, V, D, l2_bytes / 1e6),
+                       "l2": "256 MiB flush write before every timed launch", "steps": K, "warmup": W},
+            "note": "in this form the gathered rows and the red.global.add into the gradient cannot stay in the L2: the "
+                    "reduction is a DRAM read-modify-write",
             "shipped": {"kernel": "cbow_slab_fwd_kernel x %d + cbow_slab_bwd_kernel x %d (gene slabs, csrc/g2v_cbow_slab.cu): "
                                   "what train_cbow runs for tables larger than the L2"
                                   % ((sl["n_slabs"] + 1) // 2, sl["n_slabs"]),
-                        "bound": "l2 (forward: L2 reads; backward: L2 atomic units, ncu lts 61 % / l1tex 87 %)",
+                        "bound": "l2 (forward: L2 reads; backward: L2 atomic units)",
                         "ms": sl["ms"], "achieved": sl["achieved"], "unit": "GB/s", "frac_of_hbm_peak": sl["achieved"] / peak,
                         "speedup_vs_single_pass": sp["ms"] / sl["ms"],
-                        "traffic": traffic_lookup("cbow_slab_step", "stress200k", need_reps=args.hbm_reps),
-                        "note": "same algorithmic bytes in less time: rows are served by the L2 after their first touch in a "
-                                "slab pass, so the algorithmic rate exceeds the HBM peak while DRAM traffic falls to ~0.15x the "
-                                "algorithmic bytes (profiles/r2)"}}
+                        "note": "same algorithmic bytes: rows are served by the L2 after their first touch in a slab pass"}}
 
 
 def parity_block(g2v, dist, rank, world, dev, gs, V, L):

@@ -81,7 +81,7 @@ def load():
     global _lib
     if _lib is not None:
         return _lib
-    path = os.environ.get("G2VEC_B200_LIB") or _build.LIB     # A/B builds of the same ABI (profiles/variants)
+    path = os.environ.get("G2VEC_B200_LIB") or _build.LIB     # A/B builds of the same ABI
     if path == _build.LIB and _build.stale():
         try:
             _build.build_library()

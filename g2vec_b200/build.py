@@ -1,4 +1,4 @@
-"""Build libg2vec_b200.so (hand-written sm_100a CUDA + the C ABI of include/g2vec_b200.h).
+"""Build libg2vec_b200.so (hand-written sm_90a CUDA + the C ABI of include/g2vec_b200.h).
 
 nvcc cross-compiles without a GPU; the .so is built IN-TREE (g2vec_b200/libg2vec_b200.so,
 git-ignored) so that it travels to the GPU box with the repo snapshot.
@@ -14,7 +14,7 @@ CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libg2vec_b200.so")
 
 NVCC_FLAGS = [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared", "--expt-relaxed-constexpr",
 ]
 

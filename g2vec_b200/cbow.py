@@ -64,7 +64,7 @@ class CbowModel:
     def __init__(self, rowptr, gene, label, n_genes, hidden, W_ih0, W_ho0, optimizer="adam", reduce="sum",
                  lr=0.005, beta1=0.9, beta2=0.999, eps=1e-8, device=None, algo="rows", nvl_group=None):
         if not torch.cuda.is_available():
-            raise RuntimeError("g2vec_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise RuntimeError("g2vec_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.lib = _capi.load()
         dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self.device = dev

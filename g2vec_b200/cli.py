@@ -1,4 +1,4 @@
-"""The G2Vec command line, kept as the drop-in shell around the two B200 hot paths.
+"""The G2Vec command line, kept as the drop-in shell around the two H100 hot paths.
 
 Same positionals, options, progress banners and output files as /root/reference/G2Vec.py
 (parse_arguments :505-518, main :11-119, writers :127-131,159-165,203-215).  Steps 1, 2, 5, 6, 7 are
@@ -16,7 +16,7 @@ import numpy as np
 
 def parse_arguments(argv=None):
     p = argparse.ArgumentParser(
-        description="G2Vec (B200-native hot paths): network-based identification of prognostic gene "
+        description="G2Vec (H100-native hot paths): network-based identification of prognostic gene "
                     "signatures. Same interface as mathcom/G2Vec G2Vec.py.")
     p.add_argument('EXPRESSION_FILE', type=str, help="Tab-delimited file for gene expression profiles.")
     p.add_argument('CLINICAL_FILE', type=str, help="Tab-delimited clinical file. LABEL=0: good prognosis, 1: poor.")

@@ -1,4 +1,4 @@
-// g2v_cbow.cu -- HOT PATH 2: modified CBOW (G2Vec.py:217-286) as fused sm_100a kernels.
+// g2v_cbow.cu -- HOT PATH 2: modified CBOW (G2Vec.py:217-286) as fused sm_90a kernels.
 //
 // The reference builds  H = X.W_ih ; O = H.W_ho ; cost = mean(sigmoid_BCE(O, Y))  on a dense
 // multi-hot X [N, V] (99.7 % zeros) and lets TF1 autodiff + ApplyAdam train W_ih, W_ho
@@ -27,7 +27,7 @@
 namespace g2v {
 
 constexpr bool kDefaultGatherTma = false;
-constexpr bool kDefaultScatterTma = false;   // see profiles/README.md for the measurement behind this choice
+constexpr bool kDefaultScatterTma = false;   // G2V_CBOW_SCATTER=tma selects the bulk-reduction scatter
 
 // SCATTER_TMA: the gradient row dO*W_ho (identical for every gene of the window) is staged once in
 // shared memory and added into g_ih[gene,:] with one TMA bulk reduction per gene
@@ -445,7 +445,7 @@ cbow_update_nvl_kernel(float *const *__restrict__ g_ptrs, float *const *__restri
 int rows_grid(const void *kernel, size_t smem, int64_t n_win, int *grid_out) {
     DeviceProps dp;
     if (device_props(&dp)) return 1;
-    if (dp.cc_major != 10) { set_error("needs an sm_100 device (found sm_%d%d); no CPU fallback", dp.cc_major, dp.cc_minor); return 2; }
+    if (dp.cc_major != 9) { set_error("needs an sm_90 device (found sm_%d%d); no CPU fallback", dp.cc_major, dp.cc_minor); return 2; }
     int per_sm = 0;
     cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kCbowWarps * 32, smem);
     if (e != cudaSuccess || per_sm <= 0) { set_error("occupancy query failed: %s", cudaGetErrorString(e)); return 1; }

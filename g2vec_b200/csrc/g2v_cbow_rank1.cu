@@ -273,7 +273,7 @@ r1_update_ho_kernel(float *__restrict__ W_ho, float *__restrict__ m, float *__re
 static int r1_grid(const void *kernel, size_t smem, int64_t items, int *grid_out) {
     DeviceProps dp;
     if (device_props(&dp)) return 1;
-    if (dp.cc_major != 10) { set_error("needs an sm_100 device (found sm_%d%d); no CPU fallback", dp.cc_major, dp.cc_minor); return 2; }
+    if (dp.cc_major != 9) { set_error("needs an sm_90 device (found sm_%d%d); no CPU fallback", dp.cc_major, dp.cc_minor); return 2; }
     int per_sm = 0;
     cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kR1Warps * 32, smem);
     if (e != cudaSuccess || per_sm <= 0) { set_error("occupancy query failed: %s", cudaGetErrorString(e)); return 1; }

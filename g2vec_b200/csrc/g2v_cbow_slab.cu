@@ -2,9 +2,8 @@
 // logit -> BCE -> scatter-add step as cbow_rows_kernel (g2v_cbow.cu; G2Vec.py:239-246), processed GENE SLAB BY
 // GENE SLAB so that the rows being gathered and the gradient rows being added to stay L2-resident.
 //
-// Why: with V*D*4 >> L2 (200k genes x 512: 410 MB against 126 MB) every gathered row and every
-// red.global.add into g_ih misses; the reduction is then a DRAM read-modify-write (ncu, round 1: 272 GB of DRAM
-// traffic for 210 GB algorithmic, 9 % L2 hit rate, 0.74 of the HBM peak).  The windows are static across steps
+// Why: with V*D*4 >> L2 (200k genes x 512: 410 MB against H100's 50 MB) every gathered row and every
+// red.global.add into g_ih misses; the reduction is then a DRAM read-modify-write.  The windows are static across steps
 // and their gene lists are sorted (tuple(sorted(path)), G2Vec.py:345), so the genes of a window that fall into
 // the slab [lo, hi) are ONE contiguous piece of its list.  slab_setup_kernel records those pieces once
 // (slabptr [n_win, S+1]); then per optimizer step
@@ -15,7 +14,7 @@
 //                                   accuracy, dO -> dO[n_win], and h*dO into g_ho
 //   backward pass s (S launches)    every window adds dO*W_ho into g_ih rows of its genes in slab s
 //
-// During a pass the 148 SMs only touch one slab of W_ih (forward) or g_ih (backward): after its first touch a
+// During a pass the SMs only touch one slab of W_ih (forward) or g_ih (backward): after its first touch a
 // row is served by the L2 (each row of a slab is used N*l/V times per pass -- 256 times at the stress size), and
 // DRAM sees the slab once plus the streamed hbuf/gene-id traffic.  Forward slabs may be wider than backward
 // slabs (only the table has to stay resident, not table + gradient): forward group j = backward slabs
@@ -30,7 +29,7 @@
 
 namespace g2v {
 
-constexpr bool kDefaultSlabScatterTma = false;   // set from the B200 measurement in profiles/r2
+constexpr bool kDefaultSlabScatterTma = false;   // RED.128 scatter; G2V_CBOW_SLAB_SCATTER=tma selects the bulk reduction
 
 __device__ __forceinline__ float4 ld_stream4(const float4 *p) { return __ldcs(p); }
 __device__ __forceinline__ void st_stream4(float4 *p, float4 v) { __stcs(p, v); }
@@ -182,7 +181,7 @@ cbow_slab_fwd_kernel(const int32_t *__restrict__ gene, const uint8_t *__restrict
 // VEC warp-wide RED.128 per gene row).  TMA = true: the row dO*W_ho -- the same for every gene of the
 // window -- is staged once in shared memory and added into g_ih[gene,:] with ONE bulk reduction per gene
 // (cp.reduce.async.bulk.global.shared::cta.add.f32, D*4 bytes, SASS UBLKRED) issued by one lane: the scatter
-// leaves the LSU/L1TEX path, which is what bounds the L2-resident backward passes (ncu: l1tex 87 %).
+// leaves the LSU/L1TEX path, which is what bounds the L2-resident backward passes.
 // Two staging rows per warp, so that a window's row can be written while the previous window's bulk
 // reductions are still reading theirs.
 template <int VEC, bool TMA>
@@ -296,7 +295,7 @@ static int launch_fwd_passes(const int32_t *gene, const uint8_t *label, const in
 template <int VEC>
 static int launch_bwd_passes(const int32_t *gene, int64_t n_win, const SlabLayout &l, int32_t S, const float *W_ho,
                              float *g_ih, cudaStream_t st) {
-    const char *sc = getenv("G2V_CBOW_SLAB_SCATTER");             // "tma" (default) / "red": A/B hook, see profiles/r2
+    const char *sc = getenv("G2V_CBOW_SLAB_SCATTER");             // "tma" / "red" (default): A/B hook
     const bool tma = sc ? sc[0] == 't' : kDefaultSlabScatterTma;
     auto kern = tma ? cbow_slab_bwd_kernel<VEC, true> : cbow_slab_bwd_kernel<VEC, false>;
     int grid = 0, rc;
@@ -320,12 +319,17 @@ extern "C" int g2v_cbow_slab_plan(int32_t V, int32_t D, int32_t *n_slabs) {
     *n_slabs = 1;
     if (D != 128 && D != 256 && D != 512) return 0;               // the generic-D kernel has no slab form
     const double table = (double)V * D * 4.0;
-    // table + gradient resident together: the fused single-pass kernel is already L2-bound
-    const char *e = getenv("G2V_CBOW_SLAB_MB");                   // bytes of one BACKWARD slab of g_ih (tuning hook)
-    const double slab = (e && atof(e) > 0 ? atof(e) : 32.0) * 1048576.0;
+    // table + gradient resident together: the fused single-pass kernel is already L2-bound.  Measured on H100 (50 MB
+    // L2, fwd+bwd): 20k x 256 (2 x 20.5 MB) 9.8 ms single pass vs 11.6 ms in 2 slabs; 50k x 128 (2 x 25.6 MB) 16.2 ms
+    // vs 14.2 ms -- the threshold lies between the two
+    // one BACKWARD slab of g_ih is a quarter of the L2, so that a forward group (G2V_CBOW_SLAB_FWD_GROUP = 2 slabs of
+    // W_ih) stays resident with room for the streamed window data: 12.5 MiB on H100 (measured on the 200k x 512 table:
+    // 55.8 ms per fwd+bwd in 32 slabs, 56.6 ms in 13 slabs of 32 MiB, 55.1 ms in 25 of 16 MiB)
+    const char *e = getenv("G2V_CBOW_SLAB_MB");                   // tuning hook: slab size in MiB
+    const double slab = e && atof(e) > 0 ? atof(e) * 1048576.0 : 0.25 * (double)dp.l2_bytes;
     const char *f = getenv("G2V_CBOW_SLABS");                     // force a slab count (tests)
     if (f && atoi(f) >= 1) { *n_slabs = atoi(f) > V ? V : atoi(f); return 0; }
-    if (2.0 * table <= 0.75 * (double)dp.l2_bytes) return 0;
+    if (2.0 * table <= 0.9 * (double)dp.l2_bytes) return 0;
     int s = (int)((table + slab - 1) / slab);
     if (s < 2) s = 2;
     if (s > 64) s = 64;

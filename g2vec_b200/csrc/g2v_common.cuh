@@ -1,4 +1,4 @@
-// g2v_common.cuh -- shared device/host helpers of libg2vec_b200.so (sm_100a only).
+// g2v_common.cuh -- shared device/host helpers of libg2vec_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -44,8 +44,7 @@ namespace g2v {
 constexpr int kWalkWarps = 8;   // warps per CTA
 constexpr int kKC = 2;          // neighbour chunks kept in registers on the long-row path
 // resident CTAs per SM the kernels are compiled for: 6 (register cap 40) for the bitmap variants, 8 (cap 32) for the
-// hash-set variants -- measured (profiles/r2/tune_walk_minb_r2l.txt): syn10k 1.97 ms at 6 vs 2.00 ms at 8, stress200k
-// (hash set, V = 200k) 25.0 ms at 6 vs 22.0 ms at 8
+// hash-set variants (-D overrides for tuning)
 #ifndef G2V_WALK_MINB_BITMAP
 #define G2V_WALK_MINB_BITMAP 6
 #endif
@@ -59,8 +58,8 @@ enum { LAY_CSR = 0, LAY_E8 = 1, LAY_E4 = 2 };
 // word (path append, visited insert) and later reads what it stored itself: no divergence and no warp barrier on
 // the instruction-bound path.  compute-sanitizer racecheck reports these same-value stores as warnings (never as
 // errors).  -DG2V_WALK_STRICT_SYNC builds the formally race-free form -- lane 0 stores, __syncwarp() before the
-// warp reads -- which racecheck passes with 0 hazards and which is 15 % more instructions / 20 % slower
-// (profiles/r2/walk_strict_sync_r2x.txt); both forms give bit-identical walks.
+// warp reads -- which racecheck passes with 0 hazards and which issues more instructions; both forms give
+// bit-identical walks.
 #ifdef G2V_WALK_STRICT_SYNC
 #define G2V_WALK_ONE_WRITER if (lane == 0)
 #define G2V_WALK_STEP_SYNC() __syncwarp()
@@ -642,7 +641,7 @@ static int launch_walk(const WalkGraphPtrs &g, int layout, int32_t V, int64_t E,
     G2V_REQUIRE(layout == LAY_CSR || layout == LAY_E8 || (layout == LAY_E4 && V <= 65535), "%s: bad layout %d", who, layout);
     DeviceProps dp;
     if (device_props(&dp)) return 1;
-    G2V_REQUIRE(dp.cc_major == 10, "%s: needs an sm_100 device (found sm_%d%d)", who, dp.cc_major, dp.cc_minor);
+    G2V_REQUIRE(dp.cc_major == 9, "%s: needs an sm_90 device (found sm_%d%d)", who, dp.cc_major, dp.cc_minor);
 
     const bool canon = out_key != nullptr;
     // path buffer: L ints, rounded to 32 (visit order) or to the power of two the bitonic network needs
@@ -671,10 +670,9 @@ static int launch_walk(const WalkGraphPtrs &g, int layout, int32_t V, int64_t E,
     // two walkers per warp (walk_pair_kernel): packed edges + bitmap, and both tiles' bitmaps within the 56 KB budget
     const char *ft = getenv("G2V_WALK_TILE");                    // test / A-B hook: "32" / "16" force one / two walkers per warp
     const size_t pair_smem = 2 * per_warp * (size_t)(Lpad + bm_words);
-    // ... and rows that mostly fit one 64-neighbour request (longer rows take its divergent slow path; measured: syn20k,
-    // mean degree 100, 7.4 ms against 6.4 ms with one walker per warp), on graphs dense enough that walks are long (on
-    // the ex_* graphs, mean degree 3.4 and 62 % of the walks a single node, the per-walk epilogues diverge the tiles:
-    // 0.378 ms against 0.323 ms)
+    // ... and rows that mostly fit one 64-neighbour request (longer rows take its divergent slow path, e.g. syn20k with
+    // mean degree 100), on graphs dense enough that walks are long (on the ex_* graphs, mean degree 3.4 and 62 % of
+    // the walks a single node, the per-walk epilogues diverge the tiles)
 #ifdef G2V_WALK_STRICT_SYNC
     const bool short_rows = false;                               // the strictly synchronised build keeps one walker per warp
 #else

@@ -94,7 +94,7 @@ def group_csr_gpu(expr, label, group, src, dst, threshold=0.5, device=None):
     from . import _capi
     lib = _capi.load()
     if not torch.cuda.is_available():
-        raise RuntimeError("g2vec_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise RuntimeError("g2vec_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
     x = np.ascontiguousarray(np.asarray(expr, dtype=np.float32)[np.asarray(label) == group])
     S, V = x.shape

@@ -11,7 +11,7 @@ from . import _capi, graph as _graph
 
 def _dev(device=None):
     if not torch.cuda.is_available():
-        raise RuntimeError("g2vec_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise RuntimeError("g2vec_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     return torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
 
 

@@ -1,5 +1,5 @@
 /*
- * g2vec_b200.h -- C ABI of libg2vec_b200.so: the two G2Vec hot paths as sm_100a CUDA.
+ * g2vec_b200.h -- C ABI of libg2vec_b200.so: the two G2Vec hot paths as sm_90a CUDA.
  *
  * The reference (mathcom/G2Vec) has no FFI or plugin interface: its boundary for these
  * paths is two plain Python calls in main(),
@@ -17,7 +17,7 @@
  *     it and never synchronise.  Buffers are owned by the caller.
  *   - `_host` entry points take HOST pointers, do their own device allocation and
  *     host<->device copies, and return after the result is back in host memory.
- *   - there is no CPU fallback: without a usable sm_100 device the calls fail.
+ *   - there is no CPU fallback: without a usable sm_90 device the calls fail.
  */
 #ifndef G2VEC_B200_H
 #define G2VEC_B200_H

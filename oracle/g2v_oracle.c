@@ -8,7 +8,7 @@
  * It restates, in plain scalar C, the algorithm of the reference
  *   /root/reference/G2Vec.py:324-352  generate_pathSet / generate_randomPath  (walks)
  *   /root/reference/G2Vec.py:217-286  compute_genetovec                        (CBOW)
- * on the sparse layouts the B200 path uses (CSR graph, CSR windows).
+ * on the sparse layouts the GPU path uses (CSR graph, CSR windows).
  *
  * Parity status:
  *   walks  -- the walk LOGIC (directed rows, every gene starts a walk, append-then-test,

@@ -1,6 +1,6 @@
 """CPU checks of bench.py's own pieces: the synthetic window generator of the roofline_hbm block (SURVEY 8d: distinct,
 sorted genes), the counting adjacency that lets the UNMODIFIED generate_pathSet be timed on a bounded sample, and the
-traffic lookup."""
+--dump-outputs writer."""
 import os
 import sys
 import time
@@ -47,11 +47,14 @@ def test_reference_walk_is_timed_through_its_own_function():
     assert visits > 200 and 0.4 < dt < 5 and rate == pytest.approx(visits / dt)
 
 
-def test_traffic_lookup_matches_only_the_captured_configuration():
-    bench._RUN.update(reps=10, world=1)
-    assert bench.traffic_lookup("cbow_rows_fwdbwd", "syn10k") == 67148544
-    assert bench.traffic_lookup("cbow_rows_fwdbwd", "syn10k", need_reps=3) is None
-    assert bench.traffic_lookup("cbow_slab_step", "stress200k", need_reps=2) == 27482516000
-    bench._RUN.update(world=2)
-    assert bench.traffic_lookup("cbow_rows_fwdbwd", "syn10k") is None          # captures are single-GPU
-    bench._RUN.update(world=1)
+def test_dump_outputs_writes_exact_float_arrays_and_a_fixed_sample(tmp_path):
+    ids = bench.dump_sample(100_000, 4096)
+    assert len(ids) == 4096 and (np.diff(ids) > 0).all() and (ids == bench.dump_sample(100_000, 4096)).all()
+    assert (bench.dump_sample(10, 4096) == np.arange(10)).all()
+    rows = np.arange(2**31 - 64, 2**31 - 1, dtype=np.int32).reshape(3, 21)
+    bench.dump_outputs(str(tmp_path / "out"), {"rows": rows, "w": np.linspace(0, 1, 7, dtype=np.float64)})
+    got = np.load(tmp_path / "out" / "rows.npy")
+    assert got.dtype == np.float64 and (got == rows).all()
+    assert np.load(tmp_path / "out" / "w.npy").dtype == np.float32
+    with pytest.raises(AssertionError):
+        bench.dump_outputs(str(tmp_path / "big"), {"x": np.zeros((65 << 20) // 4, np.float32)})

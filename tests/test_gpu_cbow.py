@@ -339,7 +339,7 @@ def test_minibatch_variant_and_dense_adapter(g2v):
 @pytest.mark.parametrize("D", [128, 256, 512])
 def test_tma_staged_variants_equal_oracle(g2v, monkeypatch, gather, scatter, D):
     """The TMA-staged forms of the fused kernel (bulk-copy gather through shared memory, bulk-reduce
-    scatter) compute the same step; which one ships is decided by measurement (profiles/README.md)."""
+    scatter) compute the same step; which one ships is decided by measurement."""
     monkeypatch.setenv("G2V_CBOW_GATHER", gather)
     monkeypatch.setenv("G2V_CBOW_SCATTER", scatter)
     V, N = 400, 2500
@@ -545,7 +545,7 @@ def test_slab_setup_rejects_unsorted_windows(g2v, monkeypatch):
 
 
 def test_slab_plan_at_the_stress_table_size_equals_the_single_pass_kernel(g2v, monkeypatch):
-    """BASELINE configs[4]'s table (200k genes x 512 = 410 MB, 3x the L2): g2v_cbow_slab_plan must choose gene slabs on
+    """BASELINE configs[4]'s table (200k genes x 512 = 410 MB, 8x H100's L2): g2v_cbow_slab_plan must choose gene slabs on
     its own, and one step over 40k synthetic windows of 80 distinct genes must give the single-pass kernel's gradient,
     loss and accuracy counts (same sums, different float32 order), and the same accuracy pass."""
     import torch
