@@ -29,6 +29,8 @@ SIGNATURES = {
     "g2v_walk_host": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i64, _i32, _u64, _u32, _i64, _i64, _i64, _vp, _vp]),
     "g2v_cbow_fwdbwd": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp,
                                        _i32, _i32, _i32, _vp]),
+    "g2v_cbow_fwdbwd_csc": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                           _vp, _i32, _i32, _i32, _vp]),
     "g2v_cbow_update": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _f32,
                                        _f32, _f32, _i32, _vp, _vp]),
     "g2v_cbow_update_nvl": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f32, _f32, _f32,

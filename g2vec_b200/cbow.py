@@ -132,11 +132,10 @@ class CbowModel:
                                                      self.V, self.D, self._stream()), "g2v_cbow_r1_prepare")
 
     def prepare_csc(self, win):
-        """rank1 only: transpose the incidence of the window list ``win`` (int32 device tensor) once, so that
-        fwdbwd(win, ...) over the WHOLE list forms c without atomics (deterministic, and faster when few
-        genes receive many windows).  The windows are static across steps (full batch), so this is setup."""
-        if self.algo != "rank1":
-            return
+        """Transpose the incidence of the window list ``win`` (int32 device tensor) once, so that fwdbwd(win, ...)
+        over the WHOLE list reduces dO per gene without floating-point atomics: rank1 forms c deterministically,
+        rows writes each gradient row once (g2v_cbow_fwdbwd_csc) instead of red.adding a row per (window, gene).
+        The windows are static across steps (full batch), so this is setup."""
         w = win.to(torch.int64)
         starts = self.rowptr[w].to(torch.int64)
         lens = self.rowptr[w + 1].to(torch.int64) - starts
@@ -196,13 +195,20 @@ class CbowModel:
     def _ptr(t):
         return 0 if t is None else t.data_ptr()
 
+    def _csc_for(self, win, win_begin, n):
+        """The transposed incidence prepare_csc() built for exactly this list, else None."""
+        csc = getattr(self, "_csc", None)
+        if csc is not None and win is not None and csc[0] == win.data_ptr() and win_begin == 0 and n == csc[1]:
+            return csc
+        return None
+
     def fwdbwd(self, win, n_total, win_begin=0, n_win=None):
         """Accumulate the gradient of the listed windows into g_ih / g_ho (loss sum -> acc[0],
         pre-update correct count -> acc[1])."""
         n = (win.shape[0] - win_begin) if n_win is None else n_win
+        csc = self._csc_for(win, win_begin, n)
         if self.algo == "rank1":
-            csc = getattr(self, "_csc", None)
-            if csc is not None and win is not None and csc[0] == win.data_ptr() and win_begin == 0 and n == csc[1]:
+            if csc is not None:
                 rc = self.lib.g2v_cbow_r1_windows_csc(self.rowptr.data_ptr(), self.gene.data_ptr(),
                                                       self.label.data_ptr(), win.data_ptr(), int(n),
                                                       1.0 / float(n_total), self.s.data_ptr(), csc[2].data_ptr(),
@@ -225,6 +231,15 @@ class CbowModel:
                                                 self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D,
                                                 self.reduce, self._n_slabs, ws.data_ptr(), self._stream())
             _capi.check(rc, "g2v_cbow_fwdbwd_slabs")
+            return
+        if csc is not None:
+            rc = self.lib.g2v_cbow_fwdbwd_csc(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+                                              win.data_ptr(), int(n), 1.0 / float(n_total), self.W_ih.data_ptr(),
+                                              self.W_ho.data_ptr(), csc[2].data_ptr(), csc[3].data_ptr(),
+                                              csc[4].data_ptr(), self.g_ih.data_ptr(), self.g_ho.data_ptr(),
+                                              self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D,
+                                              self.reduce, self._stream())
+            _capi.check(rc, "g2v_cbow_fwdbwd_csc")
             return
         rc = self.lib.g2v_cbow_fwdbwd(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
                                       self._ptr(win), int(win_begin), int(n), 1.0 / float(n_total),
@@ -413,11 +428,12 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     tr_d = torch.from_numpy(np.ascontiguousarray(tr_loc, dtype=np.int32)).to(dev)
     va_d = torch.from_numpy(np.ascontiguousarray(va_loc, dtype=np.int32)).to(dev)
 
-    if algo == "rank1" and (batch <= 0 or batch >= n_tr) and len(tr_loc):
-        model.prepare_csc(tr_d)
+    slabs = False
     if algo == "rows" and full_batch:            # tables larger than the L2: gene-slab passes over the static lists
-        model.prepare_slabs(tr_d)
+        slabs = model.prepare_slabs(tr_d)
         model.prepare_slabs(va_d)
+    if full_batch and len(tr_loc) and not slabs:  # per-gene dO sums over the static training list (no scatter)
+        model.prepare_csc(tr_d)
     if log:
         log("     Start training the modified CBOW with early stopping")
     if max_epoch <= 0:                           # no optimizer step at all: the initial vectors

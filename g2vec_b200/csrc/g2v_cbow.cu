@@ -13,13 +13,22 @@
 //     grad     dO  = (sigmoid(o) - y) / N                 (N known up front: no global barrier)
 //     scatter  g_ih[g, :] += dO * W_ho  for g in window   (red.global.add.v4.f32, 16 B per lane)
 //              g_ho       += h * dO                       (registers -> smem -> one atomic per CTA)
-//   cbow_update_kernel                    dense epilogue over [V*D] (+[D]): TF1 Adam or SGD,
+//   cbow_rows_kernel<VEC, true, false, false, CSC=true>   the same up to dO; then, instead of the scatter,
+//                                         dO_pos[i] = dO * scale  at the window's list position i (4 B per window)
+//   cbow_csc_expand_kernel                one warp per gene: c = sum of dO_pos over the gene's segment of the list's
+//                                         transposed incidence (CSC), then g_ih[g, :] += c * W_ho, one plain
+//                                         read-modify-write per touched row.  Exact because the model is linear:
+//                                         every window adds the same row W_ho to its genes, only the scale differs.
+//                                         This is the backward of a prepared full list (g2v_cbow_fwdbwd_csc): it
+//                                         replaces l*D*4 bytes of L2 atomics per window by 8 bytes per incidence.
+//   cbow_update_kernel                   dense epilogue over [V*D] (+[D]): TF1 Adam or SGD,
 //                                         float4, zeroes the gradient for the next step
 //   adam_tick_kernel                      TF1's beta1_power / beta2_power / alpha_t kept on the device so
 //                                         that a whole step can be replayed as one CUDA graph
 //
 // No tensor cores: the 128..512-wide reduction is a memory-bound gather/scatter, not a dense
-// contraction.  Algorithmic bytes per window: l*(8D+4)+5 (DESIGN.md), per step + 32*V*D (Adam).
+// contraction.  Algorithmic bytes per window: l*(8D+4)+5 with the scatter, l*(4D+12)+9 with the CSC backward
+// (+ 8*D per touched gene row) (DESIGN.md), per step + 32*V*D (Adam).
 #include <stdlib.h>
 
 #include "g2v_cbow_common.cuh"
@@ -36,14 +45,17 @@ constexpr bool kDefaultScatterTma = false;   // G2V_CBOW_SCATTER=tma selects the
 // GATHER_TMA: embedding rows are staged through shared memory with TMA bulk copies
 // (cp.async.bulk.shared::cluster.global + mbarrier complete_tx, SASS UBLKCP), 2 stages of 2 KB per warp,
 // one lane issuing one row; the lanes then sum the rows with LDS.128 instead of LDG.128.
-template <int VEC, bool BACKWARD, bool SCATTER_TMA, bool GATHER_TMA>
+// CSC: the backward stops at dO -- it stores dO*scale at the window's list position i (dO_pos[i]) instead of
+// scattering rows into g_ih; cbow_csc_expand_kernel then sums those scalars per gene and writes each gene row once.
+template <int VEC, bool BACKWARD, bool SCATTER_TMA, bool GATHER_TMA, bool CSC = false>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
                  const uint8_t *__restrict__ label, const int32_t *__restrict__ win,
                  int64_t win_begin, int64_t n_win, float inv_n, const float *__restrict__ W_ih,
                  const float *__restrict__ W_ho, float *__restrict__ g_ih, float *__restrict__ g_ho,
                  double *__restrict__ loss_sum, unsigned long long *__restrict__ n_correct,
-                 int32_t reduce_mean, const int32_t *__restrict__ skip) {
+                 int32_t reduce_mean, const int32_t *__restrict__ skip, float *__restrict__ dO_pos) {
+    static_assert(!CSC || (BACKWARD && !SCATTER_TMA), "the CSC backward replaces the scatter");
     G2V_SKIP_IF_STOPPED(skip);
     constexpr int D = 128 * VEC;
     constexpr int D4 = D / 4;
@@ -172,7 +184,14 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
             correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
             if (BACKWARD) loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
         }
-        if (BACKWARD) {
+        if (CSC) {
+            const float dO = (sigmoid_stable(o) - y) * inv_n;
+#pragma unroll
+            for (int v = 0; v < VEC; ++v) {
+                gho[v].x += h[v].x * dO; gho[v].y += h[v].y * dO; gho[v].z += h[v].z * dO; gho[v].w += h[v].w * dO;
+            }
+            if (lane == 0) dO_pos[i] = dO * scale;
+        } else if (BACKWARD) {
             const float dO = (sigmoid_stable(o) - y) * inv_n;
             float4 gv[VEC];
 #pragma unroll
@@ -237,6 +256,7 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
 }
 
 // Any D (not a multiple of 128): h and the g_ho partial live in shared memory per warp.
+// dO_pos != NULL: the CSC backward of cbow_rows_kernel (dO*scale stored per list position, no scatter).
 template <bool BACKWARD>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 cbow_rows_generic_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
@@ -245,7 +265,7 @@ cbow_rows_generic_kernel(const int32_t *__restrict__ rowptr, const int32_t *__re
                          const float *__restrict__ W_ho, float *__restrict__ g_ih,
                          float *__restrict__ g_ho, double *__restrict__ loss_sum,
                          unsigned long long *__restrict__ n_correct, int32_t D, int32_t reduce_mean,
-                         const int32_t *__restrict__ skip) {
+                         const int32_t *__restrict__ skip, float *__restrict__ dO_pos) {
     G2V_SKIP_IF_STOPPED(skip);
     extern __shared__ float shf[];
     __shared__ CtaAcc sh_acc;
@@ -282,6 +302,10 @@ cbow_rows_generic_kernel(const int32_t *__restrict__ rowptr, const int32_t *__re
             const float dO = (sigmoid_stable(o) - y) * inv_n;
             for (int d = lane; d < D; d += 32) gho[d] += h[d] * dO;
             const float s = dO * scale;
+            if (dO_pos) {
+                if (lane == 0) dO_pos[i] = s;
+                continue;
+            }
             for (int32_t j = b; j < e; ++j) {
                 float *dst = g_ih + (size_t)__ldg(gene + j) * D;
                 for (int d = lane; d < D; d += 32) atomicAdd(dst + d, __ldg(W_ho + d) * s);
@@ -297,6 +321,37 @@ cbow_rows_generic_kernel(const int32_t *__restrict__ rowptr, const int32_t *__re
     if (threadIdx.x == 0) {
         if (BACKWARD && loss_sum) atomicAdd(loss_sum, sh_acc.loss);
         if (n_correct) atomicAdd(n_correct, sh_acc.correct);
+    }
+}
+
+// Second half of the CSC backward.  The model is linear, so every window adds the same row W_ho to its genes,
+// scaled by its dO*scale:  g_ih[g,:] += c[g] * W_ho  with  c[g] = sum of dO_pos over the list positions of the
+// windows that contain g (the gene's CSC segment).  One warp per gene owns the row: a coalesced read-modify-write,
+// no atomics.  Genes in no listed window are not touched.
+__global__ void __launch_bounds__(kCbowWarps * 32)
+cbow_csc_expand_kernel(const int32_t *__restrict__ cscptr, const int32_t *__restrict__ csc_pos,
+                       const float *__restrict__ dO_pos, const float *__restrict__ W_ho, float *__restrict__ g_ih,
+                       int32_t V, int32_t D, const int32_t *__restrict__ skip) {
+    G2V_SKIP_IF_STOPPED(skip);
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = (int64_t)blockIdx.x * kCbowWarps + (threadIdx.x >> 5);
+    const int64_t nwarps = (int64_t)gridDim.x * kCbowWarps;
+    for (int64_t g = warp; g < V; g += nwarps) {
+        const int32_t b = __ldg(cscptr + g), e = __ldg(cscptr + g + 1);
+        if (b == e) continue;
+        const float c = csc_segment_sum(csc_pos, dO_pos, b, e, lane);
+        float *row = g_ih + (size_t)g * D;
+        if ((D & 3) == 0) {
+            float4 *r4 = reinterpret_cast<float4 *>(row);
+            for (int k = lane; k < (D >> 2); k += 32) {
+                const float4 w = ldg4(reinterpret_cast<const float4 *>(W_ho) + k);
+                float4 a = r4[k];
+                a.x += c * w.x; a.y += c * w.y; a.z += c * w.z; a.w += c * w.w;
+                r4[k] = a;
+            }
+        } else {
+            for (int d = lane; d < D; d += 32) row[d] += c * __ldg(W_ho + d);
+        }
     }
 }
 
@@ -456,11 +511,12 @@ int rows_grid(const void *kernel, size_t smem, int64_t n_win, int *grid_out) {
     return 0;
 }
 
+// dO_pos != NULL (backward only): the CSC backward -- dO*scale per list position instead of the scatter into g_ih
 template <bool BACKWARD>
 static int launch_rows(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
                        int64_t win_begin, int64_t n_win, float inv_n, const float *W_ih, const float *W_ho,
                        float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t D,
-                       int32_t reduce, cudaStream_t st) {
+                       int32_t reduce, cudaStream_t st, float *dO_pos = nullptr) {
     unsigned long long *nc = reinterpret_cast<unsigned long long *>(n_correct);
     int grid = 0, rc;
     // scatter path of the backward kernel: "red" (red.global.add.v4.f32 per lane) or "tma"
@@ -475,9 +531,10 @@ static int launch_rows(const int32_t *rowptr, const int32_t *gene, const uint8_t
                                 : cbow_rows_kernel<VEC, BACKWARD, BACKWARD, false>)                  \
                         : (gtma ? cbow_rows_kernel<VEC, BACKWARD, false, true>                       \
                                 : cbow_rows_kernel<VEC, BACKWARD, false, false>);                    \
+        if (dO_pos) kern = cbow_rows_kernel<VEC, BACKWARD, false, false, BACKWARD>;                  \
         if ((rc = rows_grid((const void *)kern, 0, n_win, &grid))) return rc;                        \
-        kern<<<grid, kCbowWarps * 32, 0, st>>>(                                                      \
-            rowptr, gene, label, win, win_begin, n_win, inv_n, W_ih, W_ho, g_ih, g_ho, loss_sum, nc, reduce, loop_skip_flag()); \
+        kern<<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, win_begin, n_win, inv_n, W_ih, W_ho, g_ih, \
+                                               g_ho, loss_sum, nc, reduce, loop_skip_flag(), dO_pos); \
     }
     if (D == 128) G2V_LAUNCH_VEC(1)
     else if (D == 256) G2V_LAUNCH_VEC(2)
@@ -490,7 +547,8 @@ static int launch_rows(const int32_t *rowptr, const int32_t *gene, const uint8_t
         G2V_CUDA_OK(cudaFuncSetAttribute(cbow_rows_generic_kernel<BACKWARD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         if ((rc = rows_grid((const void *)cbow_rows_generic_kernel<BACKWARD>, smem, n_win, &grid))) return rc;
         cbow_rows_generic_kernel<BACKWARD><<<grid, kCbowWarps * 32, smem, st>>>(
-            rowptr, gene, label, win, win_begin, n_win, inv_n, W_ih, W_ho, g_ih, g_ho, loss_sum, nc, D, reduce, loop_skip_flag());
+            rowptr, gene, label, win, win_begin, n_win, inv_n, W_ih, W_ho, g_ih, g_ho, loss_sum, nc, D, reduce, loop_skip_flag(),
+            dO_pos);
     }
 #undef G2V_LAUNCH_VEC
     G2V_CUDA_OK(cudaGetLastError());
@@ -625,6 +683,27 @@ extern "C" int g2v_cbow_fwdbwd(const int32_t *rowptr, const int32_t *gene, const
     if (n_win == 0) return 0;
     return launch_rows<true>(rowptr, gene, label, win, win_begin, n_win, inv_n_total, W_ih, W_ho, g_ih, g_ho,
                              loss_sum, n_correct, D, reduce, (cudaStream_t)stream);
+}
+
+extern "C" int g2v_cbow_fwdbwd_csc(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                   const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                                   const float *W_ho, const int32_t *cscptr, const int32_t *csc_pos, float *dO,
+                                   float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
+                                   int32_t D, int32_t reduce, void *stream) {
+    G2V_REQUIRE(V > 0 && D > 0 && n_win >= 0, "g2v_cbow_fwdbwd_csc: bad sizes (V=%d D=%d n_win=%lld)", V, D, (long long)n_win);
+    G2V_REQUIRE(rowptr && label && W_ih && W_ho && cscptr && dO && g_ih && g_ho, "g2v_cbow_fwdbwd_csc: null pointer");
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "g2v_cbow_fwdbwd_csc: unknown reduce %d", reduce);
+    if (n_win == 0) return 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = launch_rows<true>(rowptr, gene, label, win, 0, n_win, inv_n_total, W_ih, W_ho, g_ih, g_ho, loss_sum,
+                               n_correct, D, reduce, st, dO);
+    if (rc) return rc;
+    int grid = 0;
+    if ((rc = rows_grid((const void *)cbow_csc_expand_kernel, 0, V, &grid))) return rc;
+    cbow_csc_expand_kernel<<<grid, kCbowWarps * 32, 0, st>>>(cscptr, csc_pos, dO, W_ho, g_ih, V, D, loop_skip_flag());
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
 }
 
 extern "C" int g2v_cbow_eval(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,

@@ -140,14 +140,7 @@ r1_csc_reduce_kernel(const int32_t *__restrict__ cscptr, const int32_t *__restri
     for (int64_t g = warp; g < V; g += nwarps) {
         const int32_t b = __ldg(cscptr + g), e = __ldg(cscptr + g + 1);
         if (b == e) continue;
-        float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-        int32_t j = b + lane;
-        for (; j + 96 < e; j += 128) {
-            a0 += __ldg(dO + __ldg(csc_pos + j));      a1 += __ldg(dO + __ldg(csc_pos + j + 32));
-            a2 += __ldg(dO + __ldg(csc_pos + j + 64)); a3 += __ldg(dO + __ldg(csc_pos + j + 96));
-        }
-        for (; j < e; j += 32) a0 += __ldg(dO + __ldg(csc_pos + j));
-        const float tot = warp_sum((a0 + a1) + (a2 + a3));
+        const float tot = csc_segment_sum(csc_pos, dO, b, e, lane);
         if (lane == 0) c[g] += tot;
     }
 }

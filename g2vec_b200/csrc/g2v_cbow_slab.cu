@@ -319,9 +319,12 @@ extern "C" int g2v_cbow_slab_plan(int32_t V, int32_t D, int32_t *n_slabs) {
     *n_slabs = 1;
     if (D != 128 && D != 256 && D != 512) return 0;               // the generic-D kernel has no slab form
     const double table = (double)V * D * 4.0;
-    // table + gradient resident together: the fused single-pass kernel is already L2-bound.  Measured on H100 (50 MB
-    // L2, fwd+bwd): 20k x 256 (2 x 20.5 MB) 9.8 ms single pass vs 11.6 ms in 2 slabs; 50k x 128 (2 x 25.6 MB) 16.2 ms
-    // vs 14.2 ms -- the threshold lies between the two
+    // table resident: the single pass is L2-bound.  With the CSC backward of a prepared training list
+    // (g2v_cbow_fwdbwd_csc) only the table has to stay in the L2 while the windows are gathered -- each gradient row is
+    // read and written once afterwards -- so the rule is on the table alone.  Measured on H100 SXM (700 W, 50 MB L2,
+    // fwd+bwd of bench.py's training lists): 20k x 256 (20.5 MB) 3.57 ms single pass + CSC vs 11.6 ms in 2 slabs;
+    // 50k x 128 (25.6 MB) 9.4 ms single pass + CSC vs 28.3 ms in 2 slabs; at 400 W, 20k x 512 (41 MB, 160k synthetic
+    // windows of 80 genes) 3.54 ms vs 11.6 ms in 4 slabs
     // one BACKWARD slab of g_ih is a quarter of the L2, so that a forward group (G2V_CBOW_SLAB_FWD_GROUP = 2 slabs of
     // W_ih) stays resident with room for the streamed window data: 12.5 MiB on H100 (measured on the 200k x 512 table:
     // 55.8 ms per fwd+bwd in 32 slabs, 56.6 ms in 13 slabs of 32 MiB, 55.1 ms in 25 of 16 MiB)
@@ -329,7 +332,7 @@ extern "C" int g2v_cbow_slab_plan(int32_t V, int32_t D, int32_t *n_slabs) {
     const double slab = e && atof(e) > 0 ? atof(e) * 1048576.0 : 0.25 * (double)dp.l2_bytes;
     const char *f = getenv("G2V_CBOW_SLABS");                     // force a slab count (tests)
     if (f && atoi(f) >= 1) { *n_slabs = atoi(f) > V ? V : atoi(f); return 0; }
-    if (2.0 * table <= 0.9 * (double)dp.l2_bytes) return 0;
+    if (table <= 0.9 * (double)dp.l2_bytes) return 0;
     int s = (int)((table + slab - 1) / slab);
     if (s < 2) s = 2;
     if (s > 64) s = 64;

@@ -115,4 +115,20 @@ __device__ __forceinline__ uint32_t warp_inclusive_scan_u32(uint32_t v, int lane
     return v;
 }
 
+// Segmented sum over the transposed incidence of a window list (CSC over list positions): the sum of
+// vals[pos[j]] for j in [b, e), returned in every lane.  Fixed lane assignment and shuffle tree, so the result
+// is the same bits from run to run (no floating-point atomics).  Used by the CBOW backward passes that reduce a
+// per-window scalar dO into a per-gene coefficient (g2v_cbow.cu, g2v_cbow_rank1.cu).
+__device__ __forceinline__ float csc_segment_sum(const int32_t *__restrict__ pos, const float *__restrict__ vals,
+                                                 int32_t b, int32_t e, int lane) {
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+    int32_t j = b + lane;
+    for (; j + 96 < e; j += 128) {
+        a0 += __ldg(vals + __ldg(pos + j));      a1 += __ldg(vals + __ldg(pos + j + 32));
+        a2 += __ldg(vals + __ldg(pos + j + 64)); a3 += __ldg(vals + __ldg(pos + j + 96));
+    }
+    for (; j < e; j += 32) a0 += __ldg(vals + __ldg(pos + j));
+    return warp_sum((a0 + a1) + (a2 + a3));
+}
+
 }  // namespace g2v

@@ -122,6 +122,19 @@ int g2v_cbow_fwdbwd(const int32_t *rowptr, const int32_t *gene, const uint8_t *l
                     double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce,
                     void *stream);
 
+/* g2v_cbow_fwdbwd_csc: the same step as g2v_cbow_fwdbwd over the WHOLE list win[0..n_win-1], with the list's
+ * windows x genes incidence also given transposed (CSC over list positions: cscptr [V+1], csc_pos [nnz] =
+ * positions i of the windows that contain the gene, as for g2v_cbow_r1_windows_csc).  The forward stores
+ * dO*scale per list position in the scratch dO [n_win]; a second kernel then adds c[g]*W_ho into g_ih[g,:] once
+ * per gene, c[g] = sum of dO over the gene's positions in a fixed order -- no floating-point atomics on g_ih.
+ * Same accumulation semantics as g2v_cbow_fwdbwd (g_ih, g_ho, loss_sum, n_correct are added into); rows of
+ * genes in no listed window are not touched. */
+int g2v_cbow_fwdbwd_csc(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                        const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                        const float *W_ho, const int32_t *cscptr, const int32_t *csc_pos, float *dO,
+                        float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
+                        int32_t D, int32_t reduce, void *stream);
+
 int g2v_cbow_update(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m_ho, float *v_ho,
                     float *g_ih, float *g_ho, int32_t V, int32_t D, int32_t optimizer, float lr,
                     float beta1, float beta2, float eps, int32_t t, const float *alpha_dev, void *stream);
@@ -181,8 +194,8 @@ int g2v_cbow_loop_counters_nvl(const int64_t *ctl, const int64_t *acc, int64_t *
  * g2v_cbow_eval, processed gene slab by gene slab so that the gathered rows and the gradient rows stay
  * L2-resident.  Needs windows whose gene lists are strictly ascending (tuple(sorted(path)), G2Vec.py:345).
  *
- * g2v_cbow_slab_plan: number of slabs for a [V, D] table on the current device (1 = table + gradient fit
- *   the L2 together, or D is not 128/256/512: use g2v_cbow_fwdbwd).
+ * g2v_cbow_slab_plan: number of slabs for a [V, D] table on the current device (1 = the table fits the L2,
+ *   or D is not 128/256/512: use g2v_cbow_fwdbwd_csc / g2v_cbow_fwdbwd).
  * g2v_cbow_slab_workspace_bytes / g2v_cbow_slab_setup: per window list (win/win_begin/n_win as in
  *   g2v_cbow_fwdbwd; the list is static across steps, G2Vec.py:262-264), records where each window's sorted gene
  *   list crosses the slab boundaries.  Synchronises the stream once; fails on an unsorted window.
