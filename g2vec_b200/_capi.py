@@ -31,6 +31,10 @@ SIGNATURES = {
                                        _i32, _i32, _i32, _vp]),
     "g2v_cbow_fwdbwd_csc": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                            _vp, _i32, _i32, _i32, _vp]),
+    "g2v_cbow_fwd_do": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32,
+                                       _vp]),
+    "g2v_cbow_lazy_adam": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32,
+                                          _f32, _f32, _f32, _i32, _vp, _vp]),
     "g2v_cbow_update": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _f32,
                                        _f32, _f32, _i32, _vp, _vp]),
     "g2v_cbow_update_nvl": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f32, _f32, _f32,

@@ -74,6 +74,11 @@ class CbowModel:
                 return a.to(device=dev, dtype=dt).contiguous()
             return torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=dt)
 
+        if optimizer == "lazy_adam" and algo != "rows":
+            raise ValueError("optimizer='lazy_adam' needs algo='rows': rank1 keeps s = W_ih.W_ho, which every W_ho step "
+                             "changes for every gene")
+        if optimizer == "lazy_adam" and nvl_group is not None:
+            raise ValueError("optimizer='lazy_adam' runs on one GPU only")
         self.rowptr = to(rowptr, torch.int32)
         self.gene = to(gene, torch.int32)
         self.label = to(label, torch.uint8)
@@ -83,6 +88,10 @@ class CbowModel:
         # group (multi-GPU) the parameters and the gradient live in symmetric memory (peer-mapped, NVLS multicast if
         # the fabric has it) and the optimizer step does the gradient exchange itself (g2v_cbow_update_nvl).
         self.nvl = None
+        # lazy_adam: TF1 LazyAdam -- only the rows a batch gathered are updated, fused with their per-gene dO sums
+        # (g2v_cbow_fwd_do + g2v_cbow_lazy_adam over the batches of prepare_batches); no g_ih is allocated
+        self.lazy = optimizer == "lazy_adam"
+        self._batches, self._pending, self._dO = {}, None, None
         if algo == "rows" and nvl_group is not None:
             self.nvl = _nvl_setup(nvl_group, n_flat, dev)
         if algo == "rows":
@@ -94,14 +103,18 @@ class CbowModel:
         else:
             self.W_ih = to(W_ih0, torch.float32).reshape(self.V, self.D).clone()
             self.W_ho = to(W_ho0, torch.float32).reshape(self.D).clone()
-        self.opt = {"adam": _capi.OPT_ADAM_TF1, "sgd": _capi.OPT_SGD}[optimizer]
+        self.opt = {"adam": _capi.OPT_ADAM_TF1, "sgd": _capi.OPT_SGD, "lazy_adam": _capi.OPT_ADAM_TF1}[optimizer]
         self.reduce = {"sum": _capi.REDUCE_SUM, "mean": _capi.REDUCE_MEAN}[reduce]
         self.lr, self.beta1, self.beta2, self.eps = float(lr), float(beta1), float(beta2), float(eps)
         z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
         if algo not in ("rows", "rank1"):
             raise ValueError("algo must be 'rows' (gather/scatter of embedding rows) or 'rank1' (collapsed)")
         self.algo = algo
-        if algo == "rows":
+        if self.lazy:
+            self.g_ih, self.g_ho = None, z(self.D)
+            self.g_flat = self.g_ho
+            self.s = self.c = None
+        elif algo == "rows":
             # one allocation [g_ih | g_ho]: a multi-GPU step all-reduces the whole gradient with ONE collective
             self.g_flat = self.nvl["g"].zero_() if self.nvl else z(n_flat)
             self.g_ih = self.g_flat[:self.V * self.D].view(self.V, self.D)
@@ -149,6 +162,44 @@ class CbowModel:
         cscptr[1:] = torch.cumsum(torch.bincount(g, minlength=self.V), 0)
         self._csc = (win.data_ptr(), int(w.shape[0]), cscptr.to(torch.int32), pos[order].to(torch.int32),
                      torch.empty(w.shape[0], dtype=torch.float32, device=self.device))
+
+    def prepare_batches(self, win, batch):
+        """lazy_adam: cut the window list ``win`` (int32 device tensor) into consecutive batches of ``batch`` windows
+        (the last one shorter) and record, once, for every batch the ascending genes it gathers, their segment
+        pointers and their positions relative to the batch start -- the transposed incidence of each batch, O(nnz +
+        sum of touched genes) in all.  fwdbwd(win, n, win_begin=lo, n_win=nb) then finds batch [lo, lo + nb)."""
+        n = int(win.shape[0])
+        B = min(int(batch), n) if batch > 0 else n
+        if n == 0:
+            return
+        w = win.to(torch.int64)
+        starts = self.rowptr[w].to(torch.int64)
+        lens = self.rowptr[w + 1].to(torch.int64) - starts
+        total = int(lens.sum())
+        pos = torch.repeat_interleave(torch.arange(n, device=self.device), lens)
+        first = torch.cumsum(lens, 0) - lens
+        idx = starts[pos] + (torch.arange(total, device=self.device) - first[pos])
+        b = pos // B
+        key, order = torch.sort(b * self.V + self.gene[idx].to(torch.int64), stable=True)   # (batch, gene, position)
+        rel = (pos - b * B)[order].to(torch.int32)
+        head = torch.ones(total, dtype=torch.bool, device=self.device)
+        head[1:] = key[1:] != key[:-1]
+        seg = torch.nonzero(head).squeeze(1)
+        rows = (key[seg] % self.V).to(torch.int32)
+        segptr = torch.cat([seg, torch.tensor([total], device=self.device)]).to(torch.int32)
+        n_b = -(-n // B)
+        per = torch.bincount(key[seg] // self.V, minlength=n_b).cpu().numpy()
+        r0 = np.concatenate([[0], np.cumsum(per)[:-1]])
+        data = (win, rows, segptr, rel)                     # keeps `win` alive: its address is part of the key
+        for k in range(n_b):
+            self._batches[(win.data_ptr(), k * B, min(B, n - k * B))] = (data, int(r0[k]), int(per[k]))
+        if self._dO is None or self._dO.shape[0] < B:
+            self._dO = torch.empty(B, dtype=torch.float32, device=self.device)
+        self._pending = None
+
+    def batch_touched(self, win, win_begin, n):
+        """Number of distinct genes of batch [win_begin, win_begin + n) of a list given to prepare_batches."""
+        return self._batches[(self._ptr(win), int(win_begin), int(n))][2]
 
     def prepare_slabs(self, win, win_begin=0, n_win=None):
         """rows only, tables larger than the L2 (csrc/g2v_cbow_slab.cu): record once, for the static window list
@@ -206,6 +257,9 @@ class CbowModel:
         """Accumulate the gradient of the listed windows into g_ih / g_ho (loss sum -> acc[0],
         pre-update correct count -> acc[1])."""
         n = (win.shape[0] - win_begin) if n_win is None else n_win
+        if self.lazy:
+            self._fwd_do(win, n_total, win_begin, n)
+            return
         csc = self._csc_for(win, win_begin, n)
         if self.algo == "rank1":
             if csc is not None:
@@ -248,6 +302,35 @@ class CbowModel:
                                       self.V, self.D, self.reduce, self._stream())
         _capi.check(rc, "g2v_cbow_fwdbwd")
 
+    def _fwd_do(self, win, n_total, win_begin, n):
+        """lazy_adam's forward: dO*scale per position of a batch prepared by prepare_batches (loss, accuracy and g_ho
+        as fwdbwd); update() then applies the lazy step to the batch's rows."""
+        plan = self._batches.get((self._ptr(win), int(win_begin), int(n)))
+        if plan is None:
+            raise RuntimeError("optimizer='lazy_adam': windows [%d, %d) of this list were not given to prepare_batches"
+                               % (win_begin, win_begin + n))
+        self._pending = plan
+        if n == 0:
+            return
+        rc = self.lib.g2v_cbow_fwd_do(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+                                      win.data_ptr() + 4 * int(win_begin), int(n), 1.0 / float(n_total),
+                                      self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._dO.data_ptr(),
+                                      self.g_ho.data_ptr(), self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V,
+                                      self.D, self.reduce, self._stream())
+        _capi.check(rc, "g2v_cbow_fwd_do")
+
+    def _lazy_update(self, adev):
+        (_, rows, segptr, pos), r0, n_rows = self._pending or ((None,) * 4, 0, 0)
+        self._pending = None
+        rc = self.lib.g2v_cbow_lazy_adam(rows.data_ptr() + 4 * r0 if n_rows else None,
+                                         segptr.data_ptr() + 4 * r0 if n_rows else None,
+                                         pos.data_ptr() if n_rows else None, self._dO.data_ptr() if n_rows else None,
+                                         n_rows, self.W_ih.data_ptr(), self.m_ih.data_ptr(), self.v_ih.data_ptr(),
+                                         self.W_ho.data_ptr(), self.m_ho.data_ptr(), self.v_ho.data_ptr(),
+                                         self.g_ho.data_ptr(), self.V, self.D, self.lr, self.beta1, self.beta2,
+                                         self.eps, self.t, adev, self._stream())
+        _capi.check(rc, "g2v_cbow_lazy_adam")
+
     def update(self):
         self.t += 1
         adev = 0
@@ -255,6 +338,9 @@ class CbowModel:
             _capi.check(self.lib.g2v_cbow_adam_tick(self.hyper.data_ptr(), self.lr, self.beta1, self.beta2,
                                                     self._stream()), "g2v_cbow_adam_tick")
             adev = self.hyper.data_ptr()
+        if self.lazy:
+            self._lazy_update(adev)
+            return
         if self.algo == "rank1":
             rc = self.lib.g2v_cbow_r1_update(self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._ptr(self.m_ih),
                                              self._ptr(self.v_ih), self._ptr(self.m_ho), self._ptr(self.v_ho),
@@ -407,8 +493,19 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     ``use_graph``: on one GPU with full batch, every step after the first replays a CUDA graph of the step's
     launches (the Adam step size lives on the device, g2v_cbow_adam_tick), so the host only replays, waits
     and applies the early-stop rule.
+
+    ``optimizer``: "adam" (TF1 AdamOptimizer, the reference's), "sgd", or "lazy_adam": TF1 LazyAdam on the
+    embedding-lookup form of the model -- a step updates W_ih / m / v only on the rows of the genes its batch
+    gathered (dense Adam on W_ho).  Full batch it computes what "adam" computes (rows outside the training list
+    keep zero gradient and zero moments); with ``batch`` it is the usual sparse mini-batch embedding update.
+    Only with algo="rows", on one GPU.
     """
     dist = _dist()
+    if optimizer == "lazy_adam" and algo != "rows":
+        raise ValueError("optimizer='lazy_adam' needs algo='rows' (rank1 keeps s = W_ih.W_ho, which every W_ho step "
+                         "changes for every gene)")
+    if optimizer == "lazy_adam" and dist:
+        raise ValueError("optimizer='lazy_adam' runs on one GPU only (world size %d)" % dist.get_world_size())
     world, rank = (dist.get_world_size(), dist.get_rank()) if dist else (1, 0)
     rowptr_np = (win_rowptr.cpu().numpy() if isinstance(win_rowptr, torch.Tensor) else np.asarray(win_rowptr))
     N = rowptr_np.shape[0] - 1
@@ -429,10 +526,12 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     va_d = torch.from_numpy(np.ascontiguousarray(va_loc, dtype=np.int32)).to(dev)
 
     slabs = False
-    if algo == "rows" and full_batch:            # tables larger than the L2: gene-slab passes over the static lists
+    if model.lazy:                               # touched genes of every batch; single-pass forward at every table size
+        model.prepare_batches(tr_d, len(tr_loc) if full_batch else batch)
+    elif algo == "rows" and full_batch:          # tables larger than the L2: gene-slab passes over the static lists
         slabs = model.prepare_slabs(tr_d)
         model.prepare_slabs(va_d)
-    if full_batch and len(tr_loc) and not slabs:  # per-gene dO sums over the static training list (no scatter)
+    if full_batch and len(tr_loc) and not slabs and not model.lazy:   # per-gene dO sums over the static training list
         model.prepare_csc(tr_d)
     if log:
         log("     Start training the modified CBOW with early stopping")

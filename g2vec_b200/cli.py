@@ -32,6 +32,11 @@ def parse_arguments(argv=None):
     p.add_argument('--algo', choices=['rows', 'rank1'], default='rows',
                    help="CBOW kernels: 'rows' = embedding-row gather/scatter (default), 'rank1' = collapsed, "
                         "bit-reproducible trainer; same results to fp32 rounding")
+    p.add_argument('--batch', type=int, default=0,
+                   help="windows per optimizer step; 0 (default) = full batch, one step per epoch as the reference")
+    p.add_argument('--optimizer', choices=['adam', 'sgd', 'lazy_adam'], default='adam',
+                   help="'adam' = TF1 AdamOptimizer (the reference's), 'sgd', or 'lazy_adam' = TF1 LazyAdam: a step "
+                        "updates only the rows of the genes its batch gathered (rows, one GPU)")
     return p.parse_args(argv)
 
 
@@ -227,7 +232,8 @@ def main(argv=None):
 
     print(">>> 4. Compute distributed representations using modified CBOW")
     mat = cbow.train_cbow(w_rowptr, w_gene, w_label, n_genes, args.sizeHiddenlayer, args.learningRate,
-                          max_epoch=args.epoch, seed=args.seed, log=print, algo=args.algo)   # print is silent off rank 0
+                          max_epoch=args.epoch, seed=args.seed, log=print, algo=args.algo,   # print is silent off rank 0
+                          batch=args.batch, optimizer=args.optimizer)
     genes = data['gene']
     if rank != 0:
         dist.barrier()

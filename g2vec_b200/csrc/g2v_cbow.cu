@@ -23,6 +23,9 @@
 //                                         replaces l*D*4 bytes of L2 atomics per window by 8 bytes per incidence.
 //   cbow_update_kernel                   dense epilogue over [V*D] (+[D]): TF1 Adam or SGD,
 //                                         float4, zeroes the gradient for the next step
+//   cbow_lazy_adam_rows_kernel            lazy (touched-row) Adam of a batch: one warp per gene the batch gathered,
+//                                         c = its segmented dO sum, then TF1 Adam on the W/m/v row with g = c * W_ho;
+//                                         g_ih is never materialised (g2v_cbow_fwd_do + g2v_cbow_lazy_adam)
 //   adam_tick_kernel                      TF1's beta1_power / beta2_power / alpha_t kept on the device so
 //                                         that a whole step can be replayed as one CUDA graph
 //
@@ -406,6 +409,47 @@ cbow_update_kernel(float *__restrict__ W, float *__restrict__ M, float *__restri
     }
 }
 
+// ---- lazy (touched-row) Adam over the rows of one batch -------------------------------------
+// TF1 LazyAdam on the embedding-lookup form of the model: only the rows a batch gathered are updated.  The gradient
+// of gene row g is c[g] * W_ho with c[g] = sum of dO*scale over the gene's positions in the batch, so the optimizer
+// step is fused with that per-gene segmented sum and g_ih is never materialised.  One warp per touched gene:
+// rows[r] = the gene, its positions pos[segptr[r] .. segptr[r+1]) index dO (batch-relative list positions).
+// Rows outside the list keep W, m and v bit for bit.  W_ho must be the value before this step: its own update is a
+// second launch (cbow_update_kernel with n = 0).  The gradient is rounded on its own (__fmul_rn, never contracted
+// into Adam's first subtraction), as the stored g_ih of the CSC backward is, so the step is the dense one bit for bit.
+__global__ void __launch_bounds__(kCbowWarps * 32)
+cbow_lazy_adam_rows_kernel(const int32_t *__restrict__ rows, const int32_t *__restrict__ segptr,
+                           const int32_t *__restrict__ pos, const float *__restrict__ dO, int64_t n_rows,
+                           float *__restrict__ W, float *__restrict__ M, float *__restrict__ Vv,
+                           const float *__restrict__ W_ho, int32_t D, float alpha_host, float omb1, float omb2,
+                           float eps, const float *__restrict__ alpha_dev, const int32_t *__restrict__ skip) {
+    G2V_SKIP_IF_STOPPED(skip);
+    const float alpha = alpha_dev ? __ldg(alpha_dev + 2) : alpha_host;
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = (int64_t)blockIdx.x * kCbowWarps + (threadIdx.x >> 5);
+    const int64_t nwarps = (int64_t)gridDim.x * kCbowWarps;
+    for (int64_t r = warp; r < n_rows; r += nwarps) {
+        const size_t off = (size_t)__ldg(rows + r) * D;
+        const float c = csc_segment_sum(pos, dO, __ldg(segptr + r), __ldg(segptr + r + 1), lane);
+        if ((D & 3) == 0) {
+            float4 *w4 = reinterpret_cast<float4 *>(W + off), *m4 = reinterpret_cast<float4 *>(M + off);
+            float4 *v4 = reinterpret_cast<float4 *>(Vv + off);
+            for (int k = lane; k < (D >> 2); k += 32) {
+                const float4 h = ldg4(reinterpret_cast<const float4 *>(W_ho) + k);
+                float4 w = w4[k], m = m4[k], v = v4[k];
+                adam1(w.x, m.x, v.x, __fmul_rn(c, h.x), alpha, omb1, omb2, eps);
+                adam1(w.y, m.y, v.y, __fmul_rn(c, h.y), alpha, omb1, omb2, eps);
+                adam1(w.z, m.z, v.z, __fmul_rn(c, h.z), alpha, omb1, omb2, eps);
+                adam1(w.w, m.w, v.w, __fmul_rn(c, h.w), alpha, omb1, omb2, eps);
+                w4[k] = w; m4[k] = m; v4[k] = v;
+            }
+        } else {
+            for (int d = lane; d < D; d += 32)
+                adam1(W[off + d], M[off + d], Vv[off + d], __fmul_rn(c, __ldg(W_ho + d)), alpha, omb1, omb2, eps);
+        }
+    }
+}
+
 // ---- optimizer epilogue fused with the gradient exchange over NVLink / NVSwitch ---------------------------
 // Multi-GPU form of cbow_update_kernel: instead of ncclAllReduce(gradient) followed by the same dense update on
 // every rank, rank r owns the slice [r*chunk, (r+1)*chunk) of the flat parameter vector [W_ih | W_ho]:
@@ -706,6 +750,18 @@ extern "C" int g2v_cbow_fwdbwd_csc(const int32_t *rowptr, const int32_t *gene, c
     return 0;
 }
 
+extern "C" int g2v_cbow_fwd_do(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                               int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho, float *dO,
+                               float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce,
+                               void *stream) {
+    G2V_REQUIRE(V > 0 && D > 0 && n_win >= 0, "g2v_cbow_fwd_do: bad sizes (V=%d D=%d n_win=%lld)", V, D, (long long)n_win);
+    G2V_REQUIRE(rowptr && label && W_ih && W_ho && dO && g_ho, "g2v_cbow_fwd_do: null pointer");
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "g2v_cbow_fwd_do: unknown reduce %d", reduce);
+    if (n_win == 0) return 0;
+    return launch_rows<true>(rowptr, gene, label, win, 0, n_win, inv_n_total, W_ih, W_ho, nullptr, g_ho, loss_sum,
+                             n_correct, D, reduce, (cudaStream_t)stream, dO);
+}
+
 extern "C" int g2v_cbow_eval(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
                              const int32_t *win, int64_t win_begin, int64_t n_win, const float *W_ih,
                              const float *W_ho, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce,
@@ -764,6 +820,37 @@ extern "C" int g2v_cbow_update(float *W_ih, float *W_ho, float *m_ih, float *v_i
     }
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_lazy_adam(const int32_t *rows, const int32_t *segptr, const int32_t *pos, const float *dO,
+                                  int64_t n_rows, float *W_ih, float *m_ih, float *v_ih, float *W_ho, float *m_ho,
+                                  float *v_ho, float *g_ho, int32_t V, int32_t D, float lr, float beta1, float beta2,
+                                  float eps, int32_t t, const float *alpha_dev, void *stream) {
+    G2V_REQUIRE(V > 0 && D > 0 && n_rows >= 0 && n_rows <= V && (t >= 1 || alpha_dev),
+                "g2v_cbow_lazy_adam: bad sizes (V=%d D=%d n_rows=%lld t=%d)", V, D, (long long)n_rows, t);
+    G2V_REQUIRE(W_ih && m_ih && v_ih && W_ho && m_ho && v_ho && g_ho, "g2v_cbow_lazy_adam: null pointer");
+    G2V_REQUIRE(n_rows == 0 || (rows && segptr && pos && dO), "g2v_cbow_lazy_adam: null row list");
+    cudaStream_t st = (cudaStream_t)stream;
+    float b1p = 1.f, b2p = 1.f;
+    for (int i = 0; i < t; ++i) { b1p *= beta1; b2p *= beta2; }
+    const float alpha = alpha_dev ? 0.f : lr * sqrtf(1.f - b2p) / (1.f - b1p);
+    int rc, launches = 1;
+    if (n_rows > 0) {
+        int grid = 0;
+        if ((rc = rows_grid((const void *)cbow_lazy_adam_rows_kernel, 0, n_rows, &grid))) return rc;
+        cbow_lazy_adam_rows_kernel<<<grid, kCbowWarps * 32, 0, st>>>(rows, segptr, pos, dO, n_rows, W_ih, m_ih, v_ih,
+                                                                     W_ho, D, alpha, 1.f - beta1, 1.f - beta2, eps,
+                                                                     alpha_dev, loop_skip_flag());
+        G2V_CUDA_OK(cudaGetLastError());
+        ++launches;
+    }
+    // W_ho (dense TF1 Adam from g_ho, which it zeroes) after every row has read the pre-step W_ho
+    cbow_update_kernel<G2V_OPT_ADAM_TF1><<<(unsigned)((D + 255) / 256), 256, 0, st>>>(
+        nullptr, nullptr, nullptr, nullptr, 0, W_ho, m_ho, v_ho, g_ho, (int64_t)D, alpha, 1.f - beta1, 1.f - beta2, eps,
+        alpha_dev, loop_skip_flag());
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch(launches);
     return 0;
 }
 

@@ -135,6 +135,25 @@ int g2v_cbow_fwdbwd_csc(const int32_t *rowptr, const int32_t *gene, const uint8_
                         float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
                         int32_t D, int32_t reduce, void *stream);
 
+/* g2v_cbow_fwd_do: the first half of g2v_cbow_fwdbwd_csc over win[0..n_win-1] (win may point into a longer list,
+ * e.g. at the start of a mini-batch): the fused forward stores dO*scale per list position i in dO [n_win] and adds
+ * into g_ho, loss_sum and n_correct as g2v_cbow_fwdbwd does.  Nothing is added into any gradient row. */
+int g2v_cbow_fwd_do(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                    int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho, float *dO, float *g_ho,
+                    double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce, void *stream);
+
+/* g2v_cbow_lazy_adam: lazy (touched-row) TF1 Adam after g2v_cbow_fwd_do, as tf.contrib.opt.LazyAdamOptimizer applies
+ * it to an embedding lookup.  rows [n_rows] = the distinct genes of the batch; the positions of gene rows[r] in the
+ * batch are pos[segptr[r] .. segptr[r+1]) (indices into dO, in the order they are summed).  For each listed gene
+ * W_ih/m_ih/v_ih[g,:] take one TF1 ApplyAdam step with gradient c*W_ho, c = the sum of dO over its positions and W_ho
+ * the value before this call; every other row is left untouched.  Then W_ho/m_ho/v_ho take the dense step from g_ho,
+ * and g_ho is zeroed.  Step size: alpha_dev as in g2v_cbow_update (device beta powers), else from t.  Two launches
+ * (one when n_rows == 0). */
+int g2v_cbow_lazy_adam(const int32_t *rows, const int32_t *segptr, const int32_t *pos, const float *dO,
+                       int64_t n_rows, float *W_ih, float *m_ih, float *v_ih, float *W_ho, float *m_ho, float *v_ho,
+                       float *g_ho, int32_t V, int32_t D, float lr, float beta1, float beta2, float eps, int32_t t,
+                       const float *alpha_dev, void *stream);
+
 int g2v_cbow_update(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m_ho, float *v_ho,
                     float *g_ih, float *g_ho, int32_t V, int32_t D, int32_t optimizer, float lr,
                     float beta1, float beta2, float eps, int32_t t, const float *alpha_dev, void *stream);
