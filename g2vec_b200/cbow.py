@@ -134,8 +134,9 @@ class CbowModel:
             self.m_ih, self.v_ih, self.m_ho, self.v_ho = z(self.V, self.D), z(self.V, self.D), z(self.D), z(self.D)
         else:
             self.m_ih = self.v_ih = self.m_ho = self.v_ho = None
-        # [loss_sum (f64 bits), n_correct_train_fwd, n_correct_val, n_correct_train] as 4 x 8 bytes
-        self.acc = torch.zeros(4, dtype=torch.int64, device=dev)
+        # [loss_sum (f64 bits), n_correct_train_fwd, n_correct_val, n_correct_train] as 4 x 8 bytes, then the carry
+        # slots a DeviceLoop's tail pass fills for the next step: [carried loss_sum (f64 bits), carried n_correct]
+        self.acc = torch.zeros(6, dtype=torch.int64, device=dev)
         self.t = 0
         # Adam's beta1^t / beta2^t / alpha_t live on the device (TF1's beta*_power variables), advanced by
         # g2v_cbow_adam_tick: no launch of a step depends on a host-side value, so a step can be a CUDA graph
@@ -588,11 +589,21 @@ class _LoopLog:
 class DeviceLoop:
     """One model's training loop state on the device (g2v_cbow_loop_*) and the launches of one iteration of the
     reference loop (G2Vec.py:262-267): snapshot + zero counters, fwd+bwd, [all-reduce], optimizer, validation
-    accuracy, [training accuracy], [all-reduce of the counters], decide.  Used by train_cbow and by bench.py."""
+    accuracy, [training accuracy], [all-reduce of the counters], decide.  Used by train_cbow and by bench.py.
+
+    Carried mode (``self.carried``: one GPU, rows, dense optimizer, fwdbwd on the CSC path of the training list):
+    the training-accuracy pass runs on every step as the tail pass (g2v_cbow_loop_tail) and is also the next step's
+    forward, so the next fwdbwd only expands its dO into g_ih.  The training list is gathered once per step instead
+    of twice.  This assumes the training windows do not change between steps: the list is static, and a
+    WindowFeeder re-uploads the same windows every step.  The first step after reset() runs the full forward,
+    decided on the device, so a graph captured right after reset() is correct from its first replay."""
 
     def __init__(self, model, dist, tr_d, va_d, n_tr, max_epoch, early_stop, snapshot=True):
         self.m, self.dist, self.tr_d, self.va_d, self.n_tr = model, dist, tr_d, va_d, n_tr
         self.n_tr_loc, self.n_va_loc = int(tr_d.shape[0]), int(va_d.shape[0])
+        self.carried = (dist is None and model.algo == "rows" and not model.lazy and self.n_tr_loc > 0
+                        and model._slab_ws(tr_d, 0, self.n_tr_loc) is None
+                        and model._csc_for(tr_d, 0, self.n_tr_loc) is not None)
         dev = model.device
         self.ctl = torch.zeros(8, dtype=torch.int64, device=dev)
         n_hist = max(max_epoch, 1) * 4
@@ -623,6 +634,9 @@ class DeviceLoop:
     def reset(self):
         _capi.check(self.m.lib.g2v_cbow_loop_init(self.ctl.data_ptr(), self.max_epoch, int(self.early_stop), self._st()),
                     "g2v_cbow_loop_init")
+        if self.carried:                             # drop a pending carry: its g_ho partial would be added twice
+            self.m.g_ho.zero_()
+            self.m.acc[4:].zero_()
         if self.hist_nvl:
             self.hist_nvl["h"].barrier(channel=2)    # no rank is still adding into the history of the previous loop
             self.hist_d.zero_()
@@ -635,13 +649,15 @@ class DeviceLoop:
         _capi.check(self.m.lib.g2v_cbow_loop_attach(None), "g2v_cbow_loop_attach")
 
     def one(self, show, m_fb=None, m_upd=None, m_val=None):
-        """Enqueue one iteration (the optional events mark the end of fwd+bwd, of the update, of the validation pass)."""
+        """Enqueue one iteration (the optional events mark the end of fwd+bwd, of the update, of the validation pass).
+        In carried mode ``show`` changes nothing: ACC[tr] comes from the tail pass on every step."""
         m, lib, dist = self.m, self.m.lib, self.dist
         _capi.check(lib.g2v_cbow_loop_begin(self.ctl.data_ptr(), m.acc.data_ptr(), m.W_ih.data_ptr(),
                                             None if self.result is None else self.result.data_ptr(), m.V * m.D,
                                             self._st()), "g2v_cbow_loop_begin")
         if self.n_tr_loc:
             m.fwdbwd(self.tr_d, self.n_tr)       # acc[1] += correct predictions with the PRE-update weights
+                                                 # (carried: the forward is skipped on the device, acc[1] carried)
         if m_fb is not None:
             m_fb.record()
         if dist:
@@ -654,7 +670,14 @@ class DeviceLoop:
             m.evaluate(self.va_d, 2)
         if m_val is not None:
             m_val.record()
-        if show and self.n_tr_loc:
+        if self.carried:
+            csc = m._csc
+            _capi.check(lib.g2v_cbow_loop_tail(self.ctl.data_ptr(), m.rowptr.data_ptr(), m.gene.data_ptr(),
+                                               m.label.data_ptr(), self.tr_d.data_ptr(), self.n_tr_loc,
+                                               1.0 / float(self.n_tr), m.W_ih.data_ptr(), m.W_ho.data_ptr(),
+                                               csc[4].data_ptr(), m.g_ho.data_ptr(), m.acc.data_ptr(), m.V, m.D,
+                                               m.reduce, self._st()), "g2v_cbow_loop_tail")
+        elif show and self.n_tr_loc:
             m.evaluate(self.tr_d, 3)
         acc_ptr = m.acc.data_ptr()
         if self.hist_nvl:
@@ -688,13 +711,13 @@ def _device_loop(model, dist, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_ep
                  use_graph, chunk=5):
     """Full-batch loop of G2Vec.py:262-283 with the early-stop rule, the result snapshot and the step counter on
     the DEVICE (g2v_cbow_loop_*): the host enqueues `chunk` iterations at a time -- one CUDA-graph replay of
-    4 plain iterations + 1 that also runs the training-accuracy pass -- and synchronises once per printed line
-    instead of once per step.  Iterations enqueued after the stop are no-ops (every kernel tests ctl.stopped).
-    Multi-GPU: the all-reduces are part of the captured graph (NCCL is capturable); if capture is refused the
-    same launches run eagerly."""
+    4 plain iterations + 1 that also runs the training-accuracy pass (in carried mode, five identical iterations
+    that all have it) -- and synchronises once per printed line instead of once per step.  Iterations enqueued after
+    the stop are no-ops (every kernel tests ctl.stopped).  Multi-GPU: the all-reduces are part of the captured graph
+    (NCCL is capturable); if capture is refused the same launches run eagerly."""
     dev = model.device
     loop = DeviceLoop(model, dist, tr_d, va_d, n_tr, max_epoch, early_stop, snapshot=bool(early_stop))
-    shown = lambda s: s % 5 == 0 or eval_train == "always"
+    shown = lambda s: loop.carried or s % 5 == 0 or eval_train == "always"
     info = _LoopLog(n_tr, n_va, log)
 
     def consume(lo, hi):
@@ -734,7 +757,8 @@ def _device_loop(model, dist, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_ep
             done += k
         stop = int(loop.ctl_pin[2]) if int(loop.ctl_pin[2]) >= 0 else None
         if stop is None and info.hist and info.hist[-1][2] is None:
-            # ACC[tr] of the last step was never needed for a log line; evaluate it once for the history
+            # ACC[tr] of the last step was never needed for a log line; evaluate it once for the history (a carried
+            # loop has it for every step)
             loop.detach()
             model.acc.zero_()
             if n_tr_loc:

@@ -23,6 +23,9 @@ void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 static thread_local const int32_t *g_skip = nullptr;
 const int32_t *loop_skip_flag() { return g_skip; }
 void set_loop_skip_flag(const int32_t *p) { g_skip = p; }
+static thread_local const int32_t *g_carry = nullptr;
+const int32_t *loop_carry_flag() { return g_carry; }
+void set_loop_carry_flag(const int32_t *p) { g_carry = p; }
 
 int device_props(DeviceProps *out) {
     static thread_local int cached_dev = -1;

@@ -50,6 +50,7 @@ constexpr bool kDefaultScatterTma = false;   // G2V_CBOW_SCATTER=tma selects the
 // one lane issuing one row; the lanes then sum the rows with LDS.128 instead of LDG.128.
 // CSC: the backward stops at dO -- it stores dO*scale at the window's list position i (dO_pos[i]) instead of
 // scattering rows into g_ih; cbow_csc_expand_kernel then sums those scalars per gene and writes each gene row once.
+// carried != NULL and set: the loop's tail pass already ran this forward at these weights (g2v_cbow_loop_tail).
 template <int VEC, bool BACKWARD, bool SCATTER_TMA, bool GATHER_TMA, bool CSC = false>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
@@ -57,9 +58,11 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
                  int64_t win_begin, int64_t n_win, float inv_n, const float *__restrict__ W_ih,
                  const float *__restrict__ W_ho, float *__restrict__ g_ih, float *__restrict__ g_ho,
                  double *__restrict__ loss_sum, unsigned long long *__restrict__ n_correct,
-                 int32_t reduce_mean, const int32_t *__restrict__ skip, float *__restrict__ dO_pos) {
+                 int32_t reduce_mean, const int32_t *__restrict__ skip, float *__restrict__ dO_pos,
+                 const int32_t *__restrict__ carried) {
     static_assert(!CSC || (BACKWARD && !SCATTER_TMA), "the CSC backward replaces the scatter");
     G2V_SKIP_IF_STOPPED(skip);
+    G2V_SKIP_IF_STOPPED(carried);
     constexpr int D = 128 * VEC;
     constexpr int D4 = D / 4;
     constexpr int UNR = 8 / VEC;                 // 8 float4 (128 B) in flight per lane
@@ -268,8 +271,10 @@ cbow_rows_generic_kernel(const int32_t *__restrict__ rowptr, const int32_t *__re
                          const float *__restrict__ W_ho, float *__restrict__ g_ih,
                          float *__restrict__ g_ho, double *__restrict__ loss_sum,
                          unsigned long long *__restrict__ n_correct, int32_t D, int32_t reduce_mean,
-                         const int32_t *__restrict__ skip, float *__restrict__ dO_pos) {
+                         const int32_t *__restrict__ skip, float *__restrict__ dO_pos,
+                         const int32_t *__restrict__ carried) {
     G2V_SKIP_IF_STOPPED(skip);
+    G2V_SKIP_IF_STOPPED(carried);
     extern __shared__ float shf[];
     __shared__ CtaAcc sh_acc;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -555,12 +560,13 @@ int rows_grid(const void *kernel, size_t smem, int64_t n_win, int *grid_out) {
     return 0;
 }
 
-// dO_pos != NULL (backward only): the CSC backward -- dO*scale per list position instead of the scatter into g_ih
+// dO_pos != NULL (backward only): the CSC backward -- dO*scale per list position instead of the scatter into g_ih.
+// carried: the word that makes the launched kernel return at once when set (besides `stopped`), or NULL.
 template <bool BACKWARD>
 static int launch_rows(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
                        int64_t win_begin, int64_t n_win, float inv_n, const float *W_ih, const float *W_ho,
                        float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t D,
-                       int32_t reduce, cudaStream_t st, float *dO_pos = nullptr) {
+                       int32_t reduce, cudaStream_t st, float *dO_pos = nullptr, const int32_t *carried = nullptr) {
     unsigned long long *nc = reinterpret_cast<unsigned long long *>(n_correct);
     int grid = 0, rc;
     // scatter path of the backward kernel: "red" (red.global.add.v4.f32 per lane) or "tma"
@@ -578,7 +584,7 @@ static int launch_rows(const int32_t *rowptr, const int32_t *gene, const uint8_t
         if (dO_pos) kern = cbow_rows_kernel<VEC, BACKWARD, false, false, BACKWARD>;                  \
         if ((rc = rows_grid((const void *)kern, 0, n_win, &grid))) return rc;                        \
         kern<<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, win_begin, n_win, inv_n, W_ih, W_ho, g_ih, \
-                                               g_ho, loss_sum, nc, reduce, loop_skip_flag(), dO_pos); \
+                                               g_ho, loss_sum, nc, reduce, loop_skip_flag(), dO_pos, carried); \
     }
     if (D == 128) G2V_LAUNCH_VEC(1)
     else if (D == 256) G2V_LAUNCH_VEC(2)
@@ -592,7 +598,7 @@ static int launch_rows(const int32_t *rowptr, const int32_t *gene, const uint8_t
         if ((rc = rows_grid((const void *)cbow_rows_generic_kernel<BACKWARD>, smem, n_win, &grid))) return rc;
         cbow_rows_generic_kernel<BACKWARD><<<grid, kCbowWarps * 32, smem, st>>>(
             rowptr, gene, label, win, win_begin, n_win, inv_n, W_ih, W_ho, g_ih, g_ho, loss_sum, nc, D, reduce, loop_skip_flag(),
-            dO_pos);
+            dO_pos, carried);
     }
 #undef G2V_LAUNCH_VEC
     G2V_CUDA_OK(cudaGetLastError());
@@ -608,8 +614,17 @@ static int launch_rows(const int32_t *rowptr, const int32_t *gene, const uint8_t
 //   [2] stop_step    step whose validation accuracy dropped, -1 if none (the reference breaks there, :279)
 //   [3] before_val   correct validation windows of the last passed step (before_acc_val, :280; -1 = the -1. of :261)
 //   [4] max_steps    cap on optimizer steps (--epoch)       [5] early_stop   0 = never stop early
+//   [6] carried      1 once a tail pass (g2v_cbow_loop_tail) has run the training forward of the current weights:
+//                    dO per list position, the g_ho partial and the carry counters acc[4..5] are pending, and the
+//                    forward of g2v_cbow_fwdbwd_csc returns at once while the loop is attached
+//   [7] unused
+// acc (int64): [0] loss sum (f64 bits)  [1] pre-update train correct  [2] validation correct  [3] train correct;
+//   with tail passes also [4] carried loss sum (f64 bits)  [5] carried train correct (this rank's own count, kept
+//   out of [1..3], the range a multi-GPU step sums over the ranks).
 // loop_begin:  if not stopped, copy the weights into `snapshot` (they are the result if THIS step's validation
-//   accuracy drops: the reference returns the W_ih read at :283 after the previous step) and zero the 4 counters.
+//   accuracy drops: the reference returns the W_ih read at :283 after the previous step) and zero the 4 counters;
+//   with a carry pending, acc[0..1] take the carried loss and count instead and acc[4..5] are zeroed.
+// loop_carry:  after a tail pass, ACC[tr] of this step (acc[3]) is the carried count; sets ctl[6].
 // loop_decide: if not stopped, record the step's counters in hist[step][0..3], apply the early-stop rule on the
 //   validation count (same ordering as the float32 ratios the reference compares while n_val < 2^24), advance.
 __global__ void __launch_bounds__(256)
@@ -617,10 +632,24 @@ loop_begin_kernel(const long long *__restrict__ ctl, long long *__restrict__ acc
                   float4 *__restrict__ S4, int64_t n4, const float *__restrict__ W, float *__restrict__ S, int64_t n) {
     if (ctl[0] != 0) return;
     const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
-    if (tid < 4) acc[tid] = 0;
+    if (tid == 0) {
+        if (ctl[6] != 0) {
+            acc[0] = acc[4]; acc[1] = acc[5];
+            acc[4] = 0; acc[5] = 0;
+        } else {
+            acc[0] = 0; acc[1] = 0;
+        }
+        acc[2] = 0; acc[3] = 0;
+    }
     if (S == nullptr) return;
     for (int64_t i = tid; i < n4; i += nth) S4[i] = W4[i];
     for (int64_t i = (n4 << 2) + tid; i < n; i += nth) S[i] = W[i];
+}
+
+__global__ void loop_carry_kernel(long long *__restrict__ ctl, long long *__restrict__ acc) {
+    if (ctl[0] != 0) return;
+    acc[3] += acc[5];
+    ctl[6] = 1;
 }
 
 // acc == NULL: the step's counters were already summed over the ranks into hist[step] (loop_counters_nvl_kernel)
@@ -674,8 +703,10 @@ extern "C" int g2v_cbow_loop_init(int64_t *ctl, int64_t max_steps, int32_t early
 }
 
 extern "C" int g2v_cbow_loop_attach(const int64_t *ctl) {
-    // the low 32 bits of ctl[0] (little endian) are the `stopped` word every step kernel tests
+    // the low 32 bits of ctl[0] (little endian) are the `stopped` word every step kernel tests; those of ctl[6]
+    // the `carried` word the forward of g2v_cbow_fwdbwd_csc also tests
     set_loop_skip_flag(reinterpret_cast<const int32_t *>(ctl));
+    set_loop_carry_flag(ctl ? reinterpret_cast<const int32_t *>(ctl + 6) : nullptr);
     return 0;
 }
 
@@ -739,8 +770,9 @@ extern "C" int g2v_cbow_fwdbwd_csc(const int32_t *rowptr, const int32_t *gene, c
     G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "g2v_cbow_fwdbwd_csc: unknown reduce %d", reduce);
     if (n_win == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
+    // with a tail pass pending (attached loop, ctl[6] set) the forward returns at once and the expansion reads its dO
     int rc = launch_rows<true>(rowptr, gene, label, win, 0, n_win, inv_n_total, W_ih, W_ho, g_ih, g_ho, loss_sum,
-                               n_correct, D, reduce, st, dO);
+                               n_correct, D, reduce, st, dO, loop_carry_flag());
     if (rc) return rc;
     int grid = 0;
     if ((rc = rows_grid((const void *)cbow_csc_expand_kernel, 0, V, &grid))) return rc;
@@ -760,6 +792,21 @@ extern "C" int g2v_cbow_fwd_do(const int32_t *rowptr, const int32_t *gene, const
     if (n_win == 0) return 0;
     return launch_rows<true>(rowptr, gene, label, win, 0, n_win, inv_n_total, W_ih, W_ho, nullptr, g_ho, loss_sum,
                              n_correct, D, reduce, (cudaStream_t)stream, dO);
+}
+
+extern "C" int g2v_cbow_loop_tail(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                  const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                                  const float *W_ho, float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D,
+                                  int32_t reduce, void *stream) {
+    G2V_REQUIRE(ctl && acc, "g2v_cbow_loop_tail: null loop state");
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = g2v_cbow_fwd_do(rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho,
+                             reinterpret_cast<double *>(acc + 4), acc + 5, V, D, reduce, st);
+    if (rc) return rc;
+    loop_carry_kernel<<<1, 1, 0, st>>>(reinterpret_cast<long long *>(ctl), reinterpret_cast<long long *>(acc));
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
 }
 
 extern "C" int g2v_cbow_eval(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,

@@ -35,6 +35,10 @@ void count_launch(int n = 1);
 // follow the early stop (G2Vec.py:276-279) inside an already enqueued graph are no-ops.
 void set_loop_skip_flag(const int32_t *p);
 const int32_t *loop_skip_flag();   // thread-local, set by g2v_cbow_loop_attach (NULL = no loop control)
+// The loop's `carried` word (set once a step's tail pass has run the next step's training forward): the forward
+// of g2v_cbow_fwdbwd_csc tests it like `stopped` and returns at once.  Thread-local, set with the skip flag.
+void set_loop_carry_flag(const int32_t *p);
+const int32_t *loop_carry_flag();
 #define G2V_SKIP_IF_STOPPED(skip) \
     do { if ((skip) != nullptr && *reinterpret_cast<const volatile int32_t *>(skip) != 0) return; } while (0)
 

@@ -186,12 +186,21 @@ int g2v_cbow_eval(const int32_t *rowptr, const int32_t *gene, const uint8_t *lab
 /* ---------------------------------------------------------------------------------------
  * Device-side control of the training loop (SURVEY.md 8f-4; G2Vec.py:262-283), so that several iterations of
  * the reference's loop can be enqueued -- or replayed as ONE CUDA graph -- without a host decision in between.
- *   ctl  [8] int64 in device memory: {stopped, step, stop_step, before_val, max_steps, early_stop, -, -}
- *        g2v_cbow_loop_init sets {0, 0, -1, -1, max_steps, early_stop}.
+ *   ctl  [8] int64 in device memory: {stopped, step, stop_step, before_val, max_steps, early_stop, carried, -}
+ *        g2v_cbow_loop_init sets {0, 0, -1, -1, max_steps, early_stop, 0}.
  *   g2v_cbow_loop_attach(ctl): from now on every CBOW kernel launched by THIS host thread first reads
- *        ctl.stopped and returns at once if it is set (attach(NULL) detaches).
+ *        ctl.stopped and returns at once if it is set (attach(NULL) detaches); the forward of
+ *        g2v_cbow_fwdbwd_csc also returns at once while ctl.carried is set (its per-gene expansion still runs).
  *   g2v_cbow_loop_begin: unless stopped, copies W_ih [n floats] into `snapshot` (nullable) -- the weights the
- *        reference would return if this step's validation accuracy drops (:283,:286) -- and zeroes acc[0..3].
+ *        reference would return if this step's validation accuracy drops (:283,:286) -- and zeroes acc[0..3];
+ *        if ctl.carried is set, acc[0..1] take the carried loss and count acc[4..5] instead, which are zeroed.
+ *   g2v_cbow_loop_tail: the training-accuracy pass of a step (after the update and the validation pass) that is
+ *        also the next step's forward -- valid because nothing changes the weights or the training list in
+ *        between.  It runs g2v_cbow_fwd_do over the training list win[0..n_win-1] for which the caller prepared
+ *        g2v_cbow_fwdbwd_csc's transposed incidence: dO [n_win] per list position, g_ho += sum h*dO (the update
+ *        has just zeroed it), loss sum into acc[4] (f64 bits), correct count into acc[5]; then, unless stopped,
+ *        acc[3] += acc[5] (the step's ACC[tr]) and ctl.carried = 1.  acc is then int64 [6]: the carry slots lie
+ *        outside acc[1..3], which a multi-GPU step sums over the ranks.  Two launches.
  *   g2v_cbow_loop_decide: unless stopped, stores acc[0..3] (loss-sum bits, pre-update train correct, validation
  *        correct, train correct) in hist[step*4 ..] (acc == NULL: they are there already, see below), applies `if acc_val < before_acc_val: break` (:276) on the
  *        validation count, else before_val = count (:280); stops after max_steps; step += 1.
@@ -200,6 +209,9 @@ int g2v_cbow_eval(const int32_t *rowptr, const int32_t *gene, const uint8_t *lab
 int g2v_cbow_loop_init(int64_t *ctl, int64_t max_steps, int32_t early_stop, void *stream);
 int g2v_cbow_loop_attach(const int64_t *ctl);
 int g2v_cbow_loop_begin(const int64_t *ctl, int64_t *acc, const float *W_ih, float *snapshot, int64_t n, void *stream);
+int g2v_cbow_loop_tail(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                       const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
+                       float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D, int32_t reduce, void *stream);
 int g2v_cbow_loop_decide(int64_t *ctl, const int64_t *acc, int64_t *hist, void *stream);
 /* Multi-GPU, hist in symmetric memory (zero-initialised, same size on every rank): add this rank's acc[1..3] into
  * hist[step][1..3] of every rank (multimem.red through hist_multicast, or system-scope atomics on hist_ptrs_dev);
