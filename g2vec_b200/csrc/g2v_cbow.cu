@@ -4,16 +4,15 @@
 // multi-hot X [N, V] (99.7 % zeros) and lets TF1 autodiff + ApplyAdam train W_ih, W_ho
 // (G2Vec.py:239-246).  Here X is CSR (window -> gene ids) and one warp owns one window:
 //
-//   cbow_rows_kernel<VEC, BACKWARD, SCATTER_TMA, GATHER_TMA>
-//                                         D = 128*VEC, each lane owns VEC float4 of the row; the two TMA
-//                                         flags select the measured-and-not-shipped staged variants (4.4)
+//   cbow_rows_kernel<VEC, MODE>          D = 128*VEC, each lane owns VEC float4 of the row; MODE: eval (the
+//                                         accuracy pass: gather and logit only), scatter, or CSC (below)
 //     gather   h   = sum_{g in window} W_ih[g, :]          (512*VEC B coalesced per row, 8 rows in flight)
 //     logit    o   = <h, W_ho>                            (warp shuffle reduction)
 //     loss/acc     max(o,0) - o*y + log1p(exp(-|o|)),  (o > 0) == y
 //     grad     dO  = (sigmoid(o) - y) / N                 (N known up front: no global barrier)
 //     scatter  g_ih[g, :] += dO * W_ho  for g in window   (red.global.add.v4.f32, 16 B per lane)
 //              g_ho       += h * dO                       (registers -> smem -> one atomic per CTA)
-//   cbow_rows_kernel<VEC, true, false, false, CSC=true>   the same up to dO; then, instead of the scatter,
+//   cbow_rows_kernel<VEC, kRowsCsc>       the same up to dO; then, instead of the scatter,
 //                                         dO_pos[i] = dO * scale  at the window's list position i (4 B per window)
 //   cbow_csc_expand_kernel                one warp per gene: c = sum of dO_pos over the gene's segment of the list's
 //                                         transposed incidence (CSC), then g_ih[g, :] += c * W_ho, one plain
@@ -32,26 +31,17 @@
 // No tensor cores: the 128..512-wide reduction is a memory-bound gather/scatter, not a dense
 // contraction.  Algorithmic bytes per window: l*(8D+4)+5 with the scatter, l*(4D+12)+9 with the CSC backward
 // (+ 8*D per touched gene row) (DESIGN.md), per step + 32*V*D (Adam).
-#include <stdlib.h>
-
 #include "g2v_cbow_common.cuh"
 
 namespace g2v {
 
-constexpr bool kDefaultGatherTma = false;
-constexpr bool kDefaultScatterTma = false;   // G2V_CBOW_SCATTER=tma selects the bulk-reduction scatter
+// MODE of cbow_rows_kernel.  kRowsCsc: the backward stops at dO -- it stores dO*scale at the window's list position i
+// (dO_pos[i]) instead of scattering rows into g_ih; cbow_csc_expand_kernel then sums those scalars per gene and writes
+// each gene row once.
+constexpr int kRowsEval = 0, kRowsScatter = 1, kRowsCsc = 2;
 
-// SCATTER_TMA: the gradient row dO*W_ho (identical for every gene of the window) is staged once in
-// shared memory and added into g_ih[gene,:] with one TMA bulk reduction per gene
-// (cp.reduce.async.bulk.global.shared::cta.add.f32, D*4 bytes, SASS UBLKRED) instead of 32 lanes x
-// red.global.add.v4.f32: the scatter leaves the LSU/L1TEX path, which bounds the L2-resident configs.
-// GATHER_TMA: embedding rows are staged through shared memory with TMA bulk copies
-// (cp.async.bulk.shared::cluster.global + mbarrier complete_tx, SASS UBLKCP), 2 stages of 2 KB per warp,
-// one lane issuing one row; the lanes then sum the rows with LDS.128 instead of LDG.128.
-// CSC: the backward stops at dO -- it stores dO*scale at the window's list position i (dO_pos[i]) instead of
-// scattering rows into g_ih; cbow_csc_expand_kernel then sums those scalars per gene and writes each gene row once.
 // carried != NULL and set: the loop's tail pass already ran this forward at these weights (g2v_cbow_loop_tail).
-template <int VEC, bool BACKWARD, bool SCATTER_TMA, bool GATHER_TMA, bool CSC = false>
+template <int VEC, int MODE>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
                  const uint8_t *__restrict__ label, const int32_t *__restrict__ win,
@@ -60,31 +50,18 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
                  double *__restrict__ loss_sum, unsigned long long *__restrict__ n_correct,
                  int32_t reduce_mean, const int32_t *__restrict__ skip, float *__restrict__ dO_pos,
                  const int32_t *__restrict__ carried) {
-    static_assert(!CSC || (BACKWARD && !SCATTER_TMA), "the CSC backward replaces the scatter");
     G2V_SKIP_IF_STOPPED(skip);
     G2V_SKIP_IF_STOPPED(carried);
+    constexpr bool BACKWARD = MODE != kRowsEval;
     constexpr int D = 128 * VEC;
     constexpr int D4 = D / 4;
     constexpr int UNR = 8 / VEC;                 // 8 float4 (128 B) in flight per lane
     __shared__ float sh_gho[BACKWARD ? D : 1];
-    // scatter staging row: its own buffer, or (both TMA paths on) stage 0 of the gather tile
-    __shared__ __align__(128) float sh_row[(BACKWARD && SCATTER_TMA && !GATHER_TMA) ? kCbowWarps * D : 4];
     __shared__ CtaAcc sh_acc;
-    constexpr int R = 4 / VEC;                   // rows per TMA stage (2 KB per warp per stage)
-    __shared__ __align__(128) float sh_tile[GATHER_TMA ? kCbowWarps * 2 * R * D : 4];
-    __shared__ __align__(8) unsigned long long sh_bar[GATHER_TMA ? kCbowWarps * 2 : 1];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (BACKWARD) for (int i = threadIdx.x; i < D; i += blockDim.x) sh_gho[i] = 0.f;
     if (threadIdx.x == 0) { sh_acc.loss = 0.0; sh_acc.correct = 0ull; }
-    if (GATHER_TMA) {
-        if (lane < 2) {
-            const uint32_t a = (uint32_t)__cvta_generic_to_shared(&sh_bar[warp * 2 + lane]);
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(a) : "memory");
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
     __syncthreads();
-    uint32_t tma_phase = 0;                      // bit s = parity of stage s
 
     const float4 *__restrict__ W4 = reinterpret_cast<const float4 *>(W_ih);
     float4 who[VEC], gho[VEC];
@@ -93,8 +70,8 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
         who[v] = ldg4(reinterpret_cast<const float4 *>(W_ho) + v * 32 + lane);
         gho[v] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    float loss_acc = 0.f;
     unsigned correct_acc = 0;
+    float loss_acc = 0.f;
 
     const int64_t warps_total = (int64_t)gridDim.x * kCbowWarps;
     for (int64_t i = (int64_t)blockIdx.x * kCbowWarps + warp; i < n_win; i += warps_total) {
@@ -104,59 +81,6 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
         float4 h[VEC];
 #pragma unroll
         for (int v = 0; v < VEC; ++v) h[v] = make_float4(0.f, 0.f, 0.f, 0.f);
-
-        // ---- gather + segmented sum
-        if (GATHER_TMA) {
-            float *tile = sh_tile + (size_t)warp * 2 * R * D;
-            if (BACKWARD && SCATTER_TMA) {        // stage 0 doubles as the scatter staging row: drain its readers
-                asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                __syncwarp();
-            }
-            const uint32_t bar0 = (uint32_t)__cvta_generic_to_shared(&sh_bar[warp * 2]);
-            const int nchunk = (e - b + R - 1) / R;
-            auto issue = [&](int c) {             // chunk c -> stage c & 1: lane r copies row r
-                const int st = c & 1;
-                const int32_t j = b + c * R + lane;
-                const int cnt = min(R, e - (b + c * R));
-                if (lane == 0)
-                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar0 + st * 8),
-                                 "r"(cnt * D * 4)
-                                 : "memory");
-                if (lane < cnt) {
-                    const float *src = W_ih + (size_t)__ldg(gene + j) * D;
-                    const uint32_t dst = (uint32_t)__cvta_generic_to_shared(tile + (size_t)(st * R + lane) * D);
-                    asm volatile(
-                        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-                        "l"(src), "n"(D * 4), "r"(bar0 + st * 8)
-                        : "memory");
-                }
-            };
-            if (nchunk > 0) issue(0);
-            for (int c = 0; c < nchunk; ++c) {
-                const int st = c & 1;
-                if (c + 1 < nchunk) issue(c + 1);
-                const uint32_t par = (tma_phase >> st) & 1u;
-                uint32_t ok = 0;
-                while (!ok)
-                    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                                 : "=r"(ok)
-                                 : "r"(bar0 + st * 8), "r"(par)
-                                 : "memory");
-                tma_phase ^= (1u << st);
-                const int cnt = min(R, e - (b + c * R));
-                const float4 *t4 = reinterpret_cast<const float4 *>(tile + (size_t)st * R * D);
-#pragma unroll
-                for (int r = 0; r < R; ++r)
-                    if (r < cnt) {
-#pragma unroll
-                        for (int v = 0; v < VEC; ++v) {
-                            const float4 x = t4[r * D4 + v * 32 + lane];
-                            h[v].x += x.x; h[v].y += x.y; h[v].z += x.z; h[v].w += x.w;
-                        }
-                    }
-                __syncwarp();                     // stage st is free for chunk c + 2
-            }
-        } else
         for (int32_t base = b; base < e; base += 32) {
             const int cnt = min(32, e - base);
             const int32_t g = (lane < cnt) ? __ldg(gene + base + lane) : 0;
@@ -190,14 +114,14 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
             correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
             if (BACKWARD) loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
         }
-        if (CSC) {
+        if (MODE == kRowsCsc) {
             const float dO = (sigmoid_stable(o) - y) * inv_n;
 #pragma unroll
             for (int v = 0; v < VEC; ++v) {
                 gho[v].x += h[v].x * dO; gho[v].y += h[v].y * dO; gho[v].z += h[v].z * dO; gho[v].w += h[v].w * dO;
             }
             if (lane == 0) dO_pos[i] = dO * scale;
-        } else if (BACKWARD) {
+        } else if (MODE == kRowsScatter) {
             const float dO = (sigmoid_stable(o) - y) * inv_n;
             float4 gv[VEC];
 #pragma unroll
@@ -206,25 +130,6 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
                 const float s = dO * scale;
                 gv[v] = make_float4(who[v].x * s, who[v].y * s, who[v].z * s, who[v].w * s);
             }
-            // ---- scatter-add the gradient rows
-            if (SCATTER_TMA) {
-                float *stage = GATHER_TMA ? sh_tile + (size_t)warp * 2 * R * D : sh_row + warp * D;
-                // the previous window's bulk reductions must have finished READING the staging row
-                asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                __syncwarp();
-#pragma unroll
-                for (int v = 0; v < VEC; ++v) reinterpret_cast<float4 *>(stage)[v * 32 + lane] = gv[v];
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy
-                __syncwarp();
-                const uint32_t src = (uint32_t)__cvta_generic_to_shared(stage);
-                for (int32_t j = b + lane; j < e; j += 32) {
-                    float *dst = g_ih + (size_t)__ldg(gene + j) * D;
-                    asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;"
-                                 ::"l"(dst), "r"(src), "n"(D * 4)
-                                 : "memory");
-                }
-                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            } else
             for (int32_t base = b; base < e; base += 32) {
                 const int cnt = min(32, e - base);
                 const int32_t g = (lane < cnt) ? __ldg(gene + base + lane) : 0;
@@ -237,28 +142,7 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
             }
         }
     }
-
-    if (BACKWARD && SCATTER_TMA) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-
-    // ---- CTA-level reduction of g_ho / loss / correct, then one global atomic each
-    if (BACKWARD) {
-#pragma unroll
-        for (int v = 0; v < VEC; ++v) {
-            float *p = sh_gho + (v * 32 + lane) * 4;
-            atomicAdd(p + 0, gho[v].x); atomicAdd(p + 1, gho[v].y);
-            atomicAdd(p + 2, gho[v].z); atomicAdd(p + 3, gho[v].w);
-        }
-    }
-    if (lane == 0) {
-        if (BACKWARD) atomicAdd(&sh_acc.loss, (double)loss_acc);
-        atomicAdd(&sh_acc.correct, (unsigned long long)correct_acc);
-    }
-    __syncthreads();
-    if (BACKWARD) for (int i = threadIdx.x; i < D; i += blockDim.x) atomicAdd(g_ho + i, sh_gho[i]);
-    if (threadIdx.x == 0) {
-        if (BACKWARD && loss_sum) atomicAdd(loss_sum, sh_acc.loss);
-        if (n_correct) atomicAdd(n_correct, sh_acc.correct);
-    }
+    cta_epilogue<VEC, BACKWARD, true>(sh_gho, sh_acc, gho, loss_acc, correct_acc, lane, g_ho, loss_sum, n_correct);
 }
 
 // Any D (not a multiple of 128): h and the g_ho partial live in shared memory per warp.
@@ -364,15 +248,6 @@ cbow_csc_expand_kernel(const int32_t *__restrict__ cscptr, const int32_t *__rest
 }
 
 // ---- optimizer epilogue --------------------------------------------------------------------
-// TF1 ApplyAdam (tensorflow/core/kernels/training_ops.cc):  m += (g-m)(1-b1); v += (g*g-v)(1-b2);
-// var -= (m*alpha)/(sqrt(v)+eps), alpha = lr*sqrt(1-b2^t)/(1-b1^t).
-__device__ __forceinline__ void adam1(float &w, float &m, float &v, float g, float alpha, float omb1,
-                                      float omb2, float eps) {
-    m += (g - m) * omb1;
-    v += (g * g - v) * omb2;
-    w -= (m * alpha) / (sqrtf(v) + eps);
-}
-
 template <int OPT>
 __global__ void __launch_bounds__(256)
 cbow_update_kernel(float *__restrict__ W, float *__restrict__ M, float *__restrict__ Vv,
@@ -546,7 +421,7 @@ cbow_update_nvl_kernel(float *const *__restrict__ g_ptrs, float *const *__restri
         }
 }
 
-int rows_grid(const void *kernel, size_t smem, int64_t n_win, int *grid_out) {
+int rows_grid(const void *kernel, size_t smem, int64_t n_items, int *grid_out) {
     DeviceProps dp;
     if (device_props(&dp)) return 1;
     if (dp.cc_major != 9) { set_error("needs an sm_90 device (found sm_%d%d); no CPU fallback", dp.cc_major, dp.cc_minor); return 2; }
@@ -554,7 +429,7 @@ int rows_grid(const void *kernel, size_t smem, int64_t n_win, int *grid_out) {
     cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kCbowWarps * 32, smem);
     if (e != cudaSuccess || per_sm <= 0) { set_error("occupancy query failed: %s", cudaGetErrorString(e)); return 1; }
     int64_t grid = (int64_t)dp.sm_count * per_sm;
-    const int64_t need = (n_win + kCbowWarps - 1) / kCbowWarps;
+    const int64_t need = (n_items + kCbowWarps - 1) / kCbowWarps;
     if (grid > need) grid = need;
     *grid_out = (int)(grid > 0 ? grid : 1);
     return 0;
@@ -569,20 +444,11 @@ static int launch_rows(const int32_t *rowptr, const int32_t *gene, const uint8_t
                        int32_t reduce, cudaStream_t st, float *dO_pos = nullptr, const int32_t *carried = nullptr) {
     unsigned long long *nc = reinterpret_cast<unsigned long long *>(n_correct);
     int grid = 0, rc;
-    // scatter path of the backward kernel: "red" (red.global.add.v4.f32 per lane) or "tma"
-    // (cp.reduce.async.bulk per gene row); G2V_CBOW_SCATTER overrides the default
-    const char *sc = getenv("G2V_CBOW_SCATTER");
-    const bool tma = BACKWARD && (sc ? sc[0] == 't' : kDefaultScatterTma);
-    const char *gc = getenv("G2V_CBOW_GATHER");       // "ldg" (LDG.128 per lane) or "tma" (bulk copies via smem)
-    const bool gtma = gc ? gc[0] == 't' : kDefaultGatherTma;
-#define G2V_LAUNCH_VEC(VEC)                                                                          \
-    {                                                                                                \
-        auto kern = tma ? (gtma ? cbow_rows_kernel<VEC, BACKWARD, BACKWARD, true>                    \
-                                : cbow_rows_kernel<VEC, BACKWARD, BACKWARD, false>)                  \
-                        : (gtma ? cbow_rows_kernel<VEC, BACKWARD, false, true>                       \
-                                : cbow_rows_kernel<VEC, BACKWARD, false, false>);                    \
-        if (dO_pos) kern = cbow_rows_kernel<VEC, BACKWARD, false, false, BACKWARD>;                  \
-        if ((rc = rows_grid((const void *)kern, 0, n_win, &grid))) return rc;                        \
+#define G2V_LAUNCH_VEC(VEC)                                                                                            \
+    {                                                                                                                  \
+        auto kern = !BACKWARD ? cbow_rows_kernel<VEC, kRowsEval>                                                       \
+                              : dO_pos ? cbow_rows_kernel<VEC, kRowsCsc> : cbow_rows_kernel<VEC, kRowsScatter>;        \
+        if ((rc = rows_grid((const void *)kern, 0, n_win, &grid))) return rc;                                          \
         kern<<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, win_begin, n_win, inv_n, W_ih, W_ho, g_ih, \
                                                g_ho, loss_sum, nc, reduce, loop_skip_flag(), dO_pos, carried); \
     }
@@ -854,10 +720,7 @@ extern "C" int g2v_cbow_update(float *W_ih, float *W_ho, float *m_ih, float *v_i
     if (blocks < 1) blocks = 1;
     cudaStream_t st = (cudaStream_t)stream;
     if (optimizer == G2V_OPT_ADAM_TF1) {
-        // beta^t by repeated float32 multiplication, as TF1's beta1_power / beta2_power variables
-        float b1p = 1.f, b2p = 1.f;
-        for (int i = 0; i < t; ++i) { b1p *= beta1; b2p *= beta2; }
-        const float alpha = alpha_dev ? 0.f : lr * sqrtf(1.f - b2p) / (1.f - b1p);
+        const float alpha = alpha_dev ? 0.f : adam_tf1_alpha(lr, beta1, beta2, t);
         cbow_update_kernel<G2V_OPT_ADAM_TF1><<<(unsigned)blocks, 256, 0, st>>>(
             W_ih, m_ih, v_ih, g_ih, n, W_ho, m_ho, v_ho, g_ho, (int64_t)D, alpha, 1.f - beta1, 1.f - beta2, eps,
             alpha_dev, loop_skip_flag());
@@ -879,9 +742,7 @@ extern "C" int g2v_cbow_lazy_adam(const int32_t *rows, const int32_t *segptr, co
     G2V_REQUIRE(W_ih && m_ih && v_ih && W_ho && m_ho && v_ho && g_ho, "g2v_cbow_lazy_adam: null pointer");
     G2V_REQUIRE(n_rows == 0 || (rows && segptr && pos && dO), "g2v_cbow_lazy_adam: null row list");
     cudaStream_t st = (cudaStream_t)stream;
-    float b1p = 1.f, b2p = 1.f;
-    for (int i = 0; i < t; ++i) { b1p *= beta1; b2p *= beta2; }
-    const float alpha = alpha_dev ? 0.f : lr * sqrtf(1.f - b2p) / (1.f - b1p);
+    const float alpha = alpha_dev ? 0.f : adam_tf1_alpha(lr, beta1, beta2, t);
     int rc, launches = 1;
     if (n_rows > 0) {
         int grid = 0;
@@ -921,9 +782,7 @@ extern "C" int g2v_cbow_update_nvl(float *const *g_ptrs_dev, float *const *w_ptr
     const bool mc = g_multicast != nullptr;
     float alpha = lr, omb1 = 0.f, omb2 = 0.f;
     if (optimizer == G2V_OPT_ADAM_TF1) {
-        float b1p = 1.f, b2p = 1.f;
-        for (int i = 0; i < t; ++i) { b1p *= beta1; b2p *= beta2; }
-        alpha = alpha_dev ? 0.f : lr * sqrtf(1.f - b2p) / (1.f - b1p);
+        alpha = alpha_dev ? 0.f : adam_tf1_alpha(lr, beta1, beta2, t);
         omb1 = 1.f - beta1; omb2 = 1.f - beta2;
     } else {
         alpha_dev = nullptr;

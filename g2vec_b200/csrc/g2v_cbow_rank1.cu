@@ -15,33 +15,18 @@
 //   r1_update_kernel    per row: g = c[g]*W_ho, g_ho += c[g]*W_ih[g,:], Adam/SGD on the row   24*V*D (Adam)
 //   r1_update_ho_kernel Adam/SGD on W_ho from g_ho
 // Multi-GPU exchanges only c (4*V bytes) per step instead of the dense gradient (4*V*D bytes).
-#include "g2v_common.cuh"
+#include "g2v_cbow_common.cuh"
 
 namespace g2v {
 
-constexpr int kR1Warps = 8;
-
-__device__ __forceinline__ float sigmoid_stable_r1(float x) {
-    if (x >= 0.f) { const float z = expf(-x); return 1.f / (1.f + z); }
-    const float z = expf(x);
-    return z / (1.f + z);
-}
-
-__device__ __forceinline__ void adam1_r1(float &w, float &m, float &v, float g, float alpha, float omb1,
-                                         float omb2, float eps) {
-    m += (g - m) * omb1;
-    v += (g * g - v) * omb2;
-    w -= (m * alpha) / (sqrtf(v) + eps);
-}
-
 // ---- s = W_ih . W_ho ----------------------------------------------------------------------------
-__global__ void __launch_bounds__(kR1Warps * 32)
+__global__ void __launch_bounds__(kCbowWarps * 32)
 r1_prepare_kernel(const float *__restrict__ W_ih, const float *__restrict__ W_ho, float *__restrict__ s,
                   int32_t V, int32_t D, const int32_t *__restrict__ skip) {
     G2V_SKIP_IF_STOPPED(skip);
     const int lane = threadIdx.x & 31;
-    const int64_t warp = (int64_t)blockIdx.x * kR1Warps + (threadIdx.x >> 5);
-    const int64_t nwarps = (int64_t)gridDim.x * kR1Warps;
+    const int64_t warp = (int64_t)blockIdx.x * kCbowWarps + (threadIdx.x >> 5);
+    const int64_t nwarps = (int64_t)gridDim.x * kCbowWarps;
     const bool vec4 = (D & 3) == 0;
     for (int64_t g = warp; g < V; g += nwarps) {
         const float *row = W_ih + (size_t)g * D;
@@ -62,12 +47,10 @@ r1_prepare_kernel(const float *__restrict__ W_ih, const float *__restrict__ W_ho
 }
 
 // ---- per-window forward (+ backward into c) -------------------------------------------------------
-struct R1Acc { double loss; unsigned long long correct; };
-
 // MODE 0: accuracy only.  MODE 1: backward with c[gene] += dO (scalar red).  MODE 2: backward that only
 // stores dO[i] for list position i; c is then formed without atomics by r1_csc_reduce_kernel.
 template <int MODE>
-__global__ void __launch_bounds__(kR1Warps * 32)
+__global__ void __launch_bounds__(kCbowWarps * 32)
 r1_windows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
                   const uint8_t *__restrict__ label, const int32_t *__restrict__ win, int64_t win_begin,
                   int64_t n_win, float inv_n, const float *__restrict__ s, float *__restrict__ c,
@@ -75,15 +58,15 @@ r1_windows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict_
                   int32_t reduce_mean, const int32_t *__restrict__ skip) {
     G2V_SKIP_IF_STOPPED(skip);
     constexpr bool BACKWARD = MODE != 0;
-    __shared__ R1Acc sh;
+    __shared__ CtaAcc sh;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int sub = lane & 7, slot = lane >> 3;          // 8 lanes per window, 4 windows per warp
     if (threadIdx.x == 0) { sh.loss = 0.0; sh.correct = 0ull; }
     __syncthreads();
     float loss_acc = 0.f;
     unsigned correct_acc = 0;
-    const int64_t stride = (int64_t)gridDim.x * kR1Warps * 4;
-    for (int64_t base = ((int64_t)blockIdx.x * kR1Warps + warp) * 4; base < n_win; base += stride) {
+    const int64_t stride = (int64_t)gridDim.x * kCbowWarps * 4;
+    for (int64_t base = ((int64_t)blockIdx.x * kCbowWarps + warp) * 4; base < n_win; base += stride) {
         const int64_t i = base + slot;
         const bool active = i < n_win;
         int32_t b = 0, e = 0;
@@ -105,7 +88,7 @@ r1_windows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict_
             correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
             if (BACKWARD) {
                 loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
-                dO = (sigmoid_stable_r1(o) - y) * inv_n * scale;
+                dO = (sigmoid_stable(o) - y) * inv_n * scale;
                 if (MODE == 2) c[i] = dO;                // c is the dO array here
             }
         }
@@ -129,14 +112,14 @@ r1_windows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict_
 
 // c[g] += sum over the list positions whose window contains g of dO[pos]: one warp per gene, fixed lane
 // assignment and shuffle tree => bit-reproducible from run to run (no floating-point atomics).
-__global__ void __launch_bounds__(kR1Warps * 32)
+__global__ void __launch_bounds__(kCbowWarps * 32)
 r1_csc_reduce_kernel(const int32_t *__restrict__ cscptr, const int32_t *__restrict__ csc_pos,
                      const float *__restrict__ dO, float *__restrict__ c, int32_t V,
                      const int32_t *__restrict__ skip) {
     G2V_SKIP_IF_STOPPED(skip);
     const int lane = threadIdx.x & 31;
-    const int64_t warp = (int64_t)blockIdx.x * kR1Warps + (threadIdx.x >> 5);
-    const int64_t nwarps = (int64_t)gridDim.x * kR1Warps;
+    const int64_t warp = (int64_t)blockIdx.x * kCbowWarps + (threadIdx.x >> 5);
+    const int64_t nwarps = (int64_t)gridDim.x * kCbowWarps;
     for (int64_t g = warp; g < V; g += nwarps) {
         const int32_t b = __ldg(cscptr + g), e = __ldg(cscptr + g + 1);
         if (b == e) continue;
@@ -148,7 +131,7 @@ r1_csc_reduce_kernel(const int32_t *__restrict__ cscptr, const int32_t *__restri
 // ---- dense optimizer pass over the rows -----------------------------------------------------------
 // VEC > 0: D = 128*VEC, register accumulators for g_ho.  VEC == 0: any D, shared-memory accumulators.
 template <int VEC, int OPT>
-__global__ void __launch_bounds__(kR1Warps * 32)
+__global__ void __launch_bounds__(kCbowWarps * 32)
 r1_update_kernel(float *__restrict__ W_ih, float *__restrict__ M, float *__restrict__ Vv,
                  const float *__restrict__ W_ho, float *__restrict__ c, float *__restrict__ g_part, int32_t V,
                  int32_t D, float alpha_host, float omb1, float omb2, float eps,
@@ -158,13 +141,13 @@ r1_update_kernel(float *__restrict__ W_ih, float *__restrict__ M, float *__restr
     // g_ho = W_ih^T . c is reduced WITHOUT atomics so that the step is bit-reproducible: every warp owns a
     // row of sh_gho, the block sums its rows in warp order into g_part[blockIdx.x][:], and
     // r1_update_ho_kernel sums the blocks in block order.
-    extern __shared__ float sh_gho[];              // [kR1Warps][D]
+    extern __shared__ float sh_gho[];              // [kCbowWarps][D]
     const int lane = threadIdx.x & 31;
     float *my = sh_gho + (size_t)(threadIdx.x >> 5) * D;
-    for (int i = threadIdx.x; i < kR1Warps * D; i += blockDim.x) sh_gho[i] = 0.f;
+    for (int i = threadIdx.x; i < kCbowWarps * D; i += blockDim.x) sh_gho[i] = 0.f;
     __syncthreads();
-    const int64_t warp = (int64_t)blockIdx.x * kR1Warps + (threadIdx.x >> 5);
-    const int64_t nwarps = (int64_t)gridDim.x * kR1Warps;
+    const int64_t warp = (int64_t)blockIdx.x * kCbowWarps + (threadIdx.x >> 5);
+    const int64_t nwarps = (int64_t)gridDim.x * kCbowWarps;
     if (VEC > 0) {
         constexpr int NV = VEC > 0 ? VEC : 1;  // (dead code when VEC == 0)
         float4 who[NV], acc[NV];
@@ -184,10 +167,10 @@ r1_update_kernel(float *__restrict__ W_ih, float *__restrict__ M, float *__restr
                 acc[v].x += cg * w.x; acc[v].y += cg * w.y; acc[v].z += cg * w.z; acc[v].w += cg * w.w;
                 if (OPT == G2V_OPT_ADAM_TF1) {
                     float4 m = m4[v * 32], vv = v4[v * 32];
-                    adam1_r1(w.x, m.x, vv.x, cg * who[v].x, alpha, omb1, omb2, eps);
-                    adam1_r1(w.y, m.y, vv.y, cg * who[v].y, alpha, omb1, omb2, eps);
-                    adam1_r1(w.z, m.z, vv.z, cg * who[v].z, alpha, omb1, omb2, eps);
-                    adam1_r1(w.w, m.w, vv.w, cg * who[v].w, alpha, omb1, omb2, eps);
+                    adam1(w.x, m.x, vv.x, cg * who[v].x, alpha, omb1, omb2, eps);
+                    adam1(w.y, m.y, vv.y, cg * who[v].y, alpha, omb1, omb2, eps);
+                    adam1(w.z, m.z, vv.z, cg * who[v].z, alpha, omb1, omb2, eps);
+                    adam1(w.w, m.w, vv.w, cg * who[v].w, alpha, omb1, omb2, eps);
                     m4[v * 32] = m; v4[v * 32] = vv;
                     w4[v * 32] = w;
                 } else if (cg != 0.f) {
@@ -210,7 +193,7 @@ r1_update_kernel(float *__restrict__ W_ih, float *__restrict__ M, float *__restr
                 if (cg != 0.f) my[d] += cg * x;            // lane-owned element of the warp's row
                 if (OPT == G2V_OPT_ADAM_TF1) {
                     float m = M[(size_t)g * D + d], vv = Vv[(size_t)g * D + d];
-                    adam1_r1(x, m, vv, cg * __ldg(W_ho + d), alpha, omb1, omb2, eps);
+                    adam1(x, m, vv, cg * __ldg(W_ho + d), alpha, omb1, omb2, eps);
                     M[(size_t)g * D + d] = m; Vv[(size_t)g * D + d] = vv;
                 } else {
                     x -= alpha * cg * __ldg(W_ho + d);
@@ -225,7 +208,7 @@ r1_update_kernel(float *__restrict__ W_ih, float *__restrict__ M, float *__restr
     for (int i = threadIdx.x; i < D; i += blockDim.x) {
         float x = 0.f;
 #pragma unroll
-        for (int w = 0; w < kR1Warps; ++w) x += sh_gho[(size_t)w * D + i];
+        for (int w = 0; w < kCbowWarps; ++w) x += sh_gho[(size_t)w * D + i];
         g_part[(size_t)blockIdx.x * D + i] = x;
     }
 }
@@ -254,27 +237,13 @@ r1_update_ho_kernel(float *__restrict__ W_ho, float *__restrict__ m, float *__re
         float w = W_ho[i];
         if (OPT == G2V_OPT_ADAM_TF1) {
             float mm = m[i], vv = v[i];
-            adam1_r1(w, mm, vv, g, alpha, omb1, omb2, eps);
+            adam1(w, mm, vv, g, alpha, omb1, omb2, eps);
             m[i] = mm; v[i] = vv;
         } else {
             w -= alpha * g;
         }
         W_ho[i] = w;
     }
-}
-
-static int r1_grid(const void *kernel, size_t smem, int64_t items, int *grid_out) {
-    DeviceProps dp;
-    if (device_props(&dp)) return 1;
-    if (dp.cc_major != 9) { set_error("needs an sm_90 device (found sm_%d%d); no CPU fallback", dp.cc_major, dp.cc_minor); return 2; }
-    int per_sm = 0;
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kR1Warps * 32, smem);
-    if (e != cudaSuccess || per_sm <= 0) { set_error("occupancy query failed: %s", cudaGetErrorString(e)); return 1; }
-    int64_t grid = (int64_t)dp.sm_count * per_sm;
-    const int64_t need = (items + kR1Warps - 1) / kR1Warps;
-    if (grid > need) grid = need;
-    *grid_out = (int)(grid > 0 ? grid : 1);
-    return 0;
 }
 
 }  // namespace g2v
@@ -285,8 +254,8 @@ extern "C" int g2v_cbow_r1_prepare(const float *W_ih, const float *W_ho, float *
                                    void *stream) {
     G2V_REQUIRE(V > 0 && D > 0 && W_ih && W_ho && s, "g2v_cbow_r1_prepare: bad arguments");
     int grid = 0, rc;
-    if ((rc = r1_grid((const void *)r1_prepare_kernel, 0, V, &grid))) return rc;
-    r1_prepare_kernel<<<grid, kR1Warps * 32, 0, (cudaStream_t)stream>>>(W_ih, W_ho, s, V, D, loop_skip_flag());
+    if ((rc = rows_grid((const void *)r1_prepare_kernel, 0, V, &grid))) return rc;
+    r1_prepare_kernel<<<grid, kCbowWarps * 32, 0, (cudaStream_t)stream>>>(W_ih, W_ho, s, V, D, loop_skip_flag());
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;
@@ -304,13 +273,13 @@ extern "C" int g2v_cbow_r1_windows(const int32_t *rowptr, const int32_t *gene, c
     int grid = 0, rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (c) {
-        if ((rc = r1_grid((const void *)r1_windows_kernel<1>, 0, (n_win + 3) / 4, &grid))) return rc;
-        r1_windows_kernel<1><<<grid, kR1Warps * 32, 0, st>>>(rowptr, gene, label, win, win_begin, n_win,
-                                                            inv_n_total, s, c, loss_sum, nc, reduce, loop_skip_flag());
+        if ((rc = rows_grid((const void *)r1_windows_kernel<1>, 0, (n_win + 3) / 4, &grid))) return rc;
+        r1_windows_kernel<1><<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, win_begin, n_win,
+                                                              inv_n_total, s, c, loss_sum, nc, reduce, loop_skip_flag());
     } else {
-        if ((rc = r1_grid((const void *)r1_windows_kernel<0>, 0, (n_win + 3) / 4, &grid))) return rc;
-        r1_windows_kernel<0><<<grid, kR1Warps * 32, 0, st>>>(rowptr, gene, label, win, win_begin, n_win, 0.f,
-                                                            s, nullptr, nullptr, nc, reduce, loop_skip_flag());
+        if ((rc = rows_grid((const void *)r1_windows_kernel<0>, 0, (n_win + 3) / 4, &grid))) return rc;
+        r1_windows_kernel<0><<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, win_begin, n_win, 0.f,
+                                                              s, nullptr, nullptr, nc, reduce, loop_skip_flag());
     }
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
@@ -329,12 +298,12 @@ extern "C" int g2v_cbow_r1_windows_csc(const int32_t *rowptr, const int32_t *gen
     unsigned long long *nc = reinterpret_cast<unsigned long long *>(n_correct);
     int grid = 0, rc;
     cudaStream_t st = (cudaStream_t)stream;
-    if ((rc = r1_grid((const void *)r1_windows_kernel<2>, 0, (n_win + 3) / 4, &grid))) return rc;
-    r1_windows_kernel<2><<<grid, kR1Warps * 32, 0, st>>>(rowptr, gene, label, win, 0, n_win, inv_n_total, s, dO,
-                                                        loss_sum, nc, reduce, loop_skip_flag());
+    if ((rc = rows_grid((const void *)r1_windows_kernel<2>, 0, (n_win + 3) / 4, &grid))) return rc;
+    r1_windows_kernel<2><<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, 0, n_win, inv_n_total, s, dO,
+                                                          loss_sum, nc, reduce, loop_skip_flag());
     G2V_CUDA_OK(cudaGetLastError());
-    if ((rc = r1_grid((const void *)r1_csc_reduce_kernel, 0, V, &grid))) return rc;
-    r1_csc_reduce_kernel<<<grid, kR1Warps * 32, 0, st>>>(cscptr, csc_pos, dO, c, V, loop_skip_flag());
+    if ((rc = rows_grid((const void *)r1_csc_reduce_kernel, 0, V, &grid))) return rc;
+    r1_csc_reduce_kernel<<<grid, kCbowWarps * 32, 0, st>>>(cscptr, csc_pos, dO, c, V, loop_skip_flag());
     G2V_CUDA_OK(cudaGetLastError());
     count_launch(2);
     return 0;
@@ -346,17 +315,17 @@ template <int VEC, int OPT>
 static int launch_r1_update(float *W_ih, float *M, float *Vv, const float *W_ho, float *c, float *g_ho, int32_t V,
                             int32_t D, float alpha, float omb1, float omb2, float eps, const float *alpha_dev,
                             cudaStream_t st, int *grid_out) {
-    const size_t smem = (size_t)kR1Warps * D * sizeof(float);
+    const size_t smem = (size_t)kCbowWarps * D * sizeof(float);
     DeviceProps dp;
     if (device_props(&dp)) return 1;
     G2V_REQUIRE(smem <= (size_t)dp.max_smem_optin, "sizeHiddenlayer %d too large", D);
     if (smem > 48 * 1024)
         G2V_CUDA_OK(cudaFuncSetAttribute(r1_update_kernel<VEC, OPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int grid = 0, rc;
-    if ((rc = r1_grid((const void *)r1_update_kernel<VEC, OPT>, smem, V, &grid))) return rc;
+    if ((rc = rows_grid((const void *)r1_update_kernel<VEC, OPT>, smem, V, &grid))) return rc;
     if (grid > kR1MaxParts) grid = kR1MaxParts;
-    r1_update_kernel<VEC, OPT><<<grid, kR1Warps * 32, smem, st>>>(W_ih, M, Vv, W_ho, c, g_ho, V, D, alpha, omb1, omb2, eps,
-                                                                  alpha_dev, loop_skip_flag());
+    r1_update_kernel<VEC, OPT><<<grid, kCbowWarps * 32, smem, st>>>(W_ih, M, Vv, W_ho, c, g_ho, V, D, alpha, omb1, omb2, eps,
+                                                                    alpha_dev, loop_skip_flag());
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     *grid_out = grid;
@@ -377,9 +346,7 @@ extern "C" int g2v_cbow_r1_update(float *W_ih, float *W_ho, float *m_ih, float *
     cudaStream_t st = (cudaStream_t)stream;
     float alpha = lr, omb1 = 0.f, omb2 = 0.f;
     if (optimizer == G2V_OPT_ADAM_TF1) {
-        float b1p = 1.f, b2p = 1.f;
-        for (int i = 0; i < t; ++i) { b1p *= beta1; b2p *= beta2; }
-        alpha = lr * sqrtf(1.f - b2p) / (1.f - b1p);
+        alpha = adam_tf1_alpha(lr, beta1, beta2, t);
         omb1 = 1.f - beta1; omb2 = 1.f - beta2;
     }
     int rc, parts = 0;

@@ -29,8 +29,6 @@
 
 namespace g2v {
 
-constexpr bool kDefaultSlabScatterTma = false;   // RED.128 scatter; G2V_CBOW_SLAB_SCATTER=tma selects the bulk reduction
-
 __device__ __forceinline__ float4 ld_stream4(const float4 *p) { return __ldcs(p); }
 __device__ __forceinline__ void st_stream4(float4 *p, float4 v) { __stcs(p, v); }
 
@@ -157,47 +155,23 @@ cbow_slab_fwd_kernel(const int32_t *__restrict__ gene, const uint8_t *__restrict
         }
     }
 
-    if (TRAIN && LAST) {
-#pragma unroll
-        for (int v = 0; v < VEC; ++v) {
-            float *p = sh_gho + (v * 32 + lane) * 4;
-            atomicAdd(p + 0, gho[v].x); atomicAdd(p + 1, gho[v].y);
-            atomicAdd(p + 2, gho[v].z); atomicAdd(p + 3, gho[v].w);
-        }
-    }
-    if (LAST && lane == 0) {
-        if (TRAIN) atomicAdd(&sh_acc.loss, (double)loss_acc);
-        atomicAdd(&sh_acc.correct, (unsigned long long)correct_acc);
-    }
-    __syncthreads();
-    if (TRAIN && LAST) for (int i = threadIdx.x; i < D; i += blockDim.x) atomicAdd(g_ho + i, sh_gho[i]);
-    if (LAST && threadIdx.x == 0) {
-        if (TRAIN && loss_sum) atomicAdd(loss_sum, sh_acc.loss);
-        if (n_correct) atomicAdd(n_correct, sh_acc.correct);
-    }
+    cta_epilogue<VEC, TRAIN, LAST>(sh_gho, sh_acc, gho, loss_acc, correct_acc, lane, g_ho, loss_sum, n_correct);
 }
 
-// TMA = false: every lane adds its 16 bytes of the gradient row with red.global.add.v4.f32 (LSU/L1TEX path:
-// VEC warp-wide RED.128 per gene row).  TMA = true: the row dO*W_ho -- the same for every gene of the
-// window -- is staged once in shared memory and added into g_ih[gene,:] with ONE bulk reduction per gene
-// (cp.reduce.async.bulk.global.shared::cta.add.f32, D*4 bytes, SASS UBLKRED) issued by one lane: the scatter
-// leaves the LSU/L1TEX path, which is what bounds the L2-resident backward passes.
-// Two staging rows per warp, so that a window's row can be written while the previous window's bulk
-// reductions are still reading theirs.
-template <int VEC, bool TMA>
+// The scatter of cbow_rows_kernel over the window's genes in slab s: every lane adds its 16 bytes of the gradient row
+// dO*W_ho with red.global.add.v4.f32 (VEC warp-wide RED.128 per gene row).
+template <int VEC>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 cbow_slab_bwd_kernel(const int32_t *__restrict__ gene, int64_t n_win, const int32_t *__restrict__ slabptr, int32_t S1,
                      int32_t s, const float *__restrict__ dOut, const float *__restrict__ W_ho,
                      float *__restrict__ g_ih, const int32_t *__restrict__ skip) {
     G2V_SKIP_IF_STOPPED(skip);
     constexpr int D = 128 * VEC;
-    __shared__ __align__(128) float sh_row[TMA ? kCbowWarps * 2 * D : 4];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float4 who[VEC];
 #pragma unroll
     for (int v = 0; v < VEC; ++v) who[v] = ldg4(reinterpret_cast<const float4 *>(W_ho) + v * 32 + lane);
     const int64_t warps_total = (int64_t)gridDim.x * kCbowWarps;
-    int stage = 0;
     for (int64_t i = (int64_t)blockIdx.x * kCbowWarps + warp; i < n_win; i += warps_total) {
         const int32_t b = __ldg(slabptr + i * S1 + s), e = __ldg(slabptr + i * S1 + s + 1);
         if (b == e) continue;
@@ -205,38 +179,17 @@ cbow_slab_bwd_kernel(const int32_t *__restrict__ gene, int64_t n_win, const int3
         float4 gv[VEC];
 #pragma unroll
         for (int v = 0; v < VEC; ++v) gv[v] = make_float4(who[v].x * hs, who[v].y * hs, who[v].z * hs, who[v].w * hs);
-        if (TMA) {
-            float *row = sh_row + (size_t)(warp * 2 + stage) * D;
-            // at most one older group (the other stage) may still be reading shared memory
-            asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-            __syncwarp();
+        for (int32_t base = b; base < e; base += 32) {
+            const int cnt = min(32, e - base);
+            const int32_t g = (lane < cnt) ? __ldg(gene + base + lane) : 0;
+            for (int k = 0; k < cnt; ++k) {
+                const int32_t gk = __shfl_sync(0xffffffffu, g, k);
+                float *dst = g_ih + (size_t)gk * D + lane * 4;
 #pragma unroll
-            for (int v = 0; v < VEC; ++v) reinterpret_cast<float4 *>(row)[v * 32 + lane] = gv[v];
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy
-            __syncwarp();
-            const uint32_t src = (uint32_t)__cvta_generic_to_shared(row);
-            for (int32_t j = b + lane; j < e; j += 32) {
-                float *dst = g_ih + (size_t)__ldg(gene + j) * D;
-                asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;"
-                             ::"l"(dst), "r"(src), "n"(D * 4)
-                             : "memory");
-            }
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            stage ^= 1;
-        } else {
-            for (int32_t base = b; base < e; base += 32) {
-                const int cnt = min(32, e - base);
-                const int32_t g = (lane < cnt) ? __ldg(gene + base + lane) : 0;
-                for (int k = 0; k < cnt; ++k) {
-                    const int32_t gk = __shfl_sync(0xffffffffu, g, k);
-                    float *dst = g_ih + (size_t)gk * D + lane * 4;
-#pragma unroll
-                    for (int v = 0; v < VEC; ++v) red_add4(dst + v * 128, gv[v]);
-                }
+                for (int v = 0; v < VEC; ++v) red_add4(dst + v * 128, gv[v]);
             }
         }
     }
-    if (TMA) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 struct SlabLayout {            // carving of the caller's workspace
@@ -295,9 +248,7 @@ static int launch_fwd_passes(const int32_t *gene, const uint8_t *label, const in
 template <int VEC>
 static int launch_bwd_passes(const int32_t *gene, int64_t n_win, const SlabLayout &l, int32_t S, const float *W_ho,
                              float *g_ih, cudaStream_t st) {
-    const char *sc = getenv("G2V_CBOW_SLAB_SCATTER");             // "tma" / "red" (default): A/B hook
-    const bool tma = sc ? sc[0] == 't' : kDefaultSlabScatterTma;
-    auto kern = tma ? cbow_slab_bwd_kernel<VEC, true> : cbow_slab_bwd_kernel<VEC, false>;
+    auto kern = cbow_slab_bwd_kernel<VEC>;
     int grid = 0, rc;
     if ((rc = rows_grid((const void *)kern, 0, n_win, &grid))) return rc;
     for (int s = 0; s < S; ++s) {
@@ -328,8 +279,7 @@ extern "C" int g2v_cbow_slab_plan(int32_t V, int32_t D, int32_t *n_slabs) {
     // one BACKWARD slab of g_ih is a quarter of the L2, so that a forward group (G2V_CBOW_SLAB_FWD_GROUP = 2 slabs of
     // W_ih) stays resident with room for the streamed window data: 12.5 MiB on H100 (measured on the 200k x 512 table:
     // 55.8 ms per fwd+bwd in 32 slabs, 56.6 ms in 13 slabs of 32 MiB, 55.1 ms in 25 of 16 MiB)
-    const char *e = getenv("G2V_CBOW_SLAB_MB");                   // tuning hook: slab size in MiB
-    const double slab = e && atof(e) > 0 ? atof(e) * 1048576.0 : 0.25 * (double)dp.l2_bytes;
+    const double slab = 0.25 * (double)dp.l2_bytes;
     const char *f = getenv("G2V_CBOW_SLABS");                     // force a slab count (tests)
     if (f && atoi(f) >= 1) { *n_slabs = atoi(f) > V ? V : atoi(f); return 0; }
     if (table <= 0.9 * (double)dp.l2_bytes) return 0;

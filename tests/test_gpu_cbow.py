@@ -335,22 +335,6 @@ def test_minibatch_variant_and_dense_adapter(g2v):
     assert lines[0].strip() == "Start training the modified CBOW with early stopping"
 
 
-@pytest.mark.parametrize("gather,scatter", [("tma", "red"), ("ldg", "tma"), ("tma", "tma")])
-@pytest.mark.parametrize("D", [128, 256, 512])
-def test_tma_staged_variants_equal_oracle(g2v, monkeypatch, gather, scatter, D):
-    """The TMA-staged forms of the fused kernel (bulk-copy gather through shared memory, bulk-reduce
-    scatter) compute the same step; which one ships is decided by measurement."""
-    monkeypatch.setenv("G2V_CBOW_GATHER", gather)
-    monkeypatch.setenv("G2V_CBOW_SCATTER", scatter)
-    V, N = 400, 2500
-    rowptr, gene, label = helpers.random_windows(N, V, 1, 80, seed=D + 7)
-    m, W0, Wo0, g_ih, g_ho, loss, nc = one_step(g2v, rowptr, gene, label, V, D)
-    win = np.arange(N, dtype=np.int64)
-    o_gih, o_gho, o_loss, o_nc = oracle.cbow_grad(rowptr, gene, label, win, N, W0, Wo0)
-    assert rel_max(g_ih, o_gih) < 2e-5 and rel_max(g_ho, o_gho) < 2e-5
-    assert abs(loss / N - o_loss) < 1e-5 * max(1.0, abs(o_loss)) and abs(nc - o_nc) <= 2
-
-
 def test_rank1_csc_backward_is_bit_reproducible(g2v):
     """With the transposed incidence (CSC) the collapsed trainer has no floating-point atomics: two runs
     give bit-identical vectors (the row formulation, with red.global.add, does not promise that)."""
