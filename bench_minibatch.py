@@ -14,6 +14,13 @@ its roofline_hbm block (200k genes x 512, synthetic windows of 80 distinct genes
 the per-step time of both optimizers, the mean number of distinct genes per batch and the byte model of both steps
 (minibatch_bytes, computed from shapes, not measured).
 
+Reshuffled epochs (DESIGN.md §4.12), per B, over the whole training list: order_ms (g2v_cbow_epoch_order), plan_ms
+(g2v_cbow_batch_plan plus the read-back of the per-batch row offsets, as prepare_batches runs it), sort_plan_ms (a
+stand-in for the earlier prepare_batches: its torch.sort construction, tests/reshuffle_oracle.batch_plan_torch, on the
+same list, without its per-batch dict loop), and epoch_ms / epoch_reshuffle_ms: one whole lazy_adam epoch over the training list without and with the new
+order and the plan rebuild (CUDA events, after one warm-up epoch, no L2 flush).  plan_bytes is the builder's byte model
+(batch_plan_bytes, from shapes).
+
 Timing: CUDA events on the launching stream, W warm-up steps, L2 flushed (256 MiB write) before every timed step,
 cycling over the first (at most 32) batches of the training list.  Prints one JSON line; writes nothing.
 """
@@ -42,6 +49,14 @@ def minibatch_bytes(V, D, n_win, nnz, T):
     dense = nnz * (8 * D + 4) + 5 * n_win + 32 * V * D
     lazy = nnz * (4 * D + 12) + 9 * n_win + 24 * D * T
     return {"adam": int(dense), "lazy_adam": int(lazy)}
+
+
+def batch_plan_bytes(V, n_win, nnz, n_b, T_sum):
+    """Algorithmic bytes of g2v_cbow_batch_plan over n_win windows with nnz incidences in n_b batches touching T_sum
+    (batch, gene) rows: two passes over the windows (win + rowptr 12 B per window, gene + counter atomic 8 B per
+    incidence, plus the 4 B scatter of the position), the segment sort (read 4 + write 4 per incidence), the counters
+    (zero, tile sums, emit read, cursor write: 16 B per (batch, gene)) and rows + segptr (8 B per touched row)."""
+    return int(2 * 12 * n_win + nnz * (8 + 12) + 16 * n_b * V + 8 * T_sum)
 
 
 def parse(argv=None):
@@ -98,6 +113,55 @@ def run(args):
         torch.cuda.synchronize()
         return [a.elapsed_time(b) for a, b in pairs]
 
+    def reshuffle_fields(rowptr, gene, label, tr, V, D, W0, Wo0, B, r):
+        """order_ms, plan_ms, sort_plan_ms, epoch_ms, epoch_reshuffle_ms over the whole training list tr."""
+        from tests.reshuffle_oracle import batch_plan_torch
+        n = int(tr.shape[0])
+        m = g2v.CbowModel(rowptr, gene, label, V, D, W0, Wo0, optimizer="lazy_adam", lr=0.005)
+        ep = torch.empty_like(tr)
+        m.prepare_batches(tr, B)
+        n_b = -(-n // B)
+
+        def host(fn, k):
+            ts = []
+            for _ in range(k):
+                torch.cuda.synchronize()
+                a, b = ev(), ev()
+                a.record(); fn(); b.record()
+                torch.cuda.synchronize()
+                ts.append(a.elapsed_time(b))
+            return ts
+        order = lambda: cbow.epoch_order(tr, 0, 1, out=ep)
+        host(order, 2)
+        r["order_ms"] = float(np.median(host(order, args.steps)))
+        plan = lambda: m.prepare_batches(ep, B)
+        host(plan, 2)
+        r["plan_ms"] = float(np.median(host(plan, args.steps)))
+        srt = lambda: batch_plan_torch(m.rowptr, m.gene, V, ep, B)
+        host(srt, 2)
+        r["sort_plan_ms"] = float(np.median(host(srt, args.steps)))
+        keys = [(ep.data_ptr(), k * B, min(B, n - k * B)) for k in range(n_b)]
+        r["plan_bytes"] = batch_plan_bytes(V, n, int(m._plan_bufs[(ep.data_ptr(), n, B)].nnz), n_b,
+                                           sum(m._batches[k][2] for k in keys))
+
+        def epoch(reshuffle, e=[1]):
+            win = tr
+            if reshuffle:
+                e[0] += 1
+                cbow.epoch_order(tr, 0, e[0], out=ep)
+                m.prepare_batches(ep, B)
+                win = ep
+            for lo in range(0, n, B):
+                nb = min(B, n - lo)
+                m.fwdbwd(win, nb, win_begin=lo, n_win=nb)
+                m.update()
+        for flag, name in ((False, "epoch_ms"), (True, "epoch_reshuffle_ms")):
+            host(lambda: epoch(flag), 1)
+            r[name] = float(np.median(host(lambda: epoch(flag), 3)))
+        r["reshuffle_overhead"] = r["epoch_reshuffle_ms"] / r["epoch_ms"] - 1.0
+        del m, ep
+        torch.cuda.empty_cache()
+
     def block(rowptr, gene, label, tr, V, D, W0, Wo0, desc):
         lens = (rowptr[1:] - rowptr[:-1]).to(torch.int64)
         out = {"config": desc, "windows_train": int(tr.shape[0])}
@@ -126,6 +190,7 @@ def run(args):
             r["lazy_speedup"] = r["adam_ms"] / r["lazy_adam_ms"]
             r["bytes_model"] = minibatch_bytes(V, D, B, nnz, r["mean_touched_genes"])
             r["touched_model"] = expected_touched(V, B, nnz / B)
+            reshuffle_fields(rowptr, gene, label, tr, V, D, W0, Wo0, B, r)
             out["B%d" % B] = r
         return out
 

@@ -35,6 +35,9 @@ SIGNATURES = {
                                        _vp]),
     "g2v_cbow_lazy_adam": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32,
                                           _f32, _f32, _f32, _i32, _vp, _vp]),
+    "g2v_cbow_epoch_order": (ctypes.c_int, [_vp, _i64, _u64, _i32, _i64, _i64, _vp, _vp]),
+    "g2v_cbow_batch_plan_workspace_bytes": (ctypes.c_size_t, [_i64, _i64, _i64, _i32]),
+    "g2v_cbow_batch_plan": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "g2v_cbow_update": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _f32,
                                        _f32, _f32, _i32, _vp, _vp]),
     "g2v_cbow_update_nvl": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f32, _f32, _f32,

@@ -91,7 +91,7 @@ class CbowModel:
         # lazy_adam: TF1 LazyAdam -- only the rows a batch gathered are updated, fused with their per-gene dO sums
         # (g2v_cbow_fwd_do + g2v_cbow_lazy_adam over the batches of prepare_batches); no g_ih is allocated
         self.lazy = optimizer == "lazy_adam"
-        self._batches, self._pending, self._dO = {}, None, None
+        self._batches, self._pending, self._dO, self._plan_bufs = {}, None, None, {}
         if algo == "rows" and nvl_group is not None:
             self.nvl = _nvl_setup(nvl_group, n_flat, dev)
         if algo == "rows":
@@ -166,34 +166,31 @@ class CbowModel:
 
     def prepare_batches(self, win, batch):
         """lazy_adam: cut the window list ``win`` (int32 device tensor) into consecutive batches of ``batch`` windows
-        (the last one shorter) and record, once, for every batch the ascending genes it gathers, their segment
-        pointers and their positions relative to the batch start -- the transposed incidence of each batch, O(nnz +
-        sum of touched genes) in all.  fwdbwd(win, n, win_begin=lo, n_win=nb) then finds batch [lo, lo + nb)."""
+        (the last one shorter) and record for every batch the ascending genes it gathers, their segment pointers and
+        their positions relative to the batch start -- the transposed incidence of each batch, O(nnz + sum of touched
+        genes) in all, built on the device by g2v_cbow_batch_plan.  fwdbwd(win, n, win_begin=lo, n_win=nb) then finds
+        batch [lo, lo + nb).  A list has one plan at a time: calling it again for the same list (rewritten in place,
+        as a reshuffled epoch is, or with another batch size) replaces the list's plan and releases the buffers of a
+        previous batch size.  The buffers are allocated on the first call for a (list, batch size) only, and each
+        call reads the per-batch row offsets back once."""
         n = int(win.shape[0])
         B = min(int(batch), n) if batch > 0 else n
         if n == 0:
             return
-        w = win.to(torch.int64)
-        starts = self.rowptr[w].to(torch.int64)
-        lens = self.rowptr[w + 1].to(torch.int64) - starts
-        total = int(lens.sum())
-        pos = torch.repeat_interleave(torch.arange(n, device=self.device), lens)
-        first = torch.cumsum(lens, 0) - lens
-        idx = starts[pos] + (torch.arange(total, device=self.device) - first[pos])
-        b = pos // B
-        key, order = torch.sort(b * self.V + self.gene[idx].to(torch.int64), stable=True)   # (batch, gene, position)
-        rel = (pos - b * B)[order].to(torch.int32)
-        head = torch.ones(total, dtype=torch.bool, device=self.device)
-        head[1:] = key[1:] != key[:-1]
-        seg = torch.nonzero(head).squeeze(1)
-        rows = (key[seg] % self.V).to(torch.int32)
-        segptr = torch.cat([seg, torch.tensor([total], device=self.device)]).to(torch.int32)
-        n_b = -(-n // B)
-        per = torch.bincount(key[seg] // self.V, minlength=n_b).cpu().numpy()
-        r0 = np.concatenate([[0], np.cumsum(per)[:-1]])
-        data = (win, rows, segptr, rel)                     # keeps `win` alive: its address is part of the key
-        for k in range(n_b):
-            self._batches[(win.data_ptr(), k * B, min(B, n - k * B))] = (data, int(r0[k]), int(per[k]))
+        ptr = win.data_ptr()
+        for k in [k for k in self._batches if k[0] == ptr]:
+            del self._batches[k]
+        key = (ptr, n, B)
+        for k in [k for k in self._plan_bufs if k[0] == ptr and k != key]:
+            del self._plan_bufs[k]
+        buf = self._plan_bufs.get(key)
+        if buf is None:
+            buf = _PlanBuffers(self, win, B)
+            self._plan_bufs[key] = buf
+        rows, segptr, pos, brp = buf.build(win)
+        data = (win, rows, segptr, pos)                     # keeps `win` alive: its address is part of the key
+        for k in range(brp.shape[0] - 1):
+            self._batches[(ptr, k * B, min(B, n - k * B))] = (data, int(brp[k]), int(brp[k + 1] - brp[k]))
         if self._dO is None or self._dO.shape[0] < B:
             self._dO = torch.empty(B, dtype=torch.float32, device=self.device)
         self._pending = None
@@ -421,6 +418,67 @@ def _nvl_setup(group, n_flat, dev):
         return None
 
 
+class _PlanBuffers:
+    """Outputs and workspace of g2v_cbow_batch_plan for one window list of a CbowModel (n windows, batches of B),
+    sized once from the list's incidence count, which no reordering of the list changes."""
+
+    def __init__(self, model, win, B):
+        self.m, self.win, self.n, self.B = model, win, int(win.shape[0]), int(B)
+        w = win.to(torch.int64)
+        self.nnz = int((model.rowptr[w + 1] - model.rowptr[w]).sum())
+        dev, i32 = model.device, torch.int32
+        self.n_b = -(-self.n // self.B)
+        self.rows = torch.empty(max(self.nnz, 1), dtype=i32, device=dev)
+        self.segptr = torch.empty(self.nnz + 1, dtype=i32, device=dev)
+        self.pos = torch.empty(max(self.nnz, 1), dtype=i32, device=dev)
+        self.brp = torch.empty(self.n_b + 1, dtype=i32, device=dev)
+        nbytes = int(model.lib.g2v_cbow_batch_plan_workspace_bytes(self.n, self.nnz, self.B, model.V))
+        self.ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+
+    def launch(self, win):
+        """Enqueue the build for ``win`` (same length as the list this was sized for); no host synchronisation."""
+        m = self.m
+        _capi.check(m.lib.g2v_cbow_batch_plan(m.rowptr.data_ptr(), m.gene.data_ptr(), win.data_ptr(), self.n, self.nnz,
+                                              self.B, m.V, self.rows.data_ptr(), self.segptr.data_ptr(),
+                                              self.pos.data_ptr(), self.brp.data_ptr(), self.ws.data_ptr(),
+                                              m._stream()), "g2v_cbow_batch_plan")
+
+    def build(self, win):
+        """launch(win), then read the per-batch row offsets back (the only host synchronisation); returns (rows,
+        segptr, pos) cut to their sizes and the row offsets as int64 NumPy [n_b + 1]."""
+        self.launch(win)
+        brp = self.brp.cpu().numpy().astype(np.int64)
+        if brp[-1] < 0:
+            raise RuntimeError("g2v_cbow_batch_plan: the list has more incidences than it was sized for")
+        S = int(brp[-1])
+        return self.rows[:S], self.segptr[:S + 1], self.pos[:self.nnz], brp
+
+
+def batch_plan(model, win, batch):
+    """The transposed incidence of every batch of ``batch`` consecutive windows of ``win`` (int32 device tensor), as
+    device tensors (rows, segptr, pos, batch_rowptr) -- what prepare_batches records (g2v_cbow_batch_plan)."""
+    n = int(win.shape[0])
+    B = min(int(batch), n) if batch > 0 else n
+    rows, segptr, pos, brp = _PlanBuffers(model, win, B).build(win)
+    return rows, segptr, pos, torch.from_numpy(brp.astype(np.int32)).to(model.device)
+
+
+def epoch_order(tr, seed, epoch, rank=0, world=1, out=None):
+    """Rank ``rank``'s share of epoch ``epoch``'s list: out[i] = tr[P(rank + i*world)], P = P(seed, epoch, len(tr)) the
+    pseudo-random permutation of DESIGN.md §4.12 (g2v_cbow_epoch_order).  ``tr``: int32 device tensor."""
+    n = int(tr.shape[0])
+    n_loc = max(0, -(-(n - rank) // world))
+    if out is None:
+        out = torch.empty(n_loc, dtype=torch.int32, device=tr.device)
+    if out.shape[0] != n_loc or out.dtype != torch.int32:
+        raise ValueError("epoch_order: out must be int32 [%d]" % n_loc)
+    lib = _capi.load()
+    _capi.check(lib.g2v_cbow_epoch_order(tr.data_ptr(), n, int(seed) & 0xFFFFFFFFFFFFFFFF, int(epoch), int(rank),
+                                         int(world), out.data_ptr(),
+                                         torch.cuda.current_stream(tr.device).cuda_stream), "g2v_cbow_epoch_order")
+    return out
+
+
 class WindowFeeder:
     """Feeds a CbowModel's context windows from pinned host memory, double-buffered.
 
@@ -479,7 +537,7 @@ def _dist():
 
 def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500, seed=0, optimizer="adam",
                reduce="sum", W_ih0=None, W_ho0=None, split=None, early_stop=True, log=print, return_info=False,
-               eval_train="lazy", algo="rows", batch=0, use_graph=True):
+               eval_train="lazy", algo="rows", batch=0, use_graph=True, reshuffle=False):
     """Train the modified CBOW on CSR windows and return W_ih (np.float32 [n_genes, hidden]) exactly as
     ``compute_genetovec`` does: the weights after the last step whose validation accuracy did not drop.
 
@@ -500,7 +558,15 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     gathered (dense Adam on W_ho).  Full batch it computes what "adam" computes (rows outside the training list
     keep zero gradient and zero moments); with ``batch`` it is the usual sparse mini-batch embedding update.
     Only with algo="rows", on one GPU.
+
+    ``reshuffle`` (with 0 < ``batch`` < n_train): epoch 0 trains on the split's order, epoch e >= 1 on tr[P(seed, e)],
+    P a pseudo-random permutation of the training list that depends on (seed, e, n_train) only (DESIGN.md §4.12), cut
+    into consecutive batches as before; several GPUs deal the epoch's list as they deal the split's.  The order is
+    written on the device every epoch, and lazy_adam rebuilds its batch plans there.  With ``batch >= n_train`` (full
+    batch) the flag has no effect; with ``batch <= 0`` it is an error.
     """
+    if reshuffle and batch <= 0:
+        raise ValueError("reshuffle=True needs mini-batches (batch > 0)")
     dist = _dist()
     if optimizer == "lazy_adam" and algo != "rows":
         raise ValueError("optimizer='lazy_adam' needs algo='rows' (rank1 keeps s = W_ih.W_ho, which every W_ho step "
@@ -524,6 +590,10 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     va_loc = shard_by_nnz(np.asarray(va), lens, world, rank)
     dev = model.device
     tr_d = torch.from_numpy(np.ascontiguousarray(tr_loc, dtype=np.int32)).to(dev)
+    reshuffle = bool(reshuffle) and not full_batch
+    tr_all = None
+    if reshuffle:                                # every rank deals each epoch's list from the global training list
+        tr_all = tr_d if world == 1 else torch.from_numpy(np.ascontiguousarray(tr, dtype=np.int32)).to(dev)
     va_d = torch.from_numpy(np.ascontiguousarray(va_loc, dtype=np.int32)).to(dev)
 
     slabs = False
@@ -543,7 +613,8 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
                                        early_stop, log, eval_train, use_graph)
     else:
         out, hist, stop = _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, len(tr_loc), len(va_loc),
-                                          max_epoch, early_stop, log, batch)
+                                          max_epoch, early_stop, log, batch,
+                                          reshuffle=(tr_all, seed, rank) if reshuffle else None)
     if log:
         log("    Optimization Finish")
     out = out.cpu().numpy()
@@ -775,15 +846,27 @@ def _device_loop(model, dist, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_ep
     return (loop.result if stop is not None else model.W_ih), info.hist, stop
 
 
-def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_epoch, early_stop, log, batch):
+def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_epoch, early_stop, log, batch,
+                    reshuffle=None):
     """north_star's mini-batch variant: one optimizer step (and one gradient all-reduce) per batch of the shuffled
-    training list, the reference's per-epoch accuracies and early stop around it; host-driven, one sync per epoch."""
+    training list, the reference's per-epoch accuracies and early stop around it; host-driven, one sync per epoch.
+    ``reshuffle`` = (global training list on the device, seed, rank): every epoch e >= 1 trains on this rank's share of
+    the epoch's order, written into one preallocated buffer (g2v_cbow_epoch_order); lazy_adam then rebuilds the
+    buffer's batch plans (one more sync)."""
     dev = model.device
     info = _LoopLog(n_tr, n_va, log)
     result = model.W_ih.clone()
     stop = None
     per = -(-batch // world)
+    ep_d = torch.empty_like(tr_d) if reshuffle else None
     for step in range(max_epoch):
+        win = tr_d
+        if reshuffle and step >= 1:
+            tr_all, seed, rank = reshuffle
+            epoch_order(tr_all, seed, step, rank, world, out=ep_d)
+            if model.lazy:
+                model.prepare_batches(ep_d, batch)
+            win = ep_d
         model.acc.zero_()
         for lo in range(0, -(-n_tr // world), per):             # same trip count on every rank (collectives inside)
             nb = max(0, min(per, n_tr_loc - lo))
@@ -791,7 +874,7 @@ def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_l
             if dist:
                 t_nb = torch.tensor([nb], dtype=torch.int64, device=dev); dist.all_reduce(t_nb)
                 nb_tot = int(t_nb[0])
-            model.fwdbwd(tr_d, nb_tot, win_begin=lo, n_win=nb)
+            model.fwdbwd(win, nb_tot, win_begin=lo, n_win=nb)
             if dist:
                 for g in model.grad_tensors():
                     dist.all_reduce(g)

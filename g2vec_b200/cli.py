@@ -37,7 +37,13 @@ def parse_arguments(argv=None):
     p.add_argument('--optimizer', choices=['adam', 'sgd', 'lazy_adam'], default='adam',
                    help="'adam' = TF1 AdamOptimizer (the reference's), 'sgd', or 'lazy_adam' = TF1 LazyAdam: a step "
                         "updates only the rows of the genes its batch gathered (rows, one GPU)")
-    return p.parse_args(argv)
+    p.add_argument('--reshuffle', action='store_true',
+                   help="with --batch: train every epoch after the first on a new pseudo-random order of the training "
+                        "windows (seeded by --seed and the epoch) instead of the same batches every epoch")
+    args = p.parse_args(argv)
+    if args.reshuffle and args.batch <= 0:
+        p.error("--reshuffle needs mini-batches (--batch B with B > 0)")
+    return args
 
 
 # ----------------------------------------------------------------------------------- step 1: I/O
@@ -233,7 +239,7 @@ def main(argv=None):
     print(">>> 4. Compute distributed representations using modified CBOW")
     mat = cbow.train_cbow(w_rowptr, w_gene, w_label, n_genes, args.sizeHiddenlayer, args.learningRate,
                           max_epoch=args.epoch, seed=args.seed, log=print, algo=args.algo,   # print is silent off rank 0
-                          batch=args.batch, optimizer=args.optimizer)
+                          batch=args.batch, optimizer=args.optimizer, reshuffle=args.reshuffle)
     genes = data['gene']
     if rank != 0:
         dist.barrier()

@@ -154,6 +154,25 @@ int g2v_cbow_lazy_adam(const int32_t *rows, const int32_t *segptr, const int32_t
                        float *g_ho, int32_t V, int32_t D, float lr, float beta1, float beta2, float eps, int32_t t,
                        const float *alpha_dev, void *stream);
 
+/* Reshuffled mini-batch epochs (csrc/g2v_cbow_plan.cu, DESIGN.md §4.12).
+ * g2v_cbow_epoch_order: out[i] = tr[P(rank + i*world)] for i < ceil((n - rank) / world): rank `rank`'s share of the
+ *   epoch's list tr[P(0..n-1)].  P = P(seed, epoch, n) is a pseudo-random permutation of [0, n) (a 4-round Feistel
+ *   network with Philox4x32-10 rounds, cycle-walked into [0, n); exact definition in DESIGN.md §4.12).  One launch.
+ * g2v_cbow_batch_plan: the plan g2v_cbow_lazy_adam reads, for every batch k of B consecutive windows of the list
+ *   win[0..n_win-1] (the last one shorter): the ascending distinct genes of the batch, rows[batch_rowptr[k] ..
+ *   batch_rowptr[k+1]); segment pointers segptr (absolute into pos, segptr[S] = nnz, S = batch_rowptr[n_b]); the
+ *   positions of each gene's windows relative to the batch start, ascending inside each segment, in pos.  nnz = the
+ *   number of (window, gene) incidences of the list; rows [nnz], segptr [nnz + 1], pos [nnz], batch_rowptr
+ *   [ceil(n_win / B) + 1]; workspace: g2v_cbow_batch_plan_workspace_bytes(n_win, nnz, B, V) bytes.  If the list has
+ *   more than nnz incidences nothing is written except batch_rowptr[n_b] = -1.  Genes must lie in [0, V).  Never
+ *   synchronises; 7 launches per wave of K = max(1, 2^22 / V) batches. */
+int g2v_cbow_epoch_order(const int32_t *tr, int64_t n, uint64_t seed, int32_t epoch, int64_t rank, int64_t world,
+                         int32_t *out, void *stream);
+size_t g2v_cbow_batch_plan_workspace_bytes(int64_t n_win, int64_t nnz, int64_t B, int32_t V);
+int g2v_cbow_batch_plan(const int32_t *rowptr, const int32_t *gene, const int32_t *win, int64_t n_win, int64_t nnz,
+                        int64_t B, int32_t V, int32_t *rows, int32_t *segptr, int32_t *pos, int32_t *batch_rowptr,
+                        void *workspace, void *stream);
+
 int g2v_cbow_update(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m_ho, float *v_ho,
                     float *g_ih, float *g_ho, int32_t V, int32_t D, int32_t optimizer, float lr,
                     float beta1, float beta2, float eps, int32_t t, const float *alpha_dev, void *stream);
