@@ -8,7 +8,9 @@ One step = fwd + bwd + update of one batch of B consecutive windows of the shuff
 train_cbow(batch=B) launches it:
   adam       g2v_cbow_fwdbwd (scatter backward into g_ih) + g2v_cbow_update (TF1 Adam over all V*D parameters);
   lazy_adam  g2v_cbow_fwd_do (dO per batch position) + g2v_cbow_lazy_adam (per-gene dO sums fused with Adam on the
-             rows the batch gathered, then the W_ho step).
+             rows the batch gathered, then the W_ho step);
+  adam_det   train_cbow(batch=B, deterministic=True) (DESIGN.md §4.13): g2v_cbow_fwd_do_det (tiled forward + fixed-order
+             tile sum) + g2v_cbow_batch_expand (per-gene dO sums over the batch plan into g_ih) + g2v_cbow_update.
 Two workloads: the syn10k windows of bench.py's headline (walks -> windows, 10k genes, hidden 128) and the table of
 its roofline_hbm block (200k genes x 512, synthetic windows of 80 distinct genes, seed 777).  For every B it reports
 the per-step time of both optimizers, the mean number of distinct genes per batch and the byte model of both steps
@@ -172,10 +174,13 @@ def run(args):
             sub = tr[:nb * B].clone()
             nnz = float(lens[sub.to(torch.int64)].sum()) / nb
             r = {"batches": nb, "mean_window_len": nnz / B}
-            for opt in ("adam", "lazy_adam"):
-                m = g2v.CbowModel(rowptr, gene, label, V, D, W0, Wo0, optimizer=opt, lr=0.005)
-                if opt == "lazy_adam":
+            for opt in ("adam", "lazy_adam", "adam_det"):
+                det = opt == "adam_det"
+                m = g2v.CbowModel(rowptr, gene, label, V, D, W0, Wo0, optimizer="adam" if det else opt, lr=0.005,
+                                  deterministic=det)
+                if opt != "adam":
                     m.prepare_batches(sub, B)
+                if opt == "lazy_adam":
                     r["mean_touched_genes"] = float(np.mean([m.batch_touched(sub, k * B, B) for k in range(nb)]))
                 it = [0]
 
@@ -188,6 +193,7 @@ def run(args):
                 del m
                 torch.cuda.empty_cache()
             r["lazy_speedup"] = r["adam_ms"] / r["lazy_adam_ms"]
+            r["det_cost_vs_adam"] = r["adam_det_ms"] / r["adam_ms"]
             r["bytes_model"] = minibatch_bytes(V, D, B, nnz, r["mean_touched_genes"])
             r["touched_model"] = expected_touched(V, B, nnz / B)
             reshuffle_fields(rowptr, gene, label, tr, V, D, W0, Wo0, B, r)

@@ -35,6 +35,14 @@ SIGNATURES = {
                                        _vp]),
     "g2v_cbow_lazy_adam": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _f32,
                                           _f32, _f32, _f32, _i32, _vp, _vp]),
+    "g2v_cbow_det_workspace_bytes": (ctypes.c_size_t, [_i64, _i32]),
+    "g2v_cbow_fwdbwd_csc_det": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                               _vp, _i32, _i32, _i32, _vp, _i32, _vp]),
+    "g2v_cbow_fwd_do_det": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
+                                           _i32, _vp, _i32, _vp]),
+    "g2v_cbow_loop_tail_det": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
+                                              _i32, _vp, _i32, _vp]),
+    "g2v_cbow_batch_expand": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _i32, _i32, _i32, _vp]),
     "g2v_cbow_epoch_order": (ctypes.c_int, [_vp, _i64, _u64, _i32, _i64, _i64, _vp, _vp]),
     "g2v_cbow_batch_plan_workspace_bytes": (ctypes.c_size_t, [_i64, _i64, _i64, _i32]),
     "g2v_cbow_batch_plan": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -62,7 +62,8 @@ class CbowModel:
     """Parameters + optimizer state + scratch in HBM, and the three kernel calls."""
 
     def __init__(self, rowptr, gene, label, n_genes, hidden, W_ih0, W_ho0, optimizer="adam", reduce="sum",
-                 lr=0.005, beta1=0.9, beta2=0.999, eps=1e-8, device=None, algo="rows", nvl_group=None):
+                 lr=0.005, beta1=0.9, beta2=0.999, eps=1e-8, device=None, algo="rows", nvl_group=None,
+                 deterministic=False):
         if not torch.cuda.is_available():
             raise RuntimeError("g2vec_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.lib = _capi.load()
@@ -79,6 +80,8 @@ class CbowModel:
                              "changes for every gene")
         if optimizer == "lazy_adam" and nvl_group is not None:
             raise ValueError("optimizer='lazy_adam' runs on one GPU only")
+        if deterministic and nvl_group is not None:
+            raise ValueError("deterministic=True runs on one GPU only")
         self.rowptr = to(rowptr, torch.int32)
         self.gene = to(gene, torch.int32)
         self.label = to(label, torch.uint8)
@@ -91,6 +94,10 @@ class CbowModel:
         # lazy_adam: TF1 LazyAdam -- only the rows a batch gathered are updated, fused with their per-gene dO sums
         # (g2v_cbow_fwd_do + g2v_cbow_lazy_adam over the batches of prepare_batches); no g_ih is allocated
         self.lazy = optimizer == "lazy_adam"
+        # deterministic (DESIGN.md §4.13): every floating-point sum of a rows step in a fixed order -- the tiled forward
+        # (g2v_cbow_*_det) on a prepared CSC list or batch plan, never the scatter or the gene slabs
+        self.det = bool(deterministic)
+        self._det_ws = None
         self._batches, self._pending, self._dO, self._plan_bufs = {}, None, None, {}
         if algo == "rows" and nvl_group is not None:
             self.nvl = _nvl_setup(nvl_group, n_flat, dev)
@@ -203,7 +210,7 @@ class CbowModel:
         """rows only, tables larger than the L2 (csrc/g2v_cbow_slab.cu): record once, for the static window list
         ``win`` (int32 device tensor or None), where every window's sorted gene list crosses the gene-slab
         boundaries; fwdbwd()/evaluate() over exactly this list then run slab by slab, L2-resident."""
-        if self.algo != "rows":
+        if self.algo != "rows" or self.det:
             return False
         import ctypes
         if not hasattr(self, "_n_slabs"):
@@ -259,6 +266,9 @@ class CbowModel:
             self._fwd_do(win, n_total, win_begin, n)
             return
         csc = self._csc_for(win, win_begin, n)
+        if self.det and self.algo == "rows":
+            self._fwdbwd_det(win, n_total, win_begin, n, csc)
+            return
         if self.algo == "rank1":
             if csc is not None:
                 rc = self.lib.g2v_cbow_r1_windows_csc(self.rowptr.data_ptr(), self.gene.data_ptr(),
@@ -300,22 +310,66 @@ class CbowModel:
                                       self.V, self.D, self.reduce, self._stream())
         _capi.check(rc, "g2v_cbow_fwdbwd")
 
+    def _plan(self, win, win_begin, n):
+        plan = self._batches.get((self._ptr(win), int(win_begin), int(n)))
+        if plan is None:
+            raise RuntimeError("%s: windows [%d, %d) of this list were not given to prepare_batches"
+                               % ("optimizer='lazy_adam'" if self.lazy else "deterministic=True", win_begin, win_begin + n))
+        return plan
+
+    def det_workspace(self, n):
+        """The tile workspace of a deterministic forward over n windows (g2v_cbow_det_workspace_bytes), grown on
+        demand and shared by every such forward of this model (they run in stream order)."""
+        nbytes = int(self.lib.g2v_cbow_det_workspace_bytes(int(n), self.D))
+        if self._det_ws is None or self._det_ws.numel() < nbytes:
+            self._det_ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=self.device)
+        return self._det_ws
+
+    def _fwd_do_call(self, win_ptr, n, n_total, dO):
+        if self.det:
+            rc = self.lib.g2v_cbow_fwd_do_det(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+                                              win_ptr, int(n), 1.0 / float(n_total), self.W_ih.data_ptr(),
+                                              self.W_ho.data_ptr(), dO.data_ptr(), self.g_ho.data_ptr(),
+                                              self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D, self.reduce,
+                                              self.det_workspace(n).data_ptr(), 0, self._stream())
+            _capi.check(rc, "g2v_cbow_fwd_do_det")
+            return
+        rc = self.lib.g2v_cbow_fwd_do(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(), win_ptr,
+                                      int(n), 1.0 / float(n_total), self.W_ih.data_ptr(), self.W_ho.data_ptr(),
+                                      dO.data_ptr(), self.g_ho.data_ptr(), self.acc.data_ptr(), self.acc.data_ptr() + 8,
+                                      self.V, self.D, self.reduce, self._stream())
+        _capi.check(rc, "g2v_cbow_fwd_do")
+
     def _fwd_do(self, win, n_total, win_begin, n):
         """lazy_adam's forward: dO*scale per position of a batch prepared by prepare_batches (loss, accuracy and g_ho
         as fwdbwd); update() then applies the lazy step to the batch's rows."""
-        plan = self._batches.get((self._ptr(win), int(win_begin), int(n)))
-        if plan is None:
-            raise RuntimeError("optimizer='lazy_adam': windows [%d, %d) of this list were not given to prepare_batches"
-                               % (win_begin, win_begin + n))
-        self._pending = plan
+        self._pending = self._plan(win, win_begin, n)
         if n == 0:
             return
-        rc = self.lib.g2v_cbow_fwd_do(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
-                                      win.data_ptr() + 4 * int(win_begin), int(n), 1.0 / float(n_total),
-                                      self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._dO.data_ptr(),
-                                      self.g_ho.data_ptr(), self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V,
-                                      self.D, self.reduce, self._stream())
-        _capi.check(rc, "g2v_cbow_fwd_do")
+        self._fwd_do_call(win.data_ptr() + 4 * int(win_begin), n, n_total, self._dO)
+
+    def _fwdbwd_det(self, win, n_total, win_begin, n, csc):
+        """Deterministic rows fwdbwd: the whole list prepared by prepare_csc (g2v_cbow_fwdbwd_csc_det), or a batch
+        prepared by prepare_batches (g2v_cbow_fwd_do_det + g2v_cbow_batch_expand over the batch's touched rows)."""
+        if csc is not None:
+            rc = self.lib.g2v_cbow_fwdbwd_csc_det(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+                                                  win.data_ptr(), int(n), 1.0 / float(n_total), self.W_ih.data_ptr(),
+                                                  self.W_ho.data_ptr(), csc[2].data_ptr(), csc[3].data_ptr(),
+                                                  csc[4].data_ptr(), self.g_ih.data_ptr(), self.g_ho.data_ptr(),
+                                                  self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D,
+                                                  self.reduce, self.det_workspace(n).data_ptr(), 0, self._stream())
+            _capi.check(rc, "g2v_cbow_fwdbwd_csc_det")
+            return
+        if win is None:
+            raise RuntimeError("deterministic=True: fwdbwd needs a window list given to prepare_csc or prepare_batches")
+        (_, rows, segptr, pos), r0, n_rows = self._plan(win, win_begin, n)
+        if n == 0:
+            return
+        self._fwd_do_call(win.data_ptr() + 4 * int(win_begin), n, n_total, self._dO)
+        rc = self.lib.g2v_cbow_batch_expand(rows.data_ptr() + 4 * r0, segptr.data_ptr() + 4 * r0, pos.data_ptr(),
+                                            self._dO.data_ptr(), n_rows, self.W_ho.data_ptr(), self.g_ih.data_ptr(),
+                                            self.V, self.D, 0, self._stream())
+        _capi.check(rc, "g2v_cbow_batch_expand")
 
     def _lazy_update(self, adev):
         (_, rows, segptr, pos), r0, n_rows = self._pending or ((None,) * 4, 0, 0)
@@ -537,7 +591,7 @@ def _dist():
 
 def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500, seed=0, optimizer="adam",
                reduce="sum", W_ih0=None, W_ho0=None, split=None, early_stop=True, log=print, return_info=False,
-               eval_train="lazy", algo="rows", batch=0, use_graph=True, reshuffle=False):
+               eval_train="lazy", algo="rows", batch=0, use_graph=True, reshuffle=False, deterministic=False):
     """Train the modified CBOW on CSR windows and return W_ih (np.float32 [n_genes, hidden]) exactly as
     ``compute_genetovec`` does: the weights after the last step whose validation accuracy did not drop.
 
@@ -564,10 +618,20 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     into consecutive batches as before; several GPUs deal the epoch's list as they deal the split's.  The order is
     written on the device every epoch, and lazy_adam rebuilds its batch plans there.  With ``batch >= n_train`` (full
     batch) the flag has no effect; with ``batch <= 0`` it is an error.
+
+    ``deterministic`` (algo="rows", one GPU): every floating-point sum of a step is taken in a fixed order (DESIGN.md
+    §4.13), so the same inputs and seed give the same bits of W_ih, W_ho, the history and the stop step on every run
+    and for any launch grid -- every optimizer, full batch or mini-batches, with or without ``reshuffle`` and CUDA
+    graphs, at every table size (no gene slabs).  Mini-batch adam/sgd then build per-batch plans as lazy_adam does.
+    algo="rank1" is already reproducible with a full batch and is accepted unchanged; with ``batch > 0`` it is an error.
     """
     if reshuffle and batch <= 0:
         raise ValueError("reshuffle=True needs mini-batches (batch > 0)")
     dist = _dist()
+    if deterministic and dist:
+        raise ValueError("deterministic=True runs on one GPU only (world size %d)" % dist.get_world_size())
+    if deterministic and algo == "rank1" and batch > 0:
+        raise ValueError("deterministic=True with algo='rank1' needs a full batch: rank1's mini-batch c uses atomics")
     if optimizer == "lazy_adam" and algo != "rows":
         raise ValueError("optimizer='lazy_adam' needs algo='rows' (rank1 keeps s = W_ih.W_ho, which every W_ho step "
                          "changes for every gene)")
@@ -582,7 +646,8 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     if W_ih0 is None or W_ho0 is None:
         W_ih0, W_ho0 = init_weights(n_genes, hidden, seed)
     model = CbowModel(win_rowptr, win_gene, labels, n_genes, hidden, W_ih0, W_ho0, optimizer, reduce, lr, algo=algo,
-                      nvl_group=dist.group.WORLD if (dist and algo == "rows") else None)
+                      nvl_group=dist.group.WORLD if (dist and algo == "rows") else None,
+                      deterministic=deterministic and algo == "rows")
     lens = np.diff(rowptr_np).astype(np.int64)
     n_tr, n_va = len(tr), len(va)
     full_batch = batch <= 0 or batch >= n_tr
@@ -597,7 +662,7 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     va_d = torch.from_numpy(np.ascontiguousarray(va_loc, dtype=np.int32)).to(dev)
 
     slabs = False
-    if model.lazy:                               # touched genes of every batch; single-pass forward at every table size
+    if model.lazy or (model.det and not full_batch):   # touched genes of every batch; single-pass forward at every size
         model.prepare_batches(tr_d, len(tr_loc) if full_batch else batch)
     elif algo == "rows" and full_batch:          # tables larger than the L2: gene-slab passes over the static lists
         slabs = model.prepare_slabs(tr_d)
@@ -741,7 +806,14 @@ class DeviceLoop:
             m.evaluate(self.va_d, 2)
         if m_val is not None:
             m_val.record()
-        if self.carried:
+        if self.carried and m.det:
+            _capi.check(lib.g2v_cbow_loop_tail_det(self.ctl.data_ptr(), m.rowptr.data_ptr(), m.gene.data_ptr(),
+                                                   m.label.data_ptr(), self.tr_d.data_ptr(), self.n_tr_loc,
+                                                   1.0 / float(self.n_tr), m.W_ih.data_ptr(), m.W_ho.data_ptr(),
+                                                   m._csc[4].data_ptr(), m.g_ho.data_ptr(), m.acc.data_ptr(), m.V, m.D,
+                                                   m.reduce, m.det_workspace(self.n_tr_loc).data_ptr(), 0, self._st()),
+                        "g2v_cbow_loop_tail_det")
+        elif self.carried:
             csc = m._csc
             _capi.check(lib.g2v_cbow_loop_tail(self.ctl.data_ptr(), m.rowptr.data_ptr(), m.gene.data_ptr(),
                                                m.label.data_ptr(), self.tr_d.data_ptr(), self.n_tr_loc,
@@ -852,7 +924,7 @@ def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_l
     training list, the reference's per-epoch accuracies and early stop around it; host-driven, one sync per epoch.
     ``reshuffle`` = (global training list on the device, seed, rank): every epoch e >= 1 trains on this rank's share of
     the epoch's order, written into one preallocated buffer (g2v_cbow_epoch_order); lazy_adam then rebuilds the
-    buffer's batch plans (one more sync)."""
+    buffer's batch plans (one more sync), as does the deterministic mode."""
     dev = model.device
     info = _LoopLog(n_tr, n_va, log)
     result = model.W_ih.clone()
@@ -864,7 +936,7 @@ def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_l
         if reshuffle and step >= 1:
             tr_all, seed, rank = reshuffle
             epoch_order(tr_all, seed, step, rank, world, out=ep_d)
-            if model.lazy:
+            if model.lazy or model.det:
                 model.prepare_batches(ep_d, batch)
             win = ep_d
         model.acc.zero_()

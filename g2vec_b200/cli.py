@@ -5,7 +5,17 @@ Same positionals, options, progress banners and output files as /root/reference/
 plain Python/NumPy/scikit-learn as in the reference; step 3 runs g2vec_b200.walks on the GPU and
 step 4 g2vec_b200.cbow.  Two documented differences: ``--epoch`` is honoured as the cap on optimizer
 steps (the reference parses it, :515, and then loops ``range(500)``, :262 -- the default 500 is the
-reference behaviour), and ``--seed`` (default 0) makes runs reproducible (the reference is unseeded).
+reference behaviour), and ``--seed`` (default 0) seeds the walk sampler, the path glue, the split and the
+initial vectors (the reference is unseeded).
+
+Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
+- ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
+  ``--reshuffle``, at every table size (DESIGN.md §4.13);
+- ``--algo rank1`` with a full batch.
+Without ``--deterministic`` the rows trainer adds some floating-point values in an order the GPU picks (the
+output-layer gradient every step; the gradient rows with ``--batch`` and adam/sgd, or on tables larger than the
+L2), so two runs can differ in the last bits of the vectors, and rarely in the stop step or the biomarkers.
+Runs on several GPUs are not bit-reproducible.
 """
 import argparse
 import sys
@@ -40,9 +50,14 @@ def parse_arguments(argv=None):
     p.add_argument('--reshuffle', action='store_true',
                    help="with --batch: train every epoch after the first on a new pseudo-random order of the training "
                         "windows (seeded by --seed and the epoch) instead of the same batches every epoch")
+    p.add_argument('--deterministic', action='store_true',
+                   help="bit-reproducible training on one GPU: every floating-point sum of a step in a fixed order "
+                        "(rows: any optimizer and batch size; rank1: full batch only); somewhat slower")
     args = p.parse_args(argv)
     if args.reshuffle and args.batch <= 0:
         p.error("--reshuffle needs mini-batches (--batch B with B > 0)")
+    if args.deterministic and args.algo == 'rank1' and args.batch > 0:
+        p.error("--deterministic with --algo rank1 needs a full batch (--batch 0)")
     return args
 
 
@@ -239,7 +254,8 @@ def main(argv=None):
     print(">>> 4. Compute distributed representations using modified CBOW")
     mat = cbow.train_cbow(w_rowptr, w_gene, w_label, n_genes, args.sizeHiddenlayer, args.learningRate,
                           max_epoch=args.epoch, seed=args.seed, log=print, algo=args.algo,   # print is silent off rank 0
-                          batch=args.batch, optimizer=args.optimizer, reshuffle=args.reshuffle)
+                          batch=args.batch, optimizer=args.optimizer, reshuffle=args.reshuffle,
+                          deterministic=args.deterministic)
     genes = data['gene']
     if rank != 0:
         dist.barrier()

@@ -247,6 +247,262 @@ cbow_csc_expand_kernel(const int32_t *__restrict__ cscptr, const int32_t *__rest
     }
 }
 
+// ---- deterministic mode (DESIGN.md §4.13): the CSC forward with every floating-point sum in a fixed order ----
+// The list is cut into tiles of kDetTile positions.  A CTA takes whole tiles (t = blockIdx.x, + gridDim.x, ...); inside
+// tile t warp w takes positions t*kDetTile + w, + kCbowWarps, ... in order and accumulates its g_ho partial and loss from
+// zero.  The warp partials are added in warp order in shared memory and stored as the tile's partial in a workspace
+// (loss: double [n_tiles], then g_ho: float [n_tiles][D]); cbow_det_sum_kernel then adds the tiles in a fixed order.
+// No value depends on the grid, so the result is the same bits for any number of CTAs.  dO_pos and the correct count
+// are the CSC mode's (integers need no order).
+constexpr int kDetTile = 64;
+constexpr int kDetSumWarps = 32;
+
+__host__ __device__ __forceinline__ size_t det_ws_loss_bytes(int64_t n_tiles) {
+    return ((size_t)n_tiles * sizeof(double) + 255) & ~(size_t)255;
+}
+
+template <int VEC>
+__global__ void __launch_bounds__(kCbowWarps * 32)
+cbow_rows_det_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
+                     const uint8_t *__restrict__ label, const int32_t *__restrict__ win, int64_t n_win, float inv_n,
+                     const float *__restrict__ W_ih, const float *__restrict__ W_ho, float *__restrict__ dO_pos,
+                     double *__restrict__ tile_loss, float *__restrict__ tile_gho,
+                     unsigned long long *__restrict__ n_correct, int32_t reduce_mean, const int32_t *__restrict__ skip,
+                     const int32_t *__restrict__ carried) {
+    G2V_SKIP_IF_STOPPED(skip);
+    G2V_SKIP_IF_STOPPED(carried);
+    constexpr int D = 128 * VEC;
+    constexpr int D4 = D / 4;
+    constexpr int UNR = 8 / VEC;
+    __shared__ float4 sh_gho[kCbowWarps][D4];
+    __shared__ float sh_loss[kCbowWarps];
+    __shared__ unsigned long long sh_correct;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) sh_correct = 0ull;
+    __syncthreads();
+    const float4 *__restrict__ W4 = reinterpret_cast<const float4 *>(W_ih);
+    float4 who[VEC];
+#pragma unroll
+    for (int v = 0; v < VEC; ++v) who[v] = ldg4(reinterpret_cast<const float4 *>(W_ho) + v * 32 + lane);
+    unsigned correct_acc = 0;
+    const int64_t n_tiles = (n_win + kDetTile - 1) / kDetTile;
+    for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        float4 gho[VEC];
+#pragma unroll
+        for (int v = 0; v < VEC; ++v) gho[v] = make_float4(0.f, 0.f, 0.f, 0.f);
+        float loss_acc = 0.f;
+        const int64_t i_end = min(n_win, (t + 1) * kDetTile);
+        for (int64_t i = t * kDetTile + warp; i < i_end; i += kCbowWarps) {
+            const int64_t n = __ldg(win + i);
+            const int32_t b = __ldg(rowptr + n), e = __ldg(rowptr + n + 1);
+            const float y = (float)__ldg(label + n);
+            float4 h[VEC];
+#pragma unroll
+            for (int v = 0; v < VEC; ++v) h[v] = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int32_t base = b; base < e; base += 32) {
+                const int cnt = min(32, e - base);
+                const int32_t g = (lane < cnt) ? __ldg(gene + base + lane) : 0;
+                for (int k = 0; k < cnt; k += UNR) {
+                    float4 r[UNR][VEC];
+#pragma unroll
+                    for (int u = 0; u < UNR; ++u) {
+                        const int32_t gk = __shfl_sync(0xffffffffu, g, (k + u) & 31);
+                        const float4 *row = W4 + (size_t)gk * D4 + lane;
+#pragma unroll
+                        for (int v = 0; v < VEC; ++v)
+                            r[u][v] = (k + u < cnt) ? ldg4(row + v * 32) : make_float4(0.f, 0.f, 0.f, 0.f);
+                    }
+#pragma unroll
+                    for (int u = 0; u < UNR; ++u)
+#pragma unroll
+                        for (int v = 0; v < VEC; ++v) {
+                            h[v].x += r[u][v].x; h[v].y += r[u][v].y; h[v].z += r[u][v].z; h[v].w += r[u][v].w;
+                        }
+                }
+            }
+            const float scale = (reduce_mean && e > b) ? 1.f / (float)(e - b) : 1.f;
+            float part = 0.f;
+#pragma unroll
+            for (int v = 0; v < VEC; ++v) {
+                if (reduce_mean) { h[v].x *= scale; h[v].y *= scale; h[v].z *= scale; h[v].w *= scale; }
+                part += h[v].x * who[v].x + h[v].y * who[v].y + h[v].z * who[v].z + h[v].w * who[v].w;
+            }
+            const float o = warp_sum(part);
+            if (lane == 0) {
+                correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
+                loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
+            }
+            const float dO = (sigmoid_stable(o) - y) * inv_n;
+#pragma unroll
+            for (int v = 0; v < VEC; ++v) {
+                gho[v].x += h[v].x * dO; gho[v].y += h[v].y * dO; gho[v].z += h[v].z * dO; gho[v].w += h[v].w * dO;
+            }
+            if (lane == 0) dO_pos[i] = dO * scale;
+        }
+#pragma unroll
+        for (int v = 0; v < VEC; ++v) sh_gho[warp][v * 32 + lane] = gho[v];
+        if (lane == 0) sh_loss[warp] = loss_acc;
+        __syncthreads();
+        float4 *out = reinterpret_cast<float4 *>(tile_gho + (size_t)t * D);
+        for (int k = threadIdx.x; k < D4; k += blockDim.x) {
+            float4 s = sh_gho[0][k];
+#pragma unroll
+            for (int w = 1; w < kCbowWarps; ++w) {
+                const float4 x = sh_gho[w][k];
+                s.x += x.x; s.y += x.y; s.z += x.z; s.w += x.w;
+            }
+            out[k] = s;
+        }
+        if (threadIdx.x == 0) {
+            double l = 0.0;
+            for (int w = 0; w < kCbowWarps; ++w) l += (double)sh_loss[w];
+            tile_loss[t] = l;
+        }
+        __syncthreads();                                   // the next tile overwrites sh_gho / sh_loss
+    }
+    if (lane == 0) atomicAdd(&sh_correct, (unsigned long long)correct_acc);
+    __syncthreads();
+    if (threadIdx.x == 0 && n_correct) atomicAdd(n_correct, sh_correct);
+}
+
+// Any D: cbow_rows_generic_kernel's CSC mode with the tiles of cbow_rows_det_kernel.
+__global__ void __launch_bounds__(kCbowWarps * 32)
+cbow_rows_generic_det_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
+                             const uint8_t *__restrict__ label, const int32_t *__restrict__ win, int64_t n_win,
+                             float inv_n, const float *__restrict__ W_ih, const float *__restrict__ W_ho,
+                             float *__restrict__ dO_pos, double *__restrict__ tile_loss, float *__restrict__ tile_gho,
+                             unsigned long long *__restrict__ n_correct, int32_t D, int32_t reduce_mean,
+                             const int32_t *__restrict__ skip, const int32_t *__restrict__ carried) {
+    G2V_SKIP_IF_STOPPED(skip);
+    G2V_SKIP_IF_STOPPED(carried);
+    extern __shared__ float shf[];
+    __shared__ float sh_loss[kCbowWarps];
+    __shared__ unsigned long long sh_correct;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float *h = shf + (size_t)warp * 2 * D;
+    float *gho = h + D;
+    if (threadIdx.x == 0) sh_correct = 0ull;
+    __syncthreads();
+    unsigned correct_acc = 0;
+    const int64_t n_tiles = (n_win + kDetTile - 1) / kDetTile;
+    for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        for (int d = lane; d < D; d += 32) gho[d] = 0.f;
+        float loss_acc = 0.f;
+        const int64_t i_end = min(n_win, (t + 1) * kDetTile);
+        for (int64_t i = t * kDetTile + warp; i < i_end; i += kCbowWarps) {
+            const int64_t n = __ldg(win + i);
+            const int32_t b = __ldg(rowptr + n), e = __ldg(rowptr + n + 1);
+            const float y = (float)__ldg(label + n);
+            for (int d = lane; d < D; d += 32) h[d] = 0.f;
+            for (int32_t j = b; j < e; ++j) {
+                const float *row = W_ih + (size_t)__ldg(gene + j) * D;
+                for (int d = lane; d < D; d += 32) h[d] += __ldg(row + d);
+            }
+            const float scale = (reduce_mean && e > b) ? 1.f / (float)(e - b) : 1.f;
+            float part = 0.f;
+            for (int d = lane; d < D; d += 32) {
+                if (reduce_mean) h[d] *= scale;
+                part += h[d] * __ldg(W_ho + d);
+            }
+            const float o = warp_sum(part);
+            if (lane == 0) {
+                correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
+                loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
+            }
+            const float dO = (sigmoid_stable(o) - y) * inv_n;
+            for (int d = lane; d < D; d += 32) gho[d] += h[d] * dO;
+            if (lane == 0) dO_pos[i] = dO * scale;
+        }
+        if (lane == 0) sh_loss[warp] = loss_acc;
+        __syncthreads();
+        float *out = tile_gho + (size_t)t * D;
+        for (int d = threadIdx.x; d < D; d += blockDim.x) {
+            float s = shf[D + d];
+            for (int w = 1; w < kCbowWarps; ++w) s += shf[(size_t)w * 2 * D + D + d];
+            out[d] = s;
+        }
+        if (threadIdx.x == 0) {
+            double l = 0.0;
+            for (int w = 0; w < kCbowWarps; ++w) l += (double)sh_loss[w];
+            tile_loss[t] = l;
+        }
+        __syncthreads();
+    }
+    if (lane == 0) atomicAdd(&sh_correct, (unsigned long long)correct_acc);
+    __syncthreads();
+    if (threadIdx.x == 0 && n_correct) atomicAdd(n_correct, sh_correct);
+}
+
+// Second step of the deterministic forward: g_ho[d] += the sum of the tile partials, *loss_sum += the sum of the tile
+// losses.  One CTA per 32 columns; warp w sums tiles w, w + kDetSumWarps, ... in order, then the warp sums are added
+// in warp order.  The losses: CTA 0, thread j sums tiles j, j + 32*kDetSumWarps, ... in order, then a fixed shuffle
+// tree per warp and the warps in order.  The launch shape depends on D only.
+__global__ void __launch_bounds__(kDetSumWarps * 32)
+cbow_det_sum_kernel(const double *__restrict__ tile_loss, const float *__restrict__ tile_gho, int64_t n_tiles,
+                    int32_t D, float *__restrict__ g_ho, double *__restrict__ loss_sum, const int32_t *__restrict__ skip,
+                    const int32_t *__restrict__ carried) {
+    G2V_SKIP_IF_STOPPED(skip);
+    G2V_SKIP_IF_STOPPED(carried);
+    __shared__ float sh[kDetSumWarps][32];
+    __shared__ double shl[kDetSumWarps];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int d = blockIdx.x * 32 + lane;
+    float s = 0.f;
+    if (d < D)
+#pragma unroll 8
+        for (int64_t t = warp; t < n_tiles; t += kDetSumWarps) s += __ldg(tile_gho + (size_t)t * D + d);
+    sh[warp][lane] = s;
+    if (blockIdx.x == 0) {
+        double l = 0.0;
+        for (int64_t t = threadIdx.x; t < n_tiles; t += kDetSumWarps * 32) l += __ldg(tile_loss + t);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
+        if (lane == 0) shl[warp] = l;
+    }
+    __syncthreads();
+    if (warp == 0) {
+        if (d < D) {
+            float a = sh[0][lane];
+            for (int w = 1; w < kDetSumWarps; ++w) a += sh[w][lane];
+            g_ho[d] += a;
+        }
+        if (blockIdx.x == 0 && lane == 0 && loss_sum) {
+            double a = shl[0];
+            for (int w = 1; w < kDetSumWarps; ++w) a += shl[w];
+            *loss_sum += a;
+        }
+    }
+}
+
+// The CSC expansion on one batch's plan (g2v_cbow_batch_plan): rows[r] = a gene the batch gathered, its batch-relative
+// positions pos[segptr[r] .. segptr[r+1]).  One warp per row, as cbow_csc_expand_kernel: c = its segmented dO sum,
+// g_ih[row,:] += c * W_ho; no atomics.
+__global__ void __launch_bounds__(kCbowWarps * 32)
+cbow_batch_expand_kernel(const int32_t *__restrict__ rows, const int32_t *__restrict__ segptr,
+                         const int32_t *__restrict__ pos, const float *__restrict__ dO_pos, int64_t n_rows,
+                         const float *__restrict__ W_ho, float *__restrict__ g_ih, int32_t D,
+                         const int32_t *__restrict__ skip) {
+    G2V_SKIP_IF_STOPPED(skip);
+    const int lane = threadIdx.x & 31;
+    const int64_t warp = (int64_t)blockIdx.x * kCbowWarps + (threadIdx.x >> 5);
+    const int64_t nwarps = (int64_t)gridDim.x * kCbowWarps;
+    for (int64_t r = warp; r < n_rows; r += nwarps) {
+        const float c = csc_segment_sum(pos, dO_pos, __ldg(segptr + r), __ldg(segptr + r + 1), lane);
+        float *row = g_ih + (size_t)__ldg(rows + r) * D;
+        if ((D & 3) == 0) {
+            float4 *r4 = reinterpret_cast<float4 *>(row);
+            for (int k = lane; k < (D >> 2); k += 32) {
+                const float4 w = ldg4(reinterpret_cast<const float4 *>(W_ho) + k);
+                float4 a = r4[k];
+                a.x += c * w.x; a.y += c * w.y; a.z += c * w.z; a.w += c * w.w;
+                r4[k] = a;
+            }
+        } else {
+            for (int d = lane; d < D; d += 32) row[d] += c * __ldg(W_ho + d);
+        }
+    }
+}
+
 // ---- optimizer epilogue --------------------------------------------------------------------
 template <int OPT>
 __global__ void __launch_bounds__(256)
@@ -472,6 +728,57 @@ static int launch_rows(const int32_t *rowptr, const int32_t *gene, const uint8_t
     return 0;
 }
 
+// Grid of a deterministic launch over n_items: rows_grid's, at most max_ctas CTAs when max_ctas > 0.  The results do
+// not depend on it; tests vary it to show that.
+static int det_grid(const void *kernel, size_t smem, int64_t n_items, int32_t max_ctas, int *grid) {
+    int rc = rows_grid(kernel, smem, n_items, grid);
+    if (rc == 0 && max_ctas > 0 && *grid > max_ctas) *grid = max_ctas;
+    return rc;
+}
+
+// The deterministic forward over win[0..n_win-1] (cbow_rows_det_kernel / cbow_rows_generic_det_kernel) and the fixed-
+// order sum of its tiles into g_ho and loss_sum (cbow_det_sum_kernel).  Both launches also test `carried` (nullable).
+static int launch_rows_det(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                           int64_t n_win, float inv_n, const float *W_ih, const float *W_ho, float *dO_pos,
+                           float *g_ho, double *loss_sum, int64_t *n_correct, int32_t D, int32_t reduce,
+                           void *workspace, int32_t max_ctas, cudaStream_t st, const int32_t *carried) {
+    unsigned long long *nc = reinterpret_cast<unsigned long long *>(n_correct);
+    const int64_t n_tiles = (n_win + kDetTile - 1) / kDetTile;
+    double *tile_loss = reinterpret_cast<double *>(workspace);
+    float *tile_gho = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + det_ws_loss_bytes(n_tiles));
+    int grid = 0, rc;
+#define G2V_LAUNCH_DET(VEC)                                                                                            \
+    {                                                                                                                  \
+        if ((rc = det_grid((const void *)cbow_rows_det_kernel<VEC>, 0, n_tiles * kCbowWarps, max_ctas, &grid)))      \
+            return rc;                                                                                                 \
+        cbow_rows_det_kernel<VEC><<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, n_win, inv_n, W_ih,     \
+                                                                    W_ho, dO_pos, tile_loss, tile_gho, nc, reduce,     \
+                                                                    loop_skip_flag(), carried);                        \
+    }
+    if (D == 128) G2V_LAUNCH_DET(1)
+    else if (D == 256) G2V_LAUNCH_DET(2)
+    else if (D == 512) G2V_LAUNCH_DET(4)
+    else {
+        const size_t smem = (size_t)kCbowWarps * 2 * D * sizeof(float);
+        DeviceProps dp;
+        if (device_props(&dp)) return 1;
+        G2V_REQUIRE(smem + 1024 <= (size_t)dp.max_smem_optin, "sizeHiddenlayer %d too large for the generic kernel", D);
+        G2V_CUDA_OK(cudaFuncSetAttribute(cbow_rows_generic_det_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        if ((rc = det_grid((const void *)cbow_rows_generic_det_kernel, smem, n_tiles * kCbowWarps, max_ctas, &grid)))
+            return rc;
+        cbow_rows_generic_det_kernel<<<grid, kCbowWarps * 32, smem, st>>>(rowptr, gene, label, win, n_win, inv_n, W_ih,
+                                                                          W_ho, dO_pos, tile_loss, tile_gho, nc, D,
+                                                                          reduce, loop_skip_flag(), carried);
+    }
+#undef G2V_LAUNCH_DET
+    G2V_CUDA_OK(cudaGetLastError());
+    cbow_det_sum_kernel<<<(D + 31) / 32, kDetSumWarps * 32, 0, st>>>(tile_loss, tile_gho, n_tiles, D, g_ho, loss_sum,
+                                                                       loop_skip_flag(), carried);
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch(2);
+    return 0;
+}
+
 
 // ---- device-side training loop control (SURVEY 8f-4; G2Vec.py:262-283) ------------------------------------
 // ctl (int64 x 8 in device memory):
@@ -670,6 +977,82 @@ extern "C" int g2v_cbow_loop_tail(int64_t *ctl, const int32_t *rowptr, const int
                              reinterpret_cast<double *>(acc + 4), acc + 5, V, D, reduce, st);
     if (rc) return rc;
     loop_carry_kernel<<<1, 1, 0, st>>>(reinterpret_cast<long long *>(ctl), reinterpret_cast<long long *>(acc));
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" size_t g2v_cbow_det_workspace_bytes(int64_t n_win, int32_t D) {
+    if (n_win < 0 || D <= 0) return 0;
+    const int64_t n_tiles = (n_win + kDetTile - 1) / kDetTile;
+    return det_ws_loss_bytes(n_tiles) + (size_t)n_tiles * (size_t)D * sizeof(float);
+}
+
+#define G2V_DET_CHECK(name)                                                                                            \
+    G2V_REQUIRE(V > 0 && D > 0 && n_win >= 0 && max_ctas >= 0, name ": bad sizes (V=%d D=%d n_win=%lld max_ctas=%d)", \
+                V, D, (long long)n_win, max_ctas);                                                                     \
+    G2V_REQUIRE(n_win == 0 || (rowptr && gene && label && win && W_ih && W_ho && dO && g_ho && workspace),            \
+                name ": null pointer");                                                                                \
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, name ": unknown reduce %d", reduce)
+
+extern "C" int g2v_cbow_fwdbwd_csc_det(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                       const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                                       const float *W_ho, const int32_t *cscptr, const int32_t *csc_pos, float *dO,
+                                       float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
+                                       int32_t D, int32_t reduce, void *workspace, int32_t max_ctas, void *stream) {
+    G2V_DET_CHECK("g2v_cbow_fwdbwd_csc_det");
+    G2V_REQUIRE(n_win == 0 || (cscptr && csc_pos && g_ih), "g2v_cbow_fwdbwd_csc_det: null pointer");
+    if (n_win == 0) return 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = launch_rows_det(rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho, loss_sum, n_correct,
+                             D, reduce, workspace, max_ctas, st, loop_carry_flag());
+    if (rc) return rc;
+    int grid = 0;
+    if ((rc = det_grid((const void *)cbow_csc_expand_kernel, 0, V, max_ctas, &grid))) return rc;
+    cbow_csc_expand_kernel<<<grid, kCbowWarps * 32, 0, st>>>(cscptr, csc_pos, dO, W_ho, g_ih, V, D, loop_skip_flag());
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_fwd_do_det(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                   const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                                   const float *W_ho, float *dO, float *g_ho, double *loss_sum, int64_t *n_correct,
+                                   int32_t V, int32_t D, int32_t reduce, void *workspace, int32_t max_ctas,
+                                   void *stream) {
+    G2V_DET_CHECK("g2v_cbow_fwd_do_det");
+    if (n_win == 0) return 0;
+    return launch_rows_det(rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho, loss_sum, n_correct, D,
+                           reduce, workspace, max_ctas, (cudaStream_t)stream, nullptr);
+}
+#undef G2V_DET_CHECK
+
+extern "C" int g2v_cbow_loop_tail_det(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                      const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                                      const float *W_ho, float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D,
+                                      int32_t reduce, void *workspace, int32_t max_ctas, void *stream) {
+    G2V_REQUIRE(ctl && acc, "g2v_cbow_loop_tail_det: null loop state");
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = g2v_cbow_fwd_do_det(rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho,
+                                 reinterpret_cast<double *>(acc + 4), acc + 5, V, D, reduce, workspace, max_ctas, st);
+    if (rc) return rc;
+    loop_carry_kernel<<<1, 1, 0, st>>>(reinterpret_cast<long long *>(ctl), reinterpret_cast<long long *>(acc));
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_batch_expand(const int32_t *rows, const int32_t *segptr, const int32_t *pos, const float *dO,
+                                     int64_t n_rows, const float *W_ho, float *g_ih, int32_t V, int32_t D,
+                                     int32_t max_ctas, void *stream) {
+    G2V_REQUIRE(V > 0 && D > 0 && n_rows >= 0 && n_rows <= V && max_ctas >= 0,
+                "g2v_cbow_batch_expand: bad sizes (V=%d D=%d n_rows=%lld max_ctas=%d)", V, D, (long long)n_rows, max_ctas);
+    G2V_REQUIRE(n_rows == 0 || (rows && segptr && pos && dO && W_ho && g_ih), "g2v_cbow_batch_expand: null pointer");
+    if (n_rows == 0) return 0;
+    int grid = 0, rc;
+    if ((rc = det_grid((const void *)cbow_batch_expand_kernel, 0, n_rows, max_ctas, &grid))) return rc;
+    cbow_batch_expand_kernel<<<grid, kCbowWarps * 32, 0, (cudaStream_t)stream>>>(rows, segptr, pos, dO, n_rows, W_ho,
+                                                                                  g_ih, D, loop_skip_flag());
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;

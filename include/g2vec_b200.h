@@ -154,6 +154,35 @@ int g2v_cbow_lazy_adam(const int32_t *rows, const int32_t *segptr, const int32_t
                        float *g_ho, int32_t V, int32_t D, float lr, float beta1, float beta2, float eps, int32_t t,
                        const float *alpha_dev, void *stream);
 
+/* Deterministic mode (DESIGN.md §4.13): the same results as g2v_cbow_fwdbwd_csc / g2v_cbow_fwd_do /
+ * g2v_cbow_loop_tail, with every floating-point sum in a fixed order, so that the bits do not depend on the run or on
+ * the launch grid.  The forward cuts the list into tiles of 64 positions, stores each tile's g_ho partial and loss in
+ * `workspace` (g2v_cbow_det_workspace_bytes(n_win, D) bytes, device memory, contents not needed across calls), and a
+ * second launch adds the tiles in a fixed order into g_ho and *loss_sum.  max_ctas > 0 caps the number of CTAs of
+ * every launch (0 = the whole chip); the results are the same for every value.  Same accumulation semantics, `stopped`
+ * and `carried` handling and launch counts plus one (the tile sum) as the forms they mirror; never synchronises.
+ * g2v_cbow_batch_expand: the expansion of g2v_cbow_fwdbwd_csc on one batch's plan from g2v_cbow_batch_plan: for
+ *   r < n_rows, g_ih[rows[r],:] += c * W_ho with c = the sum of dO over pos[segptr[r] .. segptr[r+1]) in a fixed
+ *   order; rows must be distinct.  With g2v_cbow_fwd_do_det it replaces g2v_cbow_fwdbwd's scatter on a mini-batch.
+ *   One launch (none when n_rows == 0). */
+size_t g2v_cbow_det_workspace_bytes(int64_t n_win, int32_t D);
+int g2v_cbow_fwdbwd_csc_det(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                            int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
+                            const int32_t *cscptr, const int32_t *csc_pos, float *dO, float *g_ih, float *g_ho,
+                            double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce,
+                            void *workspace, int32_t max_ctas, void *stream);
+int g2v_cbow_fwd_do_det(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                        int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho, float *dO, float *g_ho,
+                        double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce, void *workspace,
+                        int32_t max_ctas, void *stream);
+int g2v_cbow_loop_tail_det(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                           const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
+                           float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D, int32_t reduce, void *workspace,
+                           int32_t max_ctas, void *stream);
+int g2v_cbow_batch_expand(const int32_t *rows, const int32_t *segptr, const int32_t *pos, const float *dO,
+                          int64_t n_rows, const float *W_ho, float *g_ih, int32_t V, int32_t D, int32_t max_ctas,
+                          void *stream);
+
 /* Reshuffled mini-batch epochs (csrc/g2v_cbow_plan.cu, DESIGN.md §4.12).
  * g2v_cbow_epoch_order: out[i] = tr[P(rank + i*world)] for i < ceil((n - rank) / world): rank `rank`'s share of the
  *   epoch's list tr[P(0..n-1)].  P = P(seed, epoch, n) is a pseudo-random permutation of [0, n) (a 4-round Feistel
