@@ -715,7 +715,11 @@ static int launch_rows(const int32_t *rowptr, const int32_t *gene, const uint8_t
         const size_t smem = (size_t)kCbowWarps * 2 * D * sizeof(float);
         DeviceProps dp;
         if (device_props(&dp)) return 1;
-        G2V_REQUIRE(smem <= (size_t)dp.max_smem_optin, "sizeHiddenlayer %d too large for the generic kernel", D);
+        // the opt-in limit covers the kernel's static shared memory (sh_acc) as well as the dynamic part
+        cudaFuncAttributes fa;
+        G2V_CUDA_OK(cudaFuncGetAttributes(&fa, cbow_rows_generic_kernel<BACKWARD>));
+        G2V_REQUIRE(smem + fa.sharedSizeBytes <= (size_t)dp.max_smem_optin,
+                    "sizeHiddenlayer %d too large for the generic kernel", D);
         G2V_CUDA_OK(cudaFuncSetAttribute(cbow_rows_generic_kernel<BACKWARD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         if ((rc = rows_grid((const void *)cbow_rows_generic_kernel<BACKWARD>, smem, n_win, &grid))) return rc;
         cbow_rows_generic_kernel<BACKWARD><<<grid, kCbowWarps * 32, smem, st>>>(
@@ -1001,7 +1005,8 @@ extern "C" int g2v_cbow_fwdbwd_csc_det(const int32_t *rowptr, const int32_t *gen
                                        float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
                                        int32_t D, int32_t reduce, void *workspace, int32_t max_ctas, void *stream) {
     G2V_DET_CHECK("g2v_cbow_fwdbwd_csc_det");
-    G2V_REQUIRE(n_win == 0 || (cscptr && csc_pos && g_ih), "g2v_cbow_fwdbwd_csc_det: null pointer");
+    // csc_pos may be NULL: a list of empty windows has no incidences (every CSC segment is empty)
+    G2V_REQUIRE(n_win == 0 || (cscptr && g_ih), "g2v_cbow_fwdbwd_csc_det: null pointer");
     if (n_win == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
     int rc = launch_rows_det(rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho, loss_sum, n_correct,

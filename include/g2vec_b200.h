@@ -128,7 +128,8 @@ int g2v_cbow_fwdbwd(const int32_t *rowptr, const int32_t *gene, const uint8_t *l
  * dO*scale per list position in the scratch dO [n_win]; a second kernel then adds c[g]*W_ho into g_ih[g,:] once
  * per gene, c[g] = sum of dO over the gene's positions in a fixed order -- no floating-point atomics on g_ih.
  * Same accumulation semantics as g2v_cbow_fwdbwd (g_ih, g_ho, loss_sum, n_correct are added into); rows of
- * genes in no listed window are not touched. */
+ * genes in no listed window are not touched.  csc_pos may be NULL only when nnz == 0 (every listed window is empty,
+ * so every segment of cscptr is empty); g2v_cbow_fwdbwd_csc_det takes the same arguments with the same rule. */
 int g2v_cbow_fwdbwd_csc(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
                         const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
                         const float *W_ho, const int32_t *cscptr, const int32_t *csc_pos, float *dO,
