@@ -142,9 +142,8 @@ def run(args):
         srt = lambda: batch_plan_torch(m.rowptr, m.gene, V, ep, B)
         host(srt, 2)
         r["sort_plan_ms"] = float(np.median(host(srt, args.steps)))
-        keys = [(ep.data_ptr(), k * B, min(B, n - k * B)) for k in range(n_b)]
-        r["plan_bytes"] = batch_plan_bytes(V, n, int(m._plan_bufs[(ep.data_ptr(), n, B)].nnz), n_b,
-                                           sum(m._batches[k][2] for k in keys))
+        r["plan_bytes"] = batch_plan_bytes(V, n, int(m.prepared(ep).plan.nnz), n_b,
+                                           sum(m.batch_touched(ep, k * B, min(B, n - k * B)) for k in range(n_b)))
 
         def epoch(reshuffle, e=[1]):
             win = tr

@@ -64,6 +64,7 @@ class CbowModel:
     def __init__(self, rowptr, gene, label, n_genes, hidden, W_ih0, W_ho0, optimizer="adam", reduce="sum",
                  lr=0.005, beta1=0.9, beta2=0.999, eps=1e-8, device=None, algo="rows", nvl_group=None,
                  deterministic=False):
+        check_config(algo, optimizer, deterministic, several_gpus=nvl_group is not None)
         if not torch.cuda.is_available():
             raise RuntimeError("g2vec_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.lib = _capi.load()
@@ -75,13 +76,6 @@ class CbowModel:
                 return a.to(device=dev, dtype=dt).contiguous()
             return torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=dt)
 
-        if optimizer == "lazy_adam" and algo != "rows":
-            raise ValueError("optimizer='lazy_adam' needs algo='rows': rank1 keeps s = W_ih.W_ho, which every W_ho step "
-                             "changes for every gene")
-        if optimizer == "lazy_adam" and nvl_group is not None:
-            raise ValueError("optimizer='lazy_adam' runs on one GPU only")
-        if deterministic and nvl_group is not None:
-            raise ValueError("deterministic=True runs on one GPU only")
         self.rowptr = to(rowptr, torch.int32)
         self.gene = to(gene, torch.int32)
         self.label = to(label, torch.uint8)
@@ -98,7 +92,8 @@ class CbowModel:
         # (g2v_cbow_*_det) on a prepared CSC list or batch plan, never the scatter or the gene slabs
         self.det = bool(deterministic)
         self._det_ws = None
-        self._batches, self._pending, self._dO, self._plan_bufs = {}, None, None, {}
+        # (data_ptr, length) of a window list -> its _WindowList; lazy_adam's batch awaiting update(), the batch dO
+        self._lists, self._pending, self._dO = {}, None, None
         if algo == "rows" and nvl_group is not None:
             self.nvl = _nvl_setup(nvl_group, n_flat, dev)
         if algo == "rows":
@@ -114,8 +109,6 @@ class CbowModel:
         self.reduce = {"sum": _capi.REDUCE_SUM, "mean": _capi.REDUCE_MEAN}[reduce]
         self.lr, self.beta1, self.beta2, self.eps = float(lr), float(beta1), float(beta2), float(eps)
         z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
-        if algo not in ("rows", "rank1"):
-            raise ValueError("algo must be 'rows' (gather/scatter of embedding rows) or 'rank1' (collapsed)")
         self.algo = algo
         if self.lazy:
             self.g_ih, self.g_ho = None, z(self.D)
@@ -149,14 +142,32 @@ class CbowModel:
         # g2v_cbow_adam_tick: no launch of a step depends on a host-side value, so a step can be a CUDA graph
         self.hyper = torch.tensor([1.0, 1.0, 0.0, 0.0], dtype=torch.float32, device=dev)
         if algo == "rank1":
-            _capi.check(self.lib.g2v_cbow_r1_prepare(self.W_ih.data_ptr(), self.W_ho.data_ptr(), self.s.data_ptr(),
-                                                     self.V, self.D, self._stream()), "g2v_cbow_r1_prepare")
+            self._launch("g2v_cbow_r1_prepare", self.W_ih.data_ptr(), self.W_ho.data_ptr(), self.s.data_ptr(), self.V,
+                         self.D)
+
+    def _launch(self, name, *args):
+        """C ABI entry point ``name`` on the current stream of the model's device, its error raised under its name."""
+        rc = getattr(self.lib, name)(*args, self._stream())
+        if rc:
+            _capi.check(rc, name)
+
+    def _key(self, win):
+        return (0, self.rowptr.shape[0] - 1) if win is None else (win.data_ptr(), win.shape[0])
+
+    def prepared(self, win):
+        """The _WindowList of what prepare_csc / prepare_slabs / prepare_batches built for the window list ``win``
+        (int32 device tensor, or None for every window of the table), else None.  For reading only."""
+        return self._lists.get(self._key(win))
+
+    def _record(self, win):
+        key = self._key(win)
+        return self._lists.setdefault(key, _WindowList(win, key[1]))
 
     def prepare_csc(self, win):
         """Transpose the incidence of the window list ``win`` (int32 device tensor) once, so that fwdbwd(win, ...)
         over the WHOLE list reduces dO per gene without floating-point atomics: rank1 forms c deterministically,
         rows writes each gradient row once (g2v_cbow_fwdbwd_csc) instead of red.adding a row per (window, gene).
-        The windows are static across steps (full batch), so this is setup."""
+        The windows are static across steps (full batch), so this is setup; calling it again rebuilds."""
         w = win.to(torch.int64)
         starts = self.rowptr[w].to(torch.int64)
         lens = self.rowptr[w + 1].to(torch.int64) - starts
@@ -168,8 +179,9 @@ class CbowModel:
         g, order = torch.sort(g, stable=True)
         cscptr = torch.zeros(self.V + 1, dtype=torch.int64, device=self.device)
         cscptr[1:] = torch.cumsum(torch.bincount(g, minlength=self.V), 0)
-        self._csc = (win.data_ptr(), int(w.shape[0]), cscptr.to(torch.int32), pos[order].to(torch.int32),
-                     torch.empty(w.shape[0], dtype=torch.float32, device=self.device))
+        rec = self._record(win)
+        rec.cscptr, rec.pos = cscptr.to(torch.int32), pos[order].to(torch.int32)
+        rec.dO = torch.empty(w.shape[0], dtype=torch.float32, device=self.device)
 
     def prepare_batches(self, win, batch):
         """lazy_adam: cut the window list ``win`` (int32 device tensor) into consecutive batches of ``batch`` windows
@@ -184,27 +196,23 @@ class CbowModel:
         B = min(int(batch), n) if batch > 0 else n
         if n == 0:
             return
-        ptr = win.data_ptr()
-        for k in [k for k in self._batches if k[0] == ptr]:
-            del self._batches[k]
-        key = (ptr, n, B)
-        for k in [k for k in self._plan_bufs if k[0] == ptr and k != key]:
-            del self._plan_bufs[k]
-        buf = self._plan_bufs.get(key)
-        if buf is None:
-            buf = _PlanBuffers(self, win, B)
-            self._plan_bufs[key] = buf
-        rows, segptr, pos, brp = buf.build(win)
-        data = (win, rows, segptr, pos)                     # keeps `win` alive: its address is part of the key
-        for k in range(brp.shape[0] - 1):
-            self._batches[(ptr, k * B, min(B, n - k * B))] = (data, int(brp[k]), int(brp[k + 1] - brp[k]))
+        rec = self._record(win)
+        rec.brp = None
+        if rec.plan is None or rec.plan.B != B:
+            rec.plan = None
+            rec.plan = _PlanBuffers(self, win, B)
+        rec.B, rec.brp = B, rec.plan.build(win)[3].tolist()
         if self._dO is None or self._dO.shape[0] < B:
             self._dO = torch.empty(B, dtype=torch.float32, device=self.device)
         self._pending = None
 
     def batch_touched(self, win, win_begin, n):
         """Number of distinct genes of batch [win_begin, win_begin + n) of a list given to prepare_batches."""
-        return self._batches[(self._ptr(win), int(win_begin), int(n))][2]
+        rec = self.prepared(win)
+        rows = rec.batch(win_begin, n) if rec is not None else None
+        if rows is None:
+            raise KeyError((win_begin, n))
+        return rows[1]
 
     def prepare_slabs(self, win, win_begin=0, n_win=None):
         """rows only, tables larger than the L2 (csrc/g2v_cbow_slab.cu): record once, for the static window list
@@ -216,21 +224,16 @@ class CbowModel:
         if not hasattr(self, "_n_slabs"):
             s = ctypes.c_int32(1)
             _capi.check(self.lib.g2v_cbow_slab_plan(self.V, self.D, ctypes.byref(s)), "g2v_cbow_slab_plan")
-            self._n_slabs, self._slabs = int(s.value), {}
+            self._n_slabs = int(s.value)
         n = ((win.shape[0] if win is not None else self.rowptr.shape[0] - 1) - win_begin) if n_win is None else n_win
         if self._n_slabs <= 1 or n <= 0:
             return False
         ws = torch.empty(int(self.lib.g2v_cbow_slab_workspace_bytes(int(n), self.D, self._n_slabs)), dtype=torch.uint8,
                          device=self.device)
-        _capi.check(self.lib.g2v_cbow_slab_setup(self.rowptr.data_ptr(), self.gene.data_ptr(), self._ptr(win),
-                                                 int(win_begin), int(n), self.V, self._n_slabs, ws.data_ptr(),
-                                                 self._stream()), "g2v_cbow_slab_setup")
-        self._slabs[(self._ptr(win), int(win_begin), int(n))] = ws
+        self._launch("g2v_cbow_slab_setup", self.rowptr.data_ptr(), self.gene.data_ptr(), self._ptr(win),
+                     int(win_begin), int(n), self.V, self._n_slabs, ws.data_ptr())
+        self._record(win).slabs[(int(win_begin), int(n))] = ws
         return True
-
-    def _slab_ws(self, win, win_begin, n):
-        slabs = getattr(self, "_slabs", None)
-        return slabs.get((self._ptr(win), int(win_begin), int(n))) if slabs else None
 
     def grad_tensors(self):
         """What a multi-GPU step must all-reduce (sum) between fwdbwd() and update(): nothing when update() does
@@ -251,71 +254,65 @@ class CbowModel:
     def _ptr(t):
         return 0 if t is None else t.data_ptr()
 
-    def _csc_for(self, win, win_begin, n):
-        """The transposed incidence prepare_csc() built for exactly this list, else None."""
-        csc = getattr(self, "_csc", None)
-        if csc is not None and win is not None and csc[0] == win.data_ptr() and win_begin == 0 and n == csc[1]:
-            return csc
-        return None
+    def route(self, win, win_begin=0, n_win=None):
+        """The route (choose_route) fwdbwd(win, ..., win_begin, n_win) takes; raises as that fwdbwd would."""
+        n = (win.shape[0] - win_begin) if n_win is None else n_win
+        return choose_route(self.algo, self.lazy, self.det, self.prepared(win), win_begin, n, win is None)
 
     def fwdbwd(self, win, n_total, win_begin=0, n_win=None):
         """Accumulate the gradient of the listed windows into g_ih / g_ho (loss sum -> acc[0],
         pre-update correct count -> acc[1])."""
         n = (win.shape[0] - win_begin) if n_win is None else n_win
-        if self.lazy:
-            self._fwd_do(win, n_total, win_begin, n)
-            return
-        csc = self._csc_for(win, win_begin, n)
-        if self.det and self.algo == "rows":
-            self._fwdbwd_det(win, n_total, win_begin, n, csc)
-            return
-        if self.algo == "rank1":
-            if csc is not None:
-                rc = self.lib.g2v_cbow_r1_windows_csc(self.rowptr.data_ptr(), self.gene.data_ptr(),
-                                                      self.label.data_ptr(), win.data_ptr(), int(n),
-                                                      1.0 / float(n_total), self.s.data_ptr(), csc[2].data_ptr(),
-                                                      csc[3].data_ptr(), csc[4].data_ptr(), self.c.data_ptr(),
-                                                      self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V,
-                                                      self.reduce, self._stream())
-                _capi.check(rc, "g2v_cbow_r1_windows_csc")
-                return
-            rc = self.lib.g2v_cbow_r1_windows(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
-                                              self._ptr(win), int(win_begin), int(n), 1.0 / float(n_total),
-                                              self.s.data_ptr(), self.c.data_ptr(), self.acc.data_ptr(),
-                                              self.acc.data_ptr() + 8, self.V, self.reduce, self._stream())
-            _capi.check(rc, "g2v_cbow_r1_windows")
-            return
-        ws = self._slab_ws(win, win_begin, n)
-        if ws is not None:
-            rc = self.lib.g2v_cbow_fwdbwd_slabs(self.gene.data_ptr(), self.label.data_ptr(), self._ptr(win),
-                                                int(win_begin), int(n), 1.0 / float(n_total), self.W_ih.data_ptr(),
-                                                self.W_ho.data_ptr(), self.g_ih.data_ptr(), self.g_ho.data_ptr(),
-                                                self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D,
-                                                self.reduce, self._n_slabs, ws.data_ptr(), self._stream())
-            _capi.check(rc, "g2v_cbow_fwdbwd_slabs")
-            return
-        if csc is not None:
-            rc = self.lib.g2v_cbow_fwdbwd_csc(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
-                                              win.data_ptr(), int(n), 1.0 / float(n_total), self.W_ih.data_ptr(),
-                                              self.W_ho.data_ptr(), csc[2].data_ptr(), csc[3].data_ptr(),
-                                              csc[4].data_ptr(), self.g_ih.data_ptr(), self.g_ho.data_ptr(),
-                                              self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D,
-                                              self.reduce, self._stream())
-            _capi.check(rc, "g2v_cbow_fwdbwd_csc")
-            return
-        rc = self.lib.g2v_cbow_fwdbwd(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
-                                      self._ptr(win), int(win_begin), int(n), 1.0 / float(n_total),
-                                      self.W_ih.data_ptr(), self.W_ho.data_ptr(), self.g_ih.data_ptr(),
-                                      self.g_ho.data_ptr(), self.acc.data_ptr(), self.acc.data_ptr() + 8,
-                                      self.V, self.D, self.reduce, self._stream())
-        _capi.check(rc, "g2v_cbow_fwdbwd")
+        rec = self._lists.get(self._key(win))
+        r = choose_route(self.algo, self.lazy, self.det, rec, win_begin, n, win is None)
+        getattr(self, "_fwdbwd_" + r)(win, rec, 1.0 / float(n_total), int(win_begin), int(n))
 
-    def _plan(self, win, win_begin, n):
-        plan = self._batches.get((self._ptr(win), int(win_begin), int(n)))
-        if plan is None:
-            raise RuntimeError("%s: windows [%d, %d) of this list were not given to prepare_batches"
-                               % ("optimizer='lazy_adam'" if self.lazy else "deterministic=True", win_begin, win_begin + n))
-        return plan
+    def _fwdbwd_scatter(self, win, rec, scale, lo, n):
+        self._launch("g2v_cbow_fwdbwd", self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+                     self._ptr(win), lo, n, scale, self.W_ih.data_ptr(), self.W_ho.data_ptr(), self.g_ih.data_ptr(),
+                     self.g_ho.data_ptr(), self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D, self.reduce)
+
+    def _fwdbwd_slabs(self, win, rec, scale, lo, n):
+        self._launch("g2v_cbow_fwdbwd_slabs", self.gene.data_ptr(), self.label.data_ptr(), self._ptr(win), lo, n, scale,
+                     self.W_ih.data_ptr(), self.W_ho.data_ptr(), self.g_ih.data_ptr(), self.g_ho.data_ptr(),
+                     self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D, self.reduce, self._n_slabs,
+                     rec.slabs[(lo, n)].data_ptr())
+
+    def _csc_args(self, win, rec, scale, n):
+        return (self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(), win.data_ptr(), n, scale,
+                self.W_ih.data_ptr(), self.W_ho.data_ptr(), rec.cscptr.data_ptr(), rec.pos.data_ptr(),
+                rec.dO.data_ptr(), self.g_ih.data_ptr(), self.g_ho.data_ptr(), self.acc.data_ptr(),
+                self.acc.data_ptr() + 8, self.V, self.D, self.reduce)
+
+    def _fwdbwd_csc(self, win, rec, scale, lo, n):
+        self._launch("g2v_cbow_fwdbwd_csc", *self._csc_args(win, rec, scale, n))
+
+    def _fwdbwd_csc_det(self, win, rec, scale, lo, n):
+        self._launch("g2v_cbow_fwdbwd_csc_det", *self._csc_args(win, rec, scale, n), self.det_workspace(n).data_ptr(), 0)
+
+    def _fwdbwd_batch_lazy(self, win, rec, scale, lo, n):
+        """dO*scale per position of the batch; update() then applies the lazy step to the batch's rows."""
+        r0, r1 = rec.brp[lo // rec.B], rec.brp[lo // rec.B + 1]
+        self._pending = (rec.plan, r0, r1 - r0)
+        self._fwd_do(win, scale, lo, n)
+
+    def _fwdbwd_batch_det(self, win, rec, scale, lo, n):
+        r0, n_rows = rec.batch(lo, n)
+        self._fwd_do(win, scale, lo, n)
+        p = rec.plan
+        self._launch("g2v_cbow_batch_expand", p.rows.data_ptr() + 4 * r0, p.segptr.data_ptr() + 4 * r0, p.pos.data_ptr(),
+                     self._dO.data_ptr(), n_rows, self.W_ho.data_ptr(), self.g_ih.data_ptr(), self.V, self.D, 0)
+
+    def _fwdbwd_r1(self, win, rec, scale, lo, n):
+        self._launch("g2v_cbow_r1_windows", self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+                     self._ptr(win), lo, n, scale, self.s.data_ptr(), self.c.data_ptr(), self.acc.data_ptr(),
+                     self.acc.data_ptr() + 8, self.V, self.reduce)
+
+    def _fwdbwd_r1_csc(self, win, rec, scale, lo, n):
+        self._launch("g2v_cbow_r1_windows_csc", self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+                     win.data_ptr(), n, scale, self.s.data_ptr(), rec.cscptr.data_ptr(), rec.pos.data_ptr(),
+                     rec.dO.data_ptr(), self.c.data_ptr(), self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V,
+                     self.reduce)
 
     def det_workspace(self, n):
         """The tile workspace of a deterministic forward over n windows (g2v_cbow_det_workspace_bytes), grown on
@@ -325,125 +322,157 @@ class CbowModel:
             self._det_ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=self.device)
         return self._det_ws
 
-    def _fwd_do_call(self, win_ptr, n, n_total, dO):
+    def _fwd_do(self, win, scale, lo, n):
+        """dO*scale of batch [lo, lo + n) into self._dO, with its loss, count and g_ho (in a fixed order if det)."""
+        args = (self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(), win.data_ptr() + 4 * lo, n, scale,
+                self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._dO.data_ptr(), self.g_ho.data_ptr(),
+                self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D, self.reduce)
         if self.det:
-            rc = self.lib.g2v_cbow_fwd_do_det(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
-                                              win_ptr, int(n), 1.0 / float(n_total), self.W_ih.data_ptr(),
-                                              self.W_ho.data_ptr(), dO.data_ptr(), self.g_ho.data_ptr(),
-                                              self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D, self.reduce,
-                                              self.det_workspace(n).data_ptr(), 0, self._stream())
-            _capi.check(rc, "g2v_cbow_fwd_do_det")
-            return
-        rc = self.lib.g2v_cbow_fwd_do(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(), win_ptr,
-                                      int(n), 1.0 / float(n_total), self.W_ih.data_ptr(), self.W_ho.data_ptr(),
-                                      dO.data_ptr(), self.g_ho.data_ptr(), self.acc.data_ptr(), self.acc.data_ptr() + 8,
-                                      self.V, self.D, self.reduce, self._stream())
-        _capi.check(rc, "g2v_cbow_fwd_do")
+            self._launch("g2v_cbow_fwd_do_det", *args, self.det_workspace(n).data_ptr(), 0)
+        else:
+            self._launch("g2v_cbow_fwd_do", *args)
 
-    def _fwd_do(self, win, n_total, win_begin, n):
-        """lazy_adam's forward: dO*scale per position of a batch prepared by prepare_batches (loss, accuracy and g_ho
-        as fwdbwd); update() then applies the lazy step to the batch's rows."""
-        self._pending = self._plan(win, win_begin, n)
-        if n == 0:
-            return
-        self._fwd_do_call(win.data_ptr() + 4 * int(win_begin), n, n_total, self._dO)
-
-    def _fwdbwd_det(self, win, n_total, win_begin, n, csc):
-        """Deterministic rows fwdbwd: the whole list prepared by prepare_csc (g2v_cbow_fwdbwd_csc_det), or a batch
-        prepared by prepare_batches (g2v_cbow_fwd_do_det + g2v_cbow_batch_expand over the batch's touched rows)."""
-        if csc is not None:
-            rc = self.lib.g2v_cbow_fwdbwd_csc_det(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
-                                                  win.data_ptr(), int(n), 1.0 / float(n_total), self.W_ih.data_ptr(),
-                                                  self.W_ho.data_ptr(), csc[2].data_ptr(), csc[3].data_ptr(),
-                                                  csc[4].data_ptr(), self.g_ih.data_ptr(), self.g_ho.data_ptr(),
-                                                  self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D,
-                                                  self.reduce, self.det_workspace(n).data_ptr(), 0, self._stream())
-            _capi.check(rc, "g2v_cbow_fwdbwd_csc_det")
-            return
-        if win is None:
-            raise RuntimeError("deterministic=True: fwdbwd needs a window list given to prepare_csc or prepare_batches")
-        (_, rows, segptr, pos), r0, n_rows = self._plan(win, win_begin, n)
-        if n == 0:
-            return
-        self._fwd_do_call(win.data_ptr() + 4 * int(win_begin), n, n_total, self._dO)
-        rc = self.lib.g2v_cbow_batch_expand(rows.data_ptr() + 4 * r0, segptr.data_ptr() + 4 * r0, pos.data_ptr(),
-                                            self._dO.data_ptr(), n_rows, self.W_ho.data_ptr(), self.g_ih.data_ptr(),
-                                            self.V, self.D, 0, self._stream())
-        _capi.check(rc, "g2v_cbow_batch_expand")
+    def loop_tail(self, ctl, win, n_total):
+        """A carried DeviceLoop's training-accuracy pass over ``win``, whose fwdbwd routes to csc or csc_det
+        (g2v_cbow_loop_tail[_det]): it leaves dO in the list's record, which the next step's fwdbwd expands."""
+        rec = self.prepared(win)
+        args = (ctl.data_ptr(), self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(), win.data_ptr(),
+                rec.n, 1.0 / float(n_total), self.W_ih.data_ptr(), self.W_ho.data_ptr(), rec.dO.data_ptr(),
+                self.g_ho.data_ptr(), self.acc.data_ptr(), self.V, self.D, self.reduce)
+        if self.det:
+            self._launch("g2v_cbow_loop_tail_det", *args, self.det_workspace(rec.n).data_ptr(), 0)
+        else:
+            self._launch("g2v_cbow_loop_tail", *args)
 
     def _lazy_update(self, adev):
-        (_, rows, segptr, pos), r0, n_rows = self._pending or ((None,) * 4, 0, 0)
+        plan, r0, n_rows = self._pending or (None, 0, 0)
         self._pending = None
-        rc = self.lib.g2v_cbow_lazy_adam(rows.data_ptr() + 4 * r0 if n_rows else None,
-                                         segptr.data_ptr() + 4 * r0 if n_rows else None,
-                                         pos.data_ptr() if n_rows else None, self._dO.data_ptr() if n_rows else None,
-                                         n_rows, self.W_ih.data_ptr(), self.m_ih.data_ptr(), self.v_ih.data_ptr(),
-                                         self.W_ho.data_ptr(), self.m_ho.data_ptr(), self.v_ho.data_ptr(),
-                                         self.g_ho.data_ptr(), self.V, self.D, self.lr, self.beta1, self.beta2,
-                                         self.eps, self.t, adev, self._stream())
-        _capi.check(rc, "g2v_cbow_lazy_adam")
+        self._launch("g2v_cbow_lazy_adam", plan.rows.data_ptr() + 4 * r0 if n_rows else None,
+                     plan.segptr.data_ptr() + 4 * r0 if n_rows else None, plan.pos.data_ptr() if n_rows else None,
+                     self._dO.data_ptr() if n_rows else None, n_rows, self.W_ih.data_ptr(), self.m_ih.data_ptr(),
+                     self.v_ih.data_ptr(), self.W_ho.data_ptr(), self.m_ho.data_ptr(), self.v_ho.data_ptr(),
+                     self.g_ho.data_ptr(), self.V, self.D, self.lr, self.beta1, self.beta2, self.eps, self.t, adev)
 
     def update(self):
         self.t += 1
         adev = 0
         if self.opt == _capi.OPT_ADAM_TF1:
-            _capi.check(self.lib.g2v_cbow_adam_tick(self.hyper.data_ptr(), self.lr, self.beta1, self.beta2,
-                                                    self._stream()), "g2v_cbow_adam_tick")
+            self._launch("g2v_cbow_adam_tick", self.hyper.data_ptr(), self.lr, self.beta1, self.beta2)
             adev = self.hyper.data_ptr()
         if self.lazy:
             self._lazy_update(adev)
             return
         if self.algo == "rank1":
-            rc = self.lib.g2v_cbow_r1_update(self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._ptr(self.m_ih),
-                                             self._ptr(self.v_ih), self._ptr(self.m_ho), self._ptr(self.v_ho),
-                                             self.c.data_ptr(), self.g_ho.data_ptr(), self.s.data_ptr(), self.V,
-                                             self.D, self.opt, self.lr, self.beta1, self.beta2, self.eps, self.t,
-                                             adev, self._stream())
-            _capi.check(rc, "g2v_cbow_r1_update")
+            self._launch("g2v_cbow_r1_update", self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._ptr(self.m_ih),
+                         self._ptr(self.v_ih), self._ptr(self.m_ho), self._ptr(self.v_ho), self.c.data_ptr(),
+                         self.g_ho.data_ptr(), self.s.data_ptr(), self.V, self.D, self.opt, self.lr, self.beta1,
+                         self.beta2, self.eps, self.t, adev)
             return
         if self.nvl:
             # gradient exchange fused with the optimizer: barrier (every rank's gradient complete) -> reduce-scatter +
             # Adam on the owned slice + all-gather of the new weights in ONE kernel -> barrier (weights delivered)
             nv = self.nvl
             nv["hg"].barrier(channel=0)
-            rc = self.lib.g2v_cbow_update_nvl(nv["hg"].buffer_ptrs_dev, nv["hw"].buffer_ptrs_dev, nv["g_mc"], nv["w_mc"],
-                                              self._ptr(self.m_flat), self._ptr(self.v_flat),
-                                              self.V * self.D + self.D, nv["rank"], nv["world"], self.opt, self.lr,
-                                              self.beta1, self.beta2, self.eps, self.t, adev, self._stream())
-            _capi.check(rc, "g2v_cbow_update_nvl")
+            self._launch("g2v_cbow_update_nvl", nv["hg"].buffer_ptrs_dev, nv["hw"].buffer_ptrs_dev, nv["g_mc"],
+                         nv["w_mc"], self._ptr(self.m_flat), self._ptr(self.v_flat), self.V * self.D + self.D,
+                         nv["rank"], nv["world"], self.opt, self.lr, self.beta1, self.beta2, self.eps, self.t, adev)
             nv["hg"].barrier(channel=1)
             return
-        rc = self.lib.g2v_cbow_update(self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._ptr(self.m_ih),
-                                      self._ptr(self.v_ih), self._ptr(self.m_ho), self._ptr(self.v_ho),
-                                      self.g_ih.data_ptr(), self.g_ho.data_ptr(), self.V, self.D, self.opt,
-                                      self.lr, self.beta1, self.beta2, self.eps, self.t, adev, self._stream())
-        _capi.check(rc, "g2v_cbow_update")
+        self._launch("g2v_cbow_update", self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._ptr(self.m_ih),
+                     self._ptr(self.v_ih), self._ptr(self.m_ho), self._ptr(self.v_ho), self.g_ih.data_ptr(),
+                     self.g_ho.data_ptr(), self.V, self.D, self.opt, self.lr, self.beta1, self.beta2, self.eps, self.t,
+                     adev)
 
     def evaluate(self, win, slot, win_begin=0, n_win=None):
         """Add the number of correctly classified listed windows into acc[slot]."""
-        n = (win.shape[0] - win_begin) if n_win is None else n_win
-        if self.algo == "rank1":
-            rc = self.lib.g2v_cbow_r1_windows(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
-                                              self._ptr(win), int(win_begin), int(n), 0.0, self.s.data_ptr(), 0, 0,
-                                              self.acc.data_ptr() + 8 * slot, self.V, self.reduce, self._stream())
-            _capi.check(rc, "g2v_cbow_r1_windows")
-            return
-        ws = self._slab_ws(win, win_begin, n)
-        if ws is not None:
-            rc = self.lib.g2v_cbow_eval_slabs(self.gene.data_ptr(), self.label.data_ptr(), self._ptr(win),
-                                              int(win_begin), int(n), self.W_ih.data_ptr(), self.W_ho.data_ptr(),
-                                              self.acc.data_ptr() + 8 * slot, self.V, self.D, self.reduce,
-                                              self._n_slabs, ws.data_ptr(), self._stream())
-            _capi.check(rc, "g2v_cbow_eval_slabs")
-            return
-        rc = self.lib.g2v_cbow_eval(self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
-                                    self._ptr(win), int(win_begin), int(n), self.W_ih.data_ptr(),
-                                    self.W_ho.data_ptr(), self.acc.data_ptr() + 8 * slot, self.V, self.D,
-                                    self.reduce, self._stream())
-        _capi.check(rc, "g2v_cbow_eval")
+        lo = int(win_begin)
+        n = int((win.shape[0] - win_begin) if n_win is None else n_win)
+        rec = self.prepared(win)
+        # the accuracy pass has no backward: it routes as the plain forward does (rank1, or rows with or without slabs)
+        r = choose_route(self.algo, False, False, rec, lo, n)
+        acc = self.acc.data_ptr() + 8 * slot
+        if r in ("r1", "r1_csc"):
+            self._launch("g2v_cbow_r1_windows", self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+                         self._ptr(win), lo, n, 0.0, self.s.data_ptr(), 0, 0, acc, self.V, self.reduce)
+        elif r == "slabs":
+            self._launch("g2v_cbow_eval_slabs", self.gene.data_ptr(), self.label.data_ptr(), self._ptr(win), lo, n,
+                         self.W_ih.data_ptr(), self.W_ho.data_ptr(), acc, self.V, self.D, self.reduce, self._n_slabs,
+                         rec.slabs[(lo, n)].data_ptr())
+        else:
+            self._launch("g2v_cbow_eval", self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+                         self._ptr(win), lo, n, self.W_ih.data_ptr(), self.W_ho.data_ptr(), acc, self.V, self.D,
+                         self.reduce)
 
     def loss_sum(self, acc_host):
         return float(acc_host[:1].view(torch.float64)[0])
+
+
+def check_config(algo, optimizer, deterministic, several_gpus=False, batch=0, reshuffle=False):
+    """Refuse (ValueError) what train_cbow and CbowModel cannot run, before any device work.  ``several_gpus``: a
+    process group of more than one rank; ``batch`` and ``reshuffle`` as train_cbow takes them."""
+    if algo not in ("rows", "rank1"):
+        raise ValueError("algo must be 'rows' (gather/scatter of embedding rows) or 'rank1' (collapsed)")
+    if reshuffle and batch <= 0:
+        raise ValueError("reshuffle=True needs mini-batches (batch > 0)")
+    if deterministic and several_gpus:
+        raise ValueError("deterministic=True runs on one GPU only")
+    if deterministic and algo == "rank1" and batch > 0:
+        raise ValueError("deterministic=True with algo='rank1' needs a full batch: rank1's mini-batch c uses atomics")
+    if optimizer == "lazy_adam" and algo != "rows":
+        raise ValueError("optimizer='lazy_adam' needs algo='rows' (rank1 keeps s = W_ih.W_ho, which every W_ho step "
+                         "changes for every gene)")
+    if optimizer == "lazy_adam" and several_gpus:
+        raise ValueError("optimizer='lazy_adam' runs on one GPU only")
+
+
+class _WindowList:
+    """What a CbowModel prepared for one window list.  It holds the list (None: every window of the table), so the
+    list's address, the model's key for it, cannot be reused for another list while the record exists."""
+
+    def __init__(self, win, n):
+        self.win, self.n = win, n
+        self.cscptr = self.pos = self.dO = None      # prepare_csc: the whole list's CSC and its dO per list position
+        self.slabs = {}                              # prepare_slabs: (win_begin, n_win) -> slab workspace
+        self.plan, self.B, self.brp = None, 0, None  # prepare_batches: _PlanBuffers, batch size, row offset per batch
+
+    def whole(self, win_begin, n):
+        return self.cscptr is not None and win_begin == 0 and n == self.n
+
+    def batch(self, win_begin, n):
+        """(first row, number of rows) of planned batch [win_begin, win_begin + n) in the plan, else None."""
+        if self.brp is None or win_begin % self.B or n != min(self.B, self.n - win_begin):
+            return None
+        k = win_begin // self.B
+        if not 0 <= k < len(self.brp) - 1:
+            return None
+        return self.brp[k], self.brp[k + 1] - self.brp[k]
+
+
+def choose_route(algo, lazy, det, rec, win_begin, n, identity=False):
+    """The launches (DESIGN.md §4.14) CbowModel.fwdbwd runs for windows [win_begin, win_begin + n) of a list whose
+    _WindowList is ``rec`` (None: nothing prepared; ``identity``: the list is None, every window of the table).  A
+    lazy or deterministic batch that was not planned raises RuntimeError: nothing falls back to the scatter."""
+    def unplanned(mode):
+        return RuntimeError("%s: windows [%d, %d) of this list were not given to prepare_batches"
+                            % (mode, win_begin, win_begin + n))
+    if lazy:
+        if rec is None or rec.batch(win_begin, n) is None:
+            raise unplanned("optimizer='lazy_adam'")
+        return "batch_lazy"
+    whole = rec is not None and rec.whole(win_begin, n)
+    if algo == "rank1":
+        return "r1_csc" if whole else "r1"
+    if det:
+        if whole:
+            return "csc_det"
+        if identity:
+            raise RuntimeError("deterministic=True: fwdbwd needs a window list given to prepare_csc or prepare_batches")
+        if rec is None or rec.batch(win_begin, n) is None:
+            raise unplanned("deterministic=True")
+        return "batch_det"
+    if rec is not None and (win_begin, n) in rec.slabs:
+        return "slabs"
+    return "csc" if whole else "scatter"
 
 
 def _nvl_setup(group, n_flat, dev):
@@ -477,7 +506,7 @@ class _PlanBuffers:
     sized once from the list's incidence count, which no reordering of the list changes."""
 
     def __init__(self, model, win, B):
-        self.m, self.win, self.n, self.B = model, win, int(win.shape[0]), int(B)
+        self.m, self.n, self.B = model, int(win.shape[0]), int(B)
         w = win.to(torch.int64)
         self.nnz = int((model.rowptr[w + 1] - model.rowptr[w]).sum())
         dev, i32 = model.device, torch.int32
@@ -489,18 +518,14 @@ class _PlanBuffers:
         nbytes = int(model.lib.g2v_cbow_batch_plan_workspace_bytes(self.n, self.nnz, self.B, model.V))
         self.ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
 
-    def launch(self, win):
-        """Enqueue the build for ``win`` (same length as the list this was sized for); no host synchronisation."""
-        m = self.m
-        _capi.check(m.lib.g2v_cbow_batch_plan(m.rowptr.data_ptr(), m.gene.data_ptr(), win.data_ptr(), self.n, self.nnz,
-                                              self.B, m.V, self.rows.data_ptr(), self.segptr.data_ptr(),
-                                              self.pos.data_ptr(), self.brp.data_ptr(), self.ws.data_ptr(),
-                                              m._stream()), "g2v_cbow_batch_plan")
-
     def build(self, win):
-        """launch(win), then read the per-batch row offsets back (the only host synchronisation); returns (rows,
-        segptr, pos) cut to their sizes and the row offsets as int64 NumPy [n_b + 1]."""
-        self.launch(win)
+        """Build the plan of ``win`` (same length as the list this was sized for), then read the per-batch row offsets
+        back (the only host synchronisation); returns (rows, segptr, pos) cut to their sizes and the row offsets as
+        int64 NumPy [n_b + 1]."""
+        m = self.m
+        m._launch("g2v_cbow_batch_plan", m.rowptr.data_ptr(), m.gene.data_ptr(), win.data_ptr(), self.n, self.nnz,
+                  self.B, m.V, self.rows.data_ptr(), self.segptr.data_ptr(), self.pos.data_ptr(), self.brp.data_ptr(),
+                  self.ws.data_ptr())
         brp = self.brp.cpu().numpy().astype(np.int64)
         if brp[-1] < 0:
             raise RuntimeError("g2v_cbow_batch_plan: the list has more incidences than it was sized for")
@@ -625,18 +650,8 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     graphs, at every table size (no gene slabs).  Mini-batch adam/sgd then build per-batch plans as lazy_adam does.
     algo="rank1" is already reproducible with a full batch and is accepted unchanged; with ``batch > 0`` it is an error.
     """
-    if reshuffle and batch <= 0:
-        raise ValueError("reshuffle=True needs mini-batches (batch > 0)")
     dist = _dist()
-    if deterministic and dist:
-        raise ValueError("deterministic=True runs on one GPU only (world size %d)" % dist.get_world_size())
-    if deterministic and algo == "rank1" and batch > 0:
-        raise ValueError("deterministic=True with algo='rank1' needs a full batch: rank1's mini-batch c uses atomics")
-    if optimizer == "lazy_adam" and algo != "rows":
-        raise ValueError("optimizer='lazy_adam' needs algo='rows' (rank1 keeps s = W_ih.W_ho, which every W_ho step "
-                         "changes for every gene)")
-    if optimizer == "lazy_adam" and dist:
-        raise ValueError("optimizer='lazy_adam' runs on one GPU only (world size %d)" % dist.get_world_size())
+    check_config(algo, optimizer, deterministic, several_gpus=dist is not None, batch=batch, reshuffle=reshuffle)
     world, rank = (dist.get_world_size(), dist.get_rank()) if dist else (1, 0)
     rowptr_np = (win_rowptr.cpu().numpy() if isinstance(win_rowptr, torch.Tensor) else np.asarray(win_rowptr))
     N = rowptr_np.shape[0] - 1
@@ -685,6 +700,7 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     out = out.cpu().numpy()
     if return_info:
         return out, {"history": hist, "stop_step": stop, "n_train": n_tr, "n_val": n_va, "model": model,
+                     "windows": (tr_d, va_d),
                      "graph": bool(getattr(model, "loop_used_graph", False)), "exchange": model.exchange() if dist else None}
     return out
 
@@ -737,9 +753,8 @@ class DeviceLoop:
     def __init__(self, model, dist, tr_d, va_d, n_tr, max_epoch, early_stop, snapshot=True):
         self.m, self.dist, self.tr_d, self.va_d, self.n_tr = model, dist, tr_d, va_d, n_tr
         self.n_tr_loc, self.n_va_loc = int(tr_d.shape[0]), int(va_d.shape[0])
-        self.carried = (dist is None and model.algo == "rows" and not model.lazy and self.n_tr_loc > 0
-                        and model._slab_ws(tr_d, 0, self.n_tr_loc) is None
-                        and model._csc_for(tr_d, 0, self.n_tr_loc) is not None)
+        self.carried = (dist is None and not model.lazy and self.n_tr_loc > 0
+                        and model.route(tr_d) in ("csc", "csc_det"))
         dev = model.device
         self.ctl = torch.zeros(8, dtype=torch.int64, device=dev)
         n_hist = max(max_epoch, 1) * 4
@@ -764,12 +779,8 @@ class DeviceLoop:
         self.max_epoch, self.early_stop = int(max_epoch), bool(early_stop)
         self.reset()
 
-    def _st(self):
-        return torch.cuda.current_stream(self.m.device).cuda_stream
-
     def reset(self):
-        _capi.check(self.m.lib.g2v_cbow_loop_init(self.ctl.data_ptr(), self.max_epoch, int(self.early_stop), self._st()),
-                    "g2v_cbow_loop_init")
+        self.m._launch("g2v_cbow_loop_init", self.ctl.data_ptr(), self.max_epoch, int(self.early_stop))
         if self.carried:                             # drop a pending carry: its g_ho partial would be added twice
             self.m.g_ho.zero_()
             self.m.acc[4:].zero_()
@@ -787,10 +798,9 @@ class DeviceLoop:
     def one(self, show, m_fb=None, m_upd=None, m_val=None):
         """Enqueue one iteration (the optional events mark the end of fwd+bwd, of the update, of the validation pass).
         In carried mode ``show`` changes nothing: ACC[tr] comes from the tail pass on every step."""
-        m, lib, dist = self.m, self.m.lib, self.dist
-        _capi.check(lib.g2v_cbow_loop_begin(self.ctl.data_ptr(), m.acc.data_ptr(), m.W_ih.data_ptr(),
-                                            None if self.result is None else self.result.data_ptr(), m.V * m.D,
-                                            self._st()), "g2v_cbow_loop_begin")
+        m, dist = self.m, self.dist
+        m._launch("g2v_cbow_loop_begin", self.ctl.data_ptr(), m.acc.data_ptr(), m.W_ih.data_ptr(),
+                  None if self.result is None else self.result.data_ptr(), m.V * m.D)
         if self.n_tr_loc:
             m.fwdbwd(self.tr_d, self.n_tr)       # acc[1] += correct predictions with the PRE-update weights
                                                  # (carried: the forward is skipped on the device, acc[1] carried)
@@ -806,33 +816,20 @@ class DeviceLoop:
             m.evaluate(self.va_d, 2)
         if m_val is not None:
             m_val.record()
-        if self.carried and m.det:
-            _capi.check(lib.g2v_cbow_loop_tail_det(self.ctl.data_ptr(), m.rowptr.data_ptr(), m.gene.data_ptr(),
-                                                   m.label.data_ptr(), self.tr_d.data_ptr(), self.n_tr_loc,
-                                                   1.0 / float(self.n_tr), m.W_ih.data_ptr(), m.W_ho.data_ptr(),
-                                                   m._csc[4].data_ptr(), m.g_ho.data_ptr(), m.acc.data_ptr(), m.V, m.D,
-                                                   m.reduce, m.det_workspace(self.n_tr_loc).data_ptr(), 0, self._st()),
-                        "g2v_cbow_loop_tail_det")
-        elif self.carried:
-            csc = m._csc
-            _capi.check(lib.g2v_cbow_loop_tail(self.ctl.data_ptr(), m.rowptr.data_ptr(), m.gene.data_ptr(),
-                                               m.label.data_ptr(), self.tr_d.data_ptr(), self.n_tr_loc,
-                                               1.0 / float(self.n_tr), m.W_ih.data_ptr(), m.W_ho.data_ptr(),
-                                               csc[4].data_ptr(), m.g_ho.data_ptr(), m.acc.data_ptr(), m.V, m.D,
-                                               m.reduce, self._st()), "g2v_cbow_loop_tail")
+        if self.carried:
+            m.loop_tail(self.ctl, self.tr_d, self.n_tr)
         elif show and self.n_tr_loc:
             m.evaluate(self.tr_d, 3)
         acc_ptr = m.acc.data_ptr()
         if self.hist_nvl:
             hn = self.hist_nvl
-            _capi.check(lib.g2v_cbow_loop_counters_nvl(self.ctl.data_ptr(), acc_ptr, hn["h"].buffer_ptrs_dev, hn["mc"],
-                                                       m.nvl["world"], self._st()), "g2v_cbow_loop_counters_nvl")
+            m._launch("g2v_cbow_loop_counters_nvl", self.ctl.data_ptr(), acc_ptr, hn["h"].buffer_ptrs_dev, hn["mc"],
+                      m.nvl["world"])
             hn["h"].barrier(channel=3)
             acc_ptr = None                           # decide on the sums already in hist[step]
         elif dist:
             dist.all_reduce(m.acc[1:4])
-        _capi.check(lib.g2v_cbow_loop_decide(self.ctl.data_ptr(), acc_ptr, self.hist_d.data_ptr(), self._st()),
-                    "g2v_cbow_loop_decide")
+        m._launch("g2v_cbow_loop_decide", self.ctl.data_ptr(), acc_ptr, self.hist_d.data_ptr())
 
     def fetch(self):
         self.ctl_pin.copy_(self.ctl, non_blocking=True)

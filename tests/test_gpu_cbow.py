@@ -507,13 +507,14 @@ def test_slab_passes_equal_oracle_and_fused_kernel(g2v, monkeypatch, D, reduce, 
     assert rel_max(m.W_ih.cpu().numpy(), f.W_ih.cpu().numpy()) < RTOL_VEC
 
 
-def test_slab_training_run_equals_the_reference_golden(g2v, monkeypatch):
+def test_slab_training_run_routes_both_lists_to_slabs_and_equals_the_golden(g2v, monkeypatch):
     """The whole loop (train_cbow: CUDA-graph replays, early stop) on slab passes against the reference run."""
     monkeypatch.setenv("G2V_CBOW_SLABS", "3")
     g = helpers.cbow_golden("cbow_ex.npz")
     got, info = g2v.train_cbow(g["rowptr"], g["gene"], g["label"], g["V"], g["D"], g["lr"], max_epoch=500,
                                seed=g["seed"], log=None, return_info=True)
-    assert info["model"]._n_slabs == 3 and len(info["model"]._slabs) == 2
+    m = info["model"]
+    assert m._n_slabs == 3 and all(m.prepared(w).slabs and m.route(w) == "slabs" for w in info["windows"])
     assert info["stop_step"] == g["stop_step"]
     assert rel_max(got, g["W_ref"]) < RTOL_VEC
 

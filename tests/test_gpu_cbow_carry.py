@@ -46,7 +46,7 @@ def host_step(m, tr_d, va_d):
 
 
 @pytest.mark.parametrize("D", [128, 100])
-def test_tail_pass_is_the_next_forward_bit_for_bit(g2v, D):
+def test_tail_pass_writes_the_records_dO_as_the_next_forward_bit_for_bit(g2v, D):
     import torch
     from g2vec_b200 import cbow
     m, tr_d, va_d = setup(g2v, D)
@@ -60,15 +60,15 @@ def test_tail_pass_is_the_next_forward_bit_for_bit(g2v, D):
     finally:
         loop.detach()
     acc = m.acc.cpu()
-    dO_tail = m._csc[4].clone()
+    dO_tail = m.prepared(tr_d).dO.clone()
     # the same weights, a fresh model, the full CSC forward + expansion with no loop attached
     r, r_tr, _ = setup(g2v, D, W=(m.W_ih.cpu().numpy(), m.W_ho.cpu().numpy()))
-    assert r._csc_for(r_tr, 0, n) is not None and torch.equal(r_tr, tr_d)
+    assert r.route(r_tr) == "csc" and torch.equal(r_tr, tr_d)
     r.fwdbwd(r_tr, n)
     r.evaluate(r_tr, 3)
     torch.cuda.synchronize()
     racc = r.acc.cpu()
-    assert torch.equal(dO_tail, r._csc[4])
+    assert torch.equal(dO_tail, r.prepared(r_tr).dO)
     assert int(acc[3]) == int(acc[5]) == int(racc[1]) == int(racc[3])
     assert abs(m.loss_sum(acc[4:]) - r.loss_sum(racc)) <= 1e-9 * abs(r.loss_sum(racc))
     assert rel_max(m.g_ho.cpu().numpy(), r.g_ho.cpu().numpy()) < 1e-5
@@ -82,7 +82,7 @@ def test_tail_pass_is_the_next_forward_bit_for_bit(g2v, D):
     assert torch.equal(m.g_ih, r.g_ih)
 
 
-def test_pending_carry_skips_the_forward_and_feeds_the_expansion(g2v):
+def test_pending_carry_skips_the_forward_and_feeds_the_records_expansion(g2v):
     import torch
     from g2vec_b200 import cbow
     m, tr_d, va_d = setup(g2v, 128, seed=5)
@@ -92,7 +92,7 @@ def test_pending_carry_skips_the_forward_and_feeds_the_expansion(g2v):
     try:
         loop.one(True)
         torch.cuda.synchronize()
-        dO = m._csc[4]
+        dO = m.prepared(tr_d).dO
         dO[7] = 1000.0                                     # poisoned: a forward would overwrite it
         want_dO = dO.clone()
         acc0, g_ho0 = m.acc.clone(), m.g_ho.clone()
@@ -102,7 +102,7 @@ def test_pending_carry_skips_the_forward_and_feeds_the_expansion(g2v):
         loop.detach()
     assert torch.equal(dO, want_dO)
     assert torch.equal(m.acc, acc0) and torch.equal(m.g_ho, g_ho0)   # no loss, count or g_ho added
-    cscptr, pos = m._csc[2].long(), m._csc[3].long()
+    cscptr, pos = m.prepared(tr_d).cscptr.long(), m.prepared(tr_d).pos.long()
     seg = torch.repeat_interleave(torch.arange(m.V, device="cuda"), cscptr[1:] - cscptr[:-1])
     c = torch.zeros(m.V, dtype=torch.float64, device="cuda").index_add_(0, seg, want_dO[pos].double())
     want = (c[:, None] * m.W_ho.double()[None, :]).cpu().numpy()
@@ -177,3 +177,45 @@ def test_graph_captured_after_reset_equals_eager_steps(g2v):
     # g_ho's atomics differ between the two runs; Adam magnifies that noise on near-zero W_ho components
     assert rel_max(a.W_ih.cpu().numpy(), b.W_ih.cpu().numpy()) < 1e-5
     assert rel_max(a.W_ho.cpu().numpy(), b.W_ho.cpu().numpy()) < 1e-4
+
+
+@pytest.mark.parametrize("det", [False, True])
+def test_preparing_another_list_leaves_the_loop_step_unchanged(g2v, det):
+    """A loop built on tr_d, then prepare_csc of a longer list: the loop's steps still run tr_d's CSC forward, carry
+    and tail, so two steps count, carry and expand what the same steps without that prepare do."""
+    import torch
+    from g2vec_b200 import cbow
+    V, N, D = 500, 4000, 128
+    rowptr, gene, label = helpers.random_windows(N, V - 20, 1, 60, seed=13)
+    W0, Wo0 = helpers.init_weights(V, D, 13)
+    tr, va = cbow.split_indices(N, 13)
+    tr_d = torch.from_numpy(tr.astype(np.int32)).cuda()
+    va_d = torch.from_numpy(va.astype(np.int32)).cuda()
+    other = torch.cat([tr_d, va_d])
+    n = len(tr_d)
+    out = []
+    for extra in (True, False):
+        m = g2v.CbowModel(rowptr, gene, label, V, D, W0, Wo0, lr=0.005, deterministic=det)
+        m.prepare_csc(tr_d)
+        loop = cbow.DeviceLoop(m, None, tr_d, va_d, n, 10, False, snapshot=False)
+        assert loop.carried
+        if extra:
+            m.prepare_csc(other)
+            assert m.route(tr_d) == ("csc_det" if det else "csc") and m.prepared(tr_d).n == n
+        loop.attach()
+        try:
+            for _ in range(2):
+                loop.one(True)
+            loop.fetch()
+            m.fwdbwd(tr_d, n)                              # the third step's expansion of the carried dO
+            torch.cuda.synchronize()
+        finally:
+            loop.detach()
+        out.append((loop.hist_pin.view(-1, 4)[:2, 1:].tolist(), m.g_ih.cpu().numpy(), m.W_ih.cpu().numpy()))
+    (h1, g1, w1), (h2, g2, w2) = out
+    if det:
+        assert h1 == h2 and g1.tobytes() == g2.tobytes() and w1.tobytes() == w2.tobytes()
+    else:
+        for x, y in zip(h1, h2):
+            assert all(abs(p - q) <= 2 for p, q in zip(x, y)), (h1, h2)
+        assert rel_max(g1, g2) < 1e-5 and rel_max(w1, w2) < 1e-5

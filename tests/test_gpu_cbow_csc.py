@@ -94,7 +94,7 @@ def test_csc_backward_equals_oracle_and_scatter_kernel(g2v, D, reduce):
     assert (m.g_ih.cpu().numpy() == g_ih).all()
 
 
-def test_train_cbow_rows_runs_the_csc_backward(g2v, monkeypatch):
+def test_train_cbow_rows_routes_its_training_list_to_the_csc_backward(g2v, monkeypatch):
     """Full-batch train_cbow(algo="rows") prepares the transposed incidence of its training list and every step's
     backward goes through g2v_cbow_fwdbwd_csc; with gene slabs it is not prepared (the slab passes run instead)."""
     from g2vec_b200 import _capi
@@ -113,11 +113,35 @@ def test_train_cbow_rows_runs_the_csc_backward(g2v, monkeypatch):
     for use_graph in (True, False):
         got, info = g2v.train_cbow(g["rowptr"], g["gene"], g["label"], g["V"], g["D"], g["lr"], max_epoch=500,
                                    seed=g["seed"], log=None, return_info=True, use_graph=use_graph)
-        assert info["model"]._csc is not None and info["stop_step"] == g["stop_step"]
+        m, (tr_d, _) = info["model"], info["windows"]
+        assert m.prepared(tr_d).whole(0, len(tr_d)) and m.route(tr_d) == "csc" and info["stop_step"] == g["stop_step"]
         assert rel_max(got, g["W_ref"]) < 1e-4
     assert calls["csc"] >= g["stop_step"] and calls["scatter"] == 0
     monkeypatch.setenv("G2V_CBOW_SLABS", "3")
     ex = helpers.cbow_golden("cbow_ex.npz")
     _, info = g2v.train_cbow(ex["rowptr"], ex["gene"], ex["label"], ex["V"], ex["D"], ex["lr"], max_epoch=3,
                              seed=ex["seed"], early_stop=False, log=None, return_info=True)
-    assert info["model"]._n_slabs == 3 and getattr(info["model"], "_csc", None) is None
+    m = info["model"]
+    assert m._n_slabs == 3 and all(m.prepared(w).cscptr is None and m.route(w) == "slabs" for w in info["windows"])
+
+
+def test_a_freed_list_does_not_lend_its_csc_to_a_new_list(g2v):
+    """prepare_csc(a), drop a, then a list b of the same length: the caching allocator may hand b a's block, but the
+    model still holds a, so b is not taken for a prepared list and fwdbwd(b) runs the scatter."""
+    import torch
+    V, N, D, n = 500, 3000, 128, 2400
+    rowptr, gene, label = helpers.random_windows(N, V, 1, 60, seed=21)
+    W0, Wo0 = helpers.init_weights(V, D, 2)
+    m = g2v.CbowModel(rowptr, gene, label, V, D, W0, Wo0)
+    a = torch.from_numpy(np.random.RandomState(0).permutation(N)[:n].astype(np.int32)).cuda()
+    m.prepare_csc(a)
+    del a
+    b = torch.from_numpy(np.random.RandomState(1).permutation(N)[:n].astype(np.int32)).cuda()
+    assert m.route(b) == "scatter"
+    m.fwdbwd(b, n)
+    f = g2v.CbowModel(rowptr, gene, label, V, D, W0, Wo0)
+    f.fwdbwd(b, n)
+    torch.cuda.synchronize()
+    assert rel_max(m.g_ih.cpu().numpy(), f.g_ih.cpu().numpy()) < 2e-5
+    assert rel_max(m.g_ho.cpu().numpy(), f.g_ho.cpu().numpy()) < 2e-5
+    assert int(m.acc[1]) == int(f.acc[1])

@@ -36,7 +36,7 @@ def _windows(N, V, unused, seed):
 
 @pytest.mark.parametrize("reduce", ["sum", "mean"])
 @pytest.mark.parametrize("D", [128, 256, 512, 100])
-def test_forward_is_grid_independent_and_matches_the_atomic_path(g2v, D, reduce):
+def test_det_forward_on_a_prepared_record_is_grid_independent_and_matches_the_atomic_path(g2v, D, reduce):
     import torch
     from g2vec_b200 import _capi
     lib = _capi.load()
@@ -48,7 +48,7 @@ def test_forward_is_grid_independent_and_matches_the_atomic_path(g2v, D, reduce)
     wd = torch.from_numpy(win.astype(np.int32)).cuda()
     m = g2v.CbowModel(rowptr, gene, label, V, D, W0, Wo0, reduce=reduce, deterministic=True)
     m.prepare_csc(wd)
-    csc = m._csc
+    rec = m.prepared(wd)
     ws = m.det_workspace(n_list)
     st = torch.cuda.current_stream().cuda_stream
     red = {"sum": 0, "mean": 1}[reduce]
@@ -60,7 +60,7 @@ def test_forward_is_grid_independent_and_matches_the_atomic_path(g2v, D, reduce)
         l0 = _capi.launch_count()
         _capi.check(lib.g2v_cbow_fwdbwd_csc_det(m.rowptr.data_ptr(), m.gene.data_ptr(), m.label.data_ptr(),
                                                 wd.data_ptr(), n_list, 1.0 / N, m.W_ih.data_ptr(), m.W_ho.data_ptr(),
-                                                csc[2].data_ptr(), csc[3].data_ptr(), dO.data_ptr(), g_ih.data_ptr(),
+                                                rec.cscptr.data_ptr(), rec.pos.data_ptr(), dO.data_ptr(), g_ih.data_ptr(),
                                                 g_ho.data_ptr(), acc.data_ptr(), acc.data_ptr() + 8, V, D, red,
                                                 ws.data_ptr(), max_ctas, st), "g2v_cbow_fwdbwd_csc_det")
         torch.cuda.synchronize()
@@ -77,7 +77,7 @@ def test_forward_is_grid_independent_and_matches_the_atomic_path(g2v, D, reduce)
     f.prepare_csc(wd)
     f.fwdbwd(wd, N)
     torch.cuda.synchronize()
-    assert rel_max(dO, f._csc[4].cpu().numpy()) < 1e-5
+    assert rel_max(dO, f.prepared(wd).dO.cpu().numpy()) < 1e-5
     assert rel_max(g_ih, f.g_ih.cpu().numpy()) < 2e-5 and rel_max(g_ho, f.g_ho.cpu().numpy()) < 2e-5
     assert abs(loss - f.loss_sum(f.acc.cpu())) < 1e-5 * abs(loss)
     assert int(acc[1]) == int(f.acc.cpu()[1])
@@ -210,7 +210,7 @@ def test_batch_expansion_matches_the_scatter(g2v):
             det.fwdbwd(wd, 10, win_begin=3, n_win=10)
 
 
-def test_large_tables_train_single_pass(g2v, monkeypatch):
+def test_large_tables_route_deterministic_runs_to_the_single_pass(g2v, monkeypatch):
     monkeypatch.setenv("G2V_CBOW_SLABS", "3")
     ex = helpers.cbow_golden("cbow_ex.npz")
     args = (ex["rowptr"], ex["gene"], ex["label"], ex["V"], ex["D"], ex["lr"])
@@ -218,7 +218,8 @@ def test_large_tables_train_single_pass(g2v, monkeypatch):
     slab, si = g2v.train_cbow(*args, **kw)
     assert si["model"]._n_slabs == 3
     det, di = g2v.train_cbow(*args, deterministic=True, **kw)
-    assert not hasattr(di["model"], "_n_slabs") and di["model"]._csc is not None
+    tr_d = di["windows"][0]
+    assert di["model"].prepared(tr_d).slabs == {} and di["model"].route(tr_d) == "csc_det"
     assert rel_max(det, slab) < RTOL_VEC
 
 

@@ -105,7 +105,7 @@ def test_batch_plan_on_the_ex_windows(g2v):
         _check_plan(m, ro.epoch_list(tr, 0, 1), B)
 
 
-def test_prepare_batches_keeps_one_plan_per_list(g2v):
+def test_prepare_batches_keeps_one_plan_in_the_lists_record(g2v):
     """A second prepare_batches for the same list replaces its plan (and releases the buffers of the first batch
     size); the new plan is the builder's for the new batch size."""
     import torch
@@ -119,7 +119,7 @@ def test_prepare_batches_keeps_one_plan_per_list(g2v):
     m.prepare_batches(wd, 100)
     with pytest.raises(KeyError):
         m.batch_touched(wd, 64, 64)
-    assert len(m._plan_bufs) == 1
+    assert m.prepared(wd).plan.B == m.prepared(wd).B == 100
     _, _, _, brp = ro.batch_plan_torch(m.rowptr, m.gene, V, wd, 100)
     assert [m.batch_touched(wd, k * 100, 100) for k in range(10)] == list(np.diff(brp))
 
