@@ -58,6 +58,8 @@ SIGNATURES = {
     "g2v_cbow_loop_tail": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32,
                                           _vp]),
     "g2v_cbow_loop_decide": (ctypes.c_int, [_vp, _vp, _vp, _vp]),
+    "g2v_cbow_loop_decide_best": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp]),
+    "g2v_cbow_loop_keep_best": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp]),
     "g2v_cbow_loop_counters_nvl": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _vp]),
     "g2v_cbow_slab_plan": (ctypes.c_int, [_i32, _i32, _vp]),
     "g2v_cbow_slab_workspace_bytes": (ctypes.c_size_t, [_i64, _i32, _i32]),

@@ -407,9 +407,11 @@ class CbowModel:
         return float(acc_host[:1].view(torch.float64)[0])
 
 
-def check_config(algo, optimizer, deterministic, several_gpus=False, batch=0, reshuffle=False):
+def check_config(algo, optimizer, deterministic, several_gpus=False, batch=0, reshuffle=False, patience=1):
     """Refuse (ValueError) what train_cbow and CbowModel cannot run, before any device work.  ``several_gpus``: a
-    process group of more than one rank; ``batch`` and ``reshuffle`` as train_cbow takes them."""
+    process group of more than one rank; ``batch``, ``reshuffle`` and ``patience`` as train_cbow takes them."""
+    if isinstance(patience, bool) or not isinstance(patience, (int, np.integer)) or patience < 1:
+        raise ValueError("patience must be an int >= 1 (the number of bad epochs in a row that stops the run)")
     if algo not in ("rows", "rank1"):
         raise ValueError("algo must be 'rows' (gather/scatter of embedding rows) or 'rank1' (collapsed)")
     if reshuffle and batch <= 0:
@@ -616,9 +618,15 @@ def _dist():
 
 def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500, seed=0, optimizer="adam",
                reduce="sum", W_ih0=None, W_ho0=None, split=None, early_stop=True, log=print, return_info=False,
-               eval_train="lazy", algo="rows", batch=0, use_graph=True, reshuffle=False, deterministic=False):
+               eval_train="lazy", algo="rows", batch=0, use_graph=True, reshuffle=False, deterministic=False,
+               patience=1):
     """Train the modified CBOW on CSR windows and return W_ih (np.float32 [n_genes, hidden]) exactly as
     ``compute_genetovec`` does: the weights after the last step whose validation accuracy did not drop.
+
+    ``patience`` (int >= 1, with ``early_stop``): the best validation count so far is tracked, a step whose count is
+    >= the best becomes the best (ties: the later step), and the run stops at the ``patience``-th step in a row below
+    the best (DESIGN.md §4.15).  The result is the best step's W_ih, also when the run ends at ``max_epoch``.  The
+    default 1 is the reference's rule: stop at the first drop, return the weights from before it.
 
     ``max_epoch`` is the reference's ``--epoch`` (parsed at G2Vec.py:515 but ignored there; the loop is
     hard-coded ``range(500)`` at :262) -- the default 500 reproduces the reference.
@@ -649,9 +657,13 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     and for any launch grid -- every optimizer, full batch or mini-batches, with or without ``reshuffle`` and CUDA
     graphs, at every table size (no gene slabs).  Mini-batch adam/sgd then build per-batch plans as lazy_adam does.
     algo="rank1" is already reproducible with a full batch and is accepted unchanged; with ``batch > 0`` it is an error.
+
+    ``return_info=True`` also returns a dict: ``history`` [(step, ACC[val], ACC[tr])], ``stop_step`` (the step where
+    the run stopped early, else None), ``best_step`` (the step whose W_ih is returned; None if no step ran), and more.
     """
     dist = _dist()
-    check_config(algo, optimizer, deterministic, several_gpus=dist is not None, batch=batch, reshuffle=reshuffle)
+    check_config(algo, optimizer, deterministic, several_gpus=dist is not None, batch=batch, reshuffle=reshuffle,
+                 patience=patience)
     world, rank = (dist.get_world_size(), dist.get_rank()) if dist else (1, 0)
     rowptr_np = (win_rowptr.cpu().numpy() if isinstance(win_rowptr, torch.Tensor) else np.asarray(win_rowptr))
     N = rowptr_np.shape[0] - 1
@@ -687,19 +699,21 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     if log:
         log("     Start training the modified CBOW with early stopping")
     if max_epoch <= 0:                           # no optimizer step at all: the initial vectors
-        out, hist, stop = model.W_ih, [], None
+        out, hist, stop, best = model.W_ih, [], None, None
     elif full_batch:
-        out, hist, stop = _device_loop(model, dist, tr_d, va_d, n_tr, n_va, len(tr_loc), len(va_loc), max_epoch,
-                                       early_stop, log, eval_train, use_graph)
+        out, hist, stop, best = _device_loop(model, dist, tr_d, va_d, n_tr, n_va, len(tr_loc), len(va_loc), max_epoch,
+                                             early_stop, log, eval_train, use_graph, patience=patience)
     else:
-        out, hist, stop = _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, len(tr_loc), len(va_loc),
-                                          max_epoch, early_stop, log, batch,
-                                          reshuffle=(tr_all, seed, rank) if reshuffle else None)
+        out, hist, stop, best = _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, len(tr_loc), len(va_loc),
+                                                max_epoch, early_stop, log, batch,
+                                                reshuffle=(tr_all, seed, rank) if reshuffle else None,
+                                                patience=patience)
     if log:
         log("    Optimization Finish")
     out = out.cpu().numpy()
     if return_info:
-        return out, {"history": hist, "stop_step": stop, "n_train": n_tr, "n_val": n_va, "model": model,
+        return out, {"history": hist, "stop_step": stop, "best_step": best, "n_train": n_tr, "n_val": n_va,
+                     "model": model,
                      "windows": (tr_d, va_d),
                      "graph": bool(getattr(model, "loop_used_graph", False)), "exchange": model.exchange() if dist else None}
     return out
@@ -707,12 +721,21 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
 
 class _LoopLog:
     """The host side of the reference loop body after the three session runs (G2Vec.py:268-283): log line every
-    5th step, the Epoch(stop) line, the history.  Fed one step at a time with the step's counters."""
+    5th step, the Epoch(stop) line, the history.  Fed one step at a time with the step's counters.
 
-    def __init__(self, n_tr, n_va, log):
+    It also follows the early-stop rule with ``patience`` (DESIGN.md §4.15) on the integer validation counts, as
+    g2v_cbow_loop_decide[_best] do: ``best_step`` is the step whose weights the loop returns.  ``patience=None``: no
+    early stopping, every step is the new best (the loop returns the last weights)."""
+
+    def __init__(self, n_tr, n_va, log, patience=1):
         self.n_tr, self.n_va, self.log = n_tr, n_va, log
         self.hist, self.t0 = [], time.time()
-        self.before_val, self.before_tr = np.float32(-1.0), np.float32(0.0)
+        self.patience = patience
+        self.best_val, self.best_step, self.bad = -1, None, 0
+
+    def stops(self, acc):
+        """Whether a step with counters ``acc`` ends the run under the rule (host-driven loops decide with this)."""
+        return self.patience is not None and int(acc[2]) < self.best_val and self.bad + 1 >= self.patience
 
     def step(self, step, acc, shown, stopped_here):
         f32 = np.float32
@@ -722,20 +745,30 @@ class _LoopLog:
         hist, log = self.hist, self.log
         if hist and hist[-1][2] is None:
             hist[-1] = (hist[-1][0], hist[-1][1], float(acc_tr_prev))
-        if hist:
-            self.before_tr = hist[-1][2]                            # ACC[tr] of the previous step (G2Vec.py:281)
         hist.append((step, float(acc_val), None if acc_tr is None else float(acc_tr)))
+        if self.patience is None or int(acc[2]) >= self.best_val:
+            self.best_val, self.best_step, self.bad = int(acc[2]), step, 0
+        else:
+            self.bad += 1
         if step % 5 == 0 and log:
             t1 = time.time()
             log("    - Epoch: %03d\tACC[val]=%.4f\tACC[tr]=%.4f (%.3f sec)" % (step, acc_val, acc_tr, t1 - self.t0))
             self.t0 = time.time()
         if stopped_here:
+            # the best step's accuracies; its ACC[tr] is in the history by now (step-1's was filled in above)
             if log:
+                b = hist[self.best_step]
                 log("    - Epoch(stop): %03d\tACC[val]=%.4f\tACC[tr]=%.4f (%.3f sec)"
-                    % (step - 1, self.before_val, self.before_tr, time.time() - self.t0))
+                    % (b[0], b[1], b[2], time.time() - self.t0))
             return True
-        self.before_val = acc_val
         return False
+
+    def end(self):
+        """After a run that reached max_epoch: the Epoch(best) line if the best step is not the last one, which only
+        patience > 1 allows.  Call it once the last step's ACC[tr] is in the history."""
+        if self.log and self.hist and self.best_step != self.hist[-1][0]:
+            b = self.hist[self.best_step]
+            self.log("    - Epoch(best): %03d\tACC[val]=%.4f\tACC[tr]=%.4f" % b)
 
 
 class DeviceLoop:
@@ -748,9 +781,16 @@ class DeviceLoop:
     forward, so the next fwdbwd only expands its dO into g_ih.  The training list is gathered once per step instead
     of twice.  This assumes the training windows do not change between steps: the list is static, and a
     WindowFeeder re-uploads the same windows every step.  The first step after reset() runs the full forward,
-    decided on the device, so a graph captured right after reset() is correct from its first replay."""
+    decided on the device, so a graph captured right after reset() is correct from its first replay.
 
-    def __init__(self, model, dist, tr_d, va_d, n_tr, max_epoch, early_stop, snapshot=True):
+    Patience (``early_stop`` with ``patience`` > 1, DESIGN.md §4.15): no snapshot at the start of a step; the decision
+    is g2v_cbow_loop_decide_best, followed by g2v_cbow_loop_keep_best, which copies W_ih into ``result`` on the steps
+    that improve on the best validation count.  ``result`` then holds the best step's weights however the loop ends."""
+
+    # the smallest patience that takes the keep-best kernels; tests lower it to 1 to check them against the default rule
+    keep_best_from = 2
+
+    def __init__(self, model, dist, tr_d, va_d, n_tr, max_epoch, early_stop, snapshot=True, patience=1):
         self.m, self.dist, self.tr_d, self.va_d, self.n_tr = model, dist, tr_d, va_d, n_tr
         self.n_tr_loc, self.n_va_loc = int(tr_d.shape[0]), int(va_d.shape[0])
         self.carried = (dist is None and not model.lazy and self.n_tr_loc > 0
@@ -774,13 +814,21 @@ class DeviceLoop:
             self.hist_d = torch.zeros(n_hist, dtype=torch.int64, device=dev)
         self.ctl_pin = torch.zeros(8, dtype=torch.int64).pin_memory()
         self.hist_pin = torch.zeros(max(max_epoch, 1) * 4, dtype=torch.int64).pin_memory()
-        # snapshot buffer: W_ih before the step being decided (only an early stop ever returns it)
-        self.result = model.W_ih.clone() if snapshot else None
-        self.max_epoch, self.early_stop = int(max_epoch), bool(early_stop)
+        self.max_epoch, self.early_stop, self.patience = int(max_epoch), bool(early_stop), int(patience)
+        # best: {patience, best_step, bad_steps, improved} of the keep-best path, else None
+        self.best = self.best_pin = None
+        if self.early_stop and self.patience >= self.keep_best_from:
+            self.best = torch.zeros(4, dtype=torch.int64, device=dev)
+            self.best_pin = torch.zeros(4, dtype=torch.int64).pin_memory()
+        # default path: W_ih before the step being decided (only an early stop ever returns it); keep-best path: W_ih
+        # of the best step so far
+        self.result = model.W_ih.clone() if (snapshot or self.best is not None) else None
         self.reset()
 
     def reset(self):
         self.m._launch("g2v_cbow_loop_init", self.ctl.data_ptr(), self.max_epoch, int(self.early_stop))
+        if self.best is not None:
+            self.best.copy_(torch.tensor([self.patience, -1, 0, 0], dtype=torch.int64))
         if self.carried:                             # drop a pending carry: its g_ho partial would be added twice
             self.m.g_ho.zero_()
             self.m.acc[4:].zero_()
@@ -800,7 +848,7 @@ class DeviceLoop:
         In carried mode ``show`` changes nothing: ACC[tr] comes from the tail pass on every step."""
         m, dist = self.m, self.dist
         m._launch("g2v_cbow_loop_begin", self.ctl.data_ptr(), m.acc.data_ptr(), m.W_ih.data_ptr(),
-                  None if self.result is None else self.result.data_ptr(), m.V * m.D)
+                  None if (self.result is None or self.best is not None) else self.result.data_ptr(), m.V * m.D)
         if self.n_tr_loc:
             m.fwdbwd(self.tr_d, self.n_tr)       # acc[1] += correct predictions with the PRE-update weights
                                                  # (carried: the forward is skipped on the device, acc[1] carried)
@@ -829,11 +877,19 @@ class DeviceLoop:
             acc_ptr = None                           # decide on the sums already in hist[step]
         elif dist:
             dist.all_reduce(m.acc[1:4])
-        m._launch("g2v_cbow_loop_decide", self.ctl.data_ptr(), acc_ptr, self.hist_d.data_ptr())
+        if self.best is None:
+            m._launch("g2v_cbow_loop_decide", self.ctl.data_ptr(), acc_ptr, self.hist_d.data_ptr())
+        else:
+            m._launch("g2v_cbow_loop_decide_best", self.ctl.data_ptr(), self.best.data_ptr(), acc_ptr,
+                      self.hist_d.data_ptr())
+            m._launch("g2v_cbow_loop_keep_best", self.best.data_ptr(), m.W_ih.data_ptr(), self.result.data_ptr(),
+                      m.V * m.D)
 
     def fetch(self):
         self.ctl_pin.copy_(self.ctl, non_blocking=True)
         self.hist_pin.copy_(self.hist_d, non_blocking=True)
+        if self.best is not None:
+            self.best_pin.copy_(self.best, non_blocking=True)
 
     def capture(self, pattern):
         """The iterations of `pattern` (list of show flags) + the status read-back as one CUDA graph."""
@@ -848,17 +904,19 @@ class DeviceLoop:
 
 
 def _device_loop(model, dist, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_epoch, early_stop, log, eval_train,
-                 use_graph, chunk=5):
+                 use_graph, chunk=5, patience=1):
     """Full-batch loop of G2Vec.py:262-283 with the early-stop rule, the result snapshot and the step counter on
     the DEVICE (g2v_cbow_loop_*): the host enqueues `chunk` iterations at a time -- one CUDA-graph replay of
     4 plain iterations + 1 that also runs the training-accuracy pass (in carried mode, five identical iterations
     that all have it) -- and synchronises once per printed line instead of once per step.  Iterations enqueued after
     the stop are no-ops (every kernel tests ctl.stopped).  Multi-GPU: the all-reduces are part of the captured graph
-    (NCCL is capturable); if capture is refused the same launches run eagerly."""
+    (NCCL is capturable); if capture is refused the same launches run eagerly.  Returns (W_ih to return, history,
+    stop step or None, best step)."""
     dev = model.device
-    loop = DeviceLoop(model, dist, tr_d, va_d, n_tr, max_epoch, early_stop, snapshot=bool(early_stop))
+    loop = DeviceLoop(model, dist, tr_d, va_d, n_tr, max_epoch, early_stop, snapshot=bool(early_stop),
+                      patience=patience)
     shown = lambda s: loop.carried or s % 5 == 0 or eval_train == "always"
-    info = _LoopLog(n_tr, n_va, log)
+    info = _LoopLog(n_tr, n_va, log, patience if early_stop else None)
 
     def consume(lo, hi):
         """Host view of steps lo..hi-1 after a sync; True when the loop is over."""
@@ -908,22 +966,27 @@ def _device_loop(model, dist, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_ep
             a = model.acc.cpu()
             last = info.hist[-1]
             info.hist[-1] = (last[0], last[1], float(np.float32(int(a[3])) / np.float32(max(n_tr, 1))))
+        if stop is None:
+            info.end()
     finally:
         loop.detach()
     model.loop_used_graph = graph is not None
+    if loop.best is not None:                    # keep-best path: result holds the best step's weights in every case
+        return loop.result, info.hist, stop, int(loop.best_pin[1])
     # stopped early: the snapshot taken before the dropping step (G2Vec.py:283,286); else the final weights
-    return (loop.result if stop is not None else model.W_ih), info.hist, stop
+    return (loop.result if stop is not None else model.W_ih), info.hist, stop, info.best_step
 
 
 def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_epoch, early_stop, log, batch,
-                    reshuffle=None):
+                    reshuffle=None, patience=1):
     """north_star's mini-batch variant: one optimizer step (and one gradient all-reduce) per batch of the shuffled
     training list, the reference's per-epoch accuracies and early stop around it; host-driven, one sync per epoch.
     ``reshuffle`` = (global training list on the device, seed, rank): every epoch e >= 1 trains on this rank's share of
     the epoch's order, written into one preallocated buffer (g2v_cbow_epoch_order); lazy_adam then rebuilds the
-    buffer's batch plans (one more sync), as does the deterministic mode."""
+    buffer's batch plans (one more sync), as does the deterministic mode.  The early-stop rule with ``patience`` is
+    applied on the host after the epoch's sync; the result is copied on the epochs that improve on the best."""
     dev = model.device
-    info = _LoopLog(n_tr, n_va, log)
+    info = _LoopLog(n_tr, n_va, log, patience if early_stop else None)
     result = model.W_ih.clone()
     stop = None
     per = -(-batch // world)
@@ -955,12 +1018,14 @@ def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_l
         if dist:
             dist.all_reduce(model.acc[1:4])
         acc = model.acc.cpu()                                    # the epoch's only host sync
-        dropped = bool(early_stop) and (np.float32(int(acc[2])) / np.float32(max(n_va, 1))) < info.before_val
-        if info.step(step, acc, True, dropped):
+        if info.step(step, acc, True, info.stops(acc)):
             stop = step
             break
-        result.copy_(model.W_ih)
-    return result, info.hist, stop
+        if info.best_step == step:
+            result.copy_(model.W_ih)
+    if stop is None:
+        info.end()
+    return result, info.hist, stop, info.best_step
 
 
 def compute_genetovec(pathList, n_genes, hidden_size, learning_rate, max_epoch=500, seed=0, log=print):

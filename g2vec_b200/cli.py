@@ -8,6 +8,11 @@ steps (the reference parses it, :515, and then loops ``range(500)``, :262 -- the
 reference behaviour), and ``--seed`` (default 0) seeds the walk sampler, the path glue, the split and the
 initial vectors (the reference is unseeded).
 
+``--patience K`` (default 1, the reference's rule) keeps training through up to K-1 epochs in a row whose validation
+accuracy is below the best so far, stops at the K-th, and writes the vectors of the best epoch (ties: the later one);
+the ``Epoch(stop)`` line then names the best epoch, and a run that reaches ``--epoch`` with a better earlier epoch
+prints an ``Epoch(best)`` line (DESIGN.md §4.15).
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle``, at every table size (DESIGN.md §4.13);
@@ -53,7 +58,13 @@ def parse_arguments(argv=None):
     p.add_argument('--deterministic', action='store_true',
                    help="bit-reproducible training on one GPU: every floating-point sum of a step in a fixed order "
                         "(rows: any optimizer and batch size; rank1: full batch only); somewhat slower")
+    p.add_argument('--patience', type=int, default=1,
+                   help="early stopping: stop after this many epochs in a row whose validation accuracy is below the "
+                        "best so far, and write the vectors of the best epoch; 1 (default) = the reference's rule, "
+                        "stop at the first drop")
     args = p.parse_args(argv)
+    if args.patience < 1:
+        p.error("--patience must be an integer >= 1")
     if args.reshuffle and args.batch <= 0:
         p.error("--reshuffle needs mini-batches (--batch B with B > 0)")
     if args.deterministic and args.algo == 'rank1' and args.batch > 0:
@@ -255,7 +266,7 @@ def main(argv=None):
     mat = cbow.train_cbow(w_rowptr, w_gene, w_label, n_genes, args.sizeHiddenlayer, args.learningRate,
                           max_epoch=args.epoch, seed=args.seed, log=print, algo=args.algo,   # print is silent off rank 0
                           batch=args.batch, optimizer=args.optimizer, reshuffle=args.reshuffle,
-                          deterministic=args.deterministic)
+                          deterministic=args.deterministic, patience=args.patience)
     genes = data['gene']
     if rank != 0:
         dist.barrier()

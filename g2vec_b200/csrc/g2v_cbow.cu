@@ -867,6 +867,45 @@ __global__ void loop_counters_nvl_kernel(const long long *__restrict__ ctl, cons
     __threadfence_system();
 }
 
+// ---- early stopping with patience (DESIGN.md §4.15) ------------------------------------------------------------
+// best (int64 x 4 in device memory, kept apart from ctl): {patience, best_step, bad_steps, improved}.  ctl[3] holds
+// the best validation count so far, which is the previous step's count whenever patience is 1.
+// loop_decide_best: loop_decide with the patience rule -- a count >= the best is the new best (ties: the later step),
+//   a lower one is a bad step, and the patience-th bad step in a row stops the loop.  `improved` says whether THIS
+//   step's weights must be kept; it is cleared on the no-op steps enqueued after the stop.
+// loop_keep_best: copy W_ih into `result` if `improved`.  It does not test `stopped`: the step that ends the loop at
+//   max_steps can be the best one.
+__global__ void loop_decide_best_kernel(long long *__restrict__ ctl, long long *__restrict__ best,
+                                        const long long *__restrict__ acc, long long *__restrict__ hist) {
+    if (ctl[0] != 0) {
+        best[3] = 0;
+        return;
+    }
+    const long long step = ctl[1];
+    if (acc)
+        for (int k = 0; k < 4; ++k) hist[step * 4 + k] = acc[k];
+    const long long val = hist[step * 4 + 2];
+    if (val >= ctl[3]) {
+        ctl[3] = val; best[1] = step; best[2] = 0; best[3] = 1;
+    } else {
+        best[2] += 1; best[3] = 0;
+        if (ctl[5] != 0 && best[2] >= best[0]) {
+            ctl[0] = 1; ctl[2] = step;               // the patience-th bad step: the kept weights are the result
+        }
+    }
+    if (step + 1 >= ctl[4]) ctl[0] = 1;              // ran --epoch steps
+    ctl[1] = step + 1;
+}
+
+__global__ void __launch_bounds__(256)
+loop_keep_best_kernel(const long long *__restrict__ best, const float4 *__restrict__ W4, float4 *__restrict__ R4,
+                      int64_t n4, const float *__restrict__ W, float *__restrict__ R, int64_t n) {
+    if (best[3] == 0) return;
+    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = tid; i < n4; i += nth) R4[i] = W4[i];
+    for (int64_t i = (n4 << 2) + tid; i < n; i += nth) R[i] = W[i];
+}
+
 }  // namespace g2v
 
 using namespace g2v;
@@ -919,6 +958,31 @@ extern "C" int g2v_cbow_loop_decide(int64_t *ctl, const int64_t *acc, int64_t *h
     loop_decide_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(reinterpret_cast<long long *>(ctl),
                                                           reinterpret_cast<const long long *>(acc),
                                                           reinterpret_cast<long long *>(hist));
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_loop_decide_best(int64_t *ctl, int64_t *best, const int64_t *acc, int64_t *hist, void *stream) {
+    G2V_REQUIRE(ctl && best && hist, "g2v_cbow_loop_decide_best: null pointer");
+    loop_decide_best_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(
+        reinterpret_cast<long long *>(ctl), reinterpret_cast<long long *>(best),
+        reinterpret_cast<const long long *>(acc), reinterpret_cast<long long *>(hist));
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_loop_keep_best(const int64_t *best, const float *W_ih, float *result, int64_t n, void *stream) {
+    G2V_REQUIRE(best && W_ih && result && n >= 0, "g2v_cbow_loop_keep_best: bad arguments");
+    DeviceProps dp;
+    if (device_props(&dp)) return 1;
+    int64_t blocks = (n / 4 + 255) / 256;
+    if (blocks > (int64_t)dp.sm_count * 8) blocks = (int64_t)dp.sm_count * 8;
+    if (blocks < 1) blocks = 1;
+    loop_keep_best_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
+        reinterpret_cast<const long long *>(best), reinterpret_cast<const float4 *>(W_ih),
+        reinterpret_cast<float4 *>(result), n >> 2, W_ih, result, n);
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;

@@ -262,6 +262,20 @@ int g2v_cbow_loop_tail(int64_t *ctl, const int32_t *rowptr, const int32_t *gene,
                        const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
                        float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D, int32_t reduce, void *stream);
 int g2v_cbow_loop_decide(int64_t *ctl, const int64_t *acc, int64_t *hist, void *stream);
+/* Early stopping with patience (DESIGN.md §4.15): the loop keeps the weights of its best step instead of a snapshot.
+ *   best [4] int64 in device memory: {patience, best_step, bad_steps, improved}; the caller sets {K, -1, 0, 0}
+ *        after g2v_cbow_loop_init (K >= 1).  ctl.before_val then holds the best validation count so far.
+ *   g2v_cbow_loop_decide_best: in place of g2v_cbow_loop_decide (same acc / hist forms).  If stopped, clears
+ *        `improved` and returns.  Else records the counters, and a validation count >= the best so far makes this
+ *        step the best (improved = 1, bad_steps = 0); a lower count adds one bad step (improved = 0), and with
+ *        ctl.early_stop set the K-th bad step in a row stops the loop with stop_step = step.  Stops after max_steps;
+ *        step += 1.  With K = 1 it decides exactly as g2v_cbow_loop_decide.
+ *   g2v_cbow_loop_keep_best: after it, copies W_ih [n floats] into `result` if `improved`.  It does not test
+ *        ctl.stopped (the step that reaches max_steps may be the best one), so `result` ends as W_ih of best_step.
+ * Pass snapshot = NULL to g2v_cbow_loop_begin on this path.  Neither call depends on a host value that changes between
+ * steps or synchronises, so both are captured in the loop's CUDA graphs. */
+int g2v_cbow_loop_decide_best(int64_t *ctl, int64_t *best, const int64_t *acc, int64_t *hist, void *stream);
+int g2v_cbow_loop_keep_best(const int64_t *best, const float *W_ih, float *result, int64_t n, void *stream);
 /* Multi-GPU, hist in symmetric memory (zero-initialised, same size on every rank): add this rank's acc[1..3] into
  * hist[step][1..3] of every rank (multimem.red through hist_multicast, or system-scope atomics on hist_ptrs_dev);
  * after a cross-GPU barrier call g2v_cbow_loop_decide with acc == NULL, which then decides on the summed counters
