@@ -52,6 +52,8 @@ SIGNATURES = {
                                            _f32, _i32, _vp, _vp]),
     "g2v_cbow_adam_tick": (ctypes.c_int, [_vp, _f32, _f32, _f32, _vp]),
     "g2v_cbow_eval": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "g2v_cbow_eval_certified": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
+                                               _i32, _i32, _vp]),
     "g2v_cbow_loop_init": (ctypes.c_int, [_vp, _i64, _i32, _vp]),
     "g2v_cbow_loop_attach": (ctypes.c_int, [_vp]),
     "g2v_cbow_loop_begin": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp]),

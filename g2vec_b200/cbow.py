@@ -110,6 +110,8 @@ class CbowModel:
         self.lr, self.beta1, self.beta2, self.eps = float(lr), float(beta1), float(beta2), float(eps)
         z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
         self.algo = algo
+        # rows: scratch of the certified accuracy pass, {s[g], t[g]} per gene (g2v_cbow_eval_certified)
+        self.st = z(2 * self.V) if algo == "rows" else None
         if self.lazy:
             self.g_ih, self.g_ho = None, z(self.D)
             self.g_flat = self.g_ho
@@ -399,9 +401,10 @@ class CbowModel:
                          self.W_ih.data_ptr(), self.W_ho.data_ptr(), acc, self.V, self.D, self.reduce, self._n_slabs,
                          rec.slabs[(lo, n)].data_ptr())
         else:
-            self._launch("g2v_cbow_eval", self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
-                         self._ptr(win), lo, n, self.W_ih.data_ptr(), self.W_ho.data_ptr(), acc, self.V, self.D,
-                         self.reduce)
+            # the count g2v_cbow_eval gives, rows gathered only for windows a float32 bound cannot decide (§4.16)
+            self._launch("g2v_cbow_eval_certified", self.rowptr.data_ptr(), self.gene.data_ptr(),
+                         self.label.data_ptr(), self._ptr(win), lo, n, self.W_ih.data_ptr(), self.W_ho.data_ptr(),
+                         self.st.data_ptr(), acc, None, self.V, self.D, self.reduce, 0)
 
     def loss_sum(self, acc_host):
         return float(acc_host[:1].view(torch.float64)[0])

@@ -54,8 +54,6 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
     G2V_SKIP_IF_STOPPED(carried);
     constexpr bool BACKWARD = MODE != kRowsEval;
     constexpr int D = 128 * VEC;
-    constexpr int D4 = D / 4;
-    constexpr int UNR = 8 / VEC;                 // 8 float4 (128 B) in flight per lane
     __shared__ float sh_gho[BACKWARD ? D : 1];
     __shared__ CtaAcc sh_acc;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -79,37 +77,8 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
         const int32_t b = __ldg(rowptr + n), e = __ldg(rowptr + n + 1);
         const float y = (float)__ldg(label + n);
         float4 h[VEC];
-#pragma unroll
-        for (int v = 0; v < VEC; ++v) h[v] = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int32_t base = b; base < e; base += 32) {
-            const int cnt = min(32, e - base);
-            const int32_t g = (lane < cnt) ? __ldg(gene + base + lane) : 0;
-            for (int k = 0; k < cnt; k += UNR) {
-                float4 r[UNR][VEC];
-#pragma unroll
-                for (int u = 0; u < UNR; ++u) {
-                    const int32_t gk = __shfl_sync(0xffffffffu, g, (k + u) & 31);
-                    const float4 *row = W4 + (size_t)gk * D4 + lane;
-#pragma unroll
-                    for (int v = 0; v < VEC; ++v)
-                        r[u][v] = (k + u < cnt) ? ldg4(row + v * 32) : make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-#pragma unroll
-                for (int u = 0; u < UNR; ++u)
-#pragma unroll
-                    for (int v = 0; v < VEC; ++v) {
-                        h[v].x += r[u][v].x; h[v].y += r[u][v].y; h[v].z += r[u][v].z; h[v].w += r[u][v].w;
-                    }
-            }
-        }
-        const float scale = (reduce_mean && e > b) ? 1.f / (float)(e - b) : 1.f;
-        float part = 0.f;
-#pragma unroll
-        for (int v = 0; v < VEC; ++v) {
-            if (reduce_mean) { h[v].x *= scale; h[v].y *= scale; h[v].z *= scale; h[v].w *= scale; }
-            part += h[v].x * who[v].x + h[v].y * who[v].y + h[v].z * who[v].z + h[v].w * who[v].w;
-        }
-        const float o = warp_sum(part);
+        float scale;
+        const float o = rows_logit<VEC>(gene, W4, b, e, lane, reduce_mean, who, h, scale);
         if (lane == 0) {
             correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
             if (BACKWARD) loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
@@ -174,18 +143,8 @@ cbow_rows_generic_kernel(const int32_t *__restrict__ rowptr, const int32_t *__re
         const int64_t n = win ? (int64_t)__ldg(win + win_begin + i) : win_begin + i;
         const int32_t b = __ldg(rowptr + n), e = __ldg(rowptr + n + 1);
         const float y = (float)__ldg(label + n);
-        for (int d = lane; d < D; d += 32) h[d] = 0.f;
-        for (int32_t j = b; j < e; ++j) {
-            const float *row = W_ih + (size_t)__ldg(gene + j) * D;
-            for (int d = lane; d < D; d += 32) h[d] += __ldg(row + d);
-        }
-        const float scale = (reduce_mean && e > b) ? 1.f / (float)(e - b) : 1.f;
-        float part = 0.f;
-        for (int d = lane; d < D; d += 32) {
-            if (reduce_mean) h[d] *= scale;
-            part += h[d] * __ldg(W_ho + d);
-        }
-        const float o = warp_sum(part);
+        float scale;
+        const float o = rows_generic_logit(gene, W_ih, W_ho, b, e, lane, D, reduce_mean, h, scale);
         if (lane == 0) {
             correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
             if (BACKWARD) loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
@@ -213,6 +172,123 @@ cbow_rows_generic_kernel(const int32_t *__restrict__ rowptr, const int32_t *__re
     if (threadIdx.x == 0) {
         if (BACKWARD && loss_sum) atomicAdd(loss_sum, sh_acc.loss);
         if (n_correct) atomicAdd(n_correct, sh_acc.correct);
+    }
+}
+
+// ---- certified accuracy pass (DESIGN.md §4.16) ----------------------------------------------------------------
+// The count of (o > 0) == y over the windows, the same integer cbow_rows_kernel's eval mode gives, from the collapsed
+// logit o' = scale * sum_{g in n} s[g] where it provably has o's sign.  st[g] = {s[g], t[g]} (r1_prepare_kernel<true>):
+// s[g] = <W_ih[g,:], W_ho>, t[g] = sum_d |W_ih[g,d] W_ho[d]|.  Both o and o' are float32 evaluations of the same real
+// number with at most k = l + D + 16 roundings on any term's path, so |o - o'| <= certified_tau(T, scale, l, D, A)
+// with T = sum_{g in n} t[g] and A = sum_d |W_ho[d]|; a window with |o'| > tau is decided by o', every other one
+// (empty, tau or o' not finite, |o'| within the band) gets o from rows_logit / rows_generic_logit, the code
+// cbow_rows_kernel runs.  The absolute term covers underflowing products: each product of o and o' may lose 2^-150,
+// and in o the product scale * h[d] (mean) is then multiplied by W_ho[d], so its loss counts |W_ho[d]| times.
+__device__ __forceinline__ float certified_tau(float T, float scale, int32_t l, int32_t D, float A) {
+    const int64_t k = (int64_t)l + D + 16;
+    if (!(T <= 0x1p126f) || k > (1 << 22)) return __int_as_float(0x7f800000);
+    const float rel = __fmul_rn(__fmul_rn((float)k, 0x1p-21f), scale);           // 8 k u s, u = 2^-24
+    // 32 ((l + 3) D + A) 2^-150; A = +inf or NaN makes tau so, and the window is gathered
+    const float abs_ = __fmul_rn(__fadd_rn((float)(((int64_t)l + 3) * D), A), 0x1p-145f);
+    return __fadd_rn(__fmul_rn(rel, T), abs_);
+}
+
+// 8 lanes per window, 4 windows per warp (r1_windows_kernel's layout) for o' and T; then the whole warp gathers the
+// rows of each undecided window of the four in turn.  VEC > 0: D = 128 * VEC; VEC == 0: any D, h in shared memory
+// ([kCbowWarps][D], dynamic).  force_gather: every window takes the row gather (tests).  n_gathered (nullable): the
+// number of windows that took it.
+template <int VEC>
+__global__ void __launch_bounds__(kCbowWarps * 32)
+cbow_eval_certified_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
+                           const uint8_t *__restrict__ label, const int32_t *__restrict__ win, int64_t win_begin,
+                           int64_t n_win, const float *__restrict__ W_ih, const float *__restrict__ W_ho,
+                           const float2 *__restrict__ st, unsigned long long *__restrict__ n_correct,
+                           unsigned long long *__restrict__ n_gathered, int32_t D, int32_t reduce_mean,
+                           int32_t force_gather, const int32_t *__restrict__ skip) {
+    G2V_SKIP_IF_STOPPED(skip);
+    constexpr int NV = VEC > 0 ? VEC : 1;
+    extern __shared__ float shf[];
+    __shared__ unsigned long long sh_cnt[2];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int sub = lane & 7, slot = lane >> 3;
+    if (threadIdx.x < 2) sh_cnt[threadIdx.x] = 0ull;
+    __syncthreads();
+    const float4 *__restrict__ W4 = reinterpret_cast<const float4 *>(W_ih);
+    float4 who[NV];
+    if (VEC > 0) {
+#pragma unroll
+        for (int v = 0; v < NV; ++v) who[v] = ldg4(reinterpret_cast<const float4 *>(W_ho) + v * 32 + lane);
+    }
+    float *h_generic = shf + (size_t)warp * D;
+    // A = sum_d |W_ho[d]| (certified_tau's underflow term).  VEC > 0: from the lanes' who, summed where it is first
+    // needed, so that the warp does not wait for W_ho before its first window's loads are issued
+    float A = 0.f;
+    if (VEC == 0) {
+        for (int d = lane; d < D; d += 32) A += fabsf(__ldg(W_ho + d));
+        A = warp_sum(A);
+    }
+    unsigned correct_acc = 0, gathered_acc = 0;
+    const int64_t stride = (int64_t)gridDim.x * kCbowWarps * 4;
+    for (int64_t base = ((int64_t)blockIdx.x * kCbowWarps + warp) * 4; base < n_win; base += stride) {
+        const int64_t i = base + slot;
+        const bool active = i < n_win;
+        int32_t b = 0, e = 0;
+        float y = 0.f;
+        if (active) {
+            const int64_t n = win ? (int64_t)__ldg(win + win_begin + i) : win_begin + i;
+            b = __ldg(rowptr + n); e = __ldg(rowptr + n + 1);
+            y = (float)__ldg(label + n);
+        }
+        float ps = 0.f, pt = 0.f;
+        for (int32_t j = b + sub; j < e; j += 8) {
+            const float2 q = __ldg(st + __ldg(gene + j));
+            ps += q.x; pt += q.y;
+        }
+#pragma unroll
+        for (int o = 4; o > 0; o >>= 1) {
+            ps += __shfl_xor_sync(0xffffffffu, ps, o);
+            pt += __shfl_xor_sync(0xffffffffu, pt, o);
+        }
+        if (VEC > 0) {
+            A = 0.f;
+#pragma unroll
+            for (int v = 0; v < NV; ++v)
+                A += (fabsf(who[v].x) + fabsf(who[v].y)) + (fabsf(who[v].z) + fabsf(who[v].w));
+            A = warp_sum(A);
+        }
+        const float scale = (reduce_mean && e > b) ? 1.f / (float)(e - b) : 1.f;
+        const float o1 = ps * scale;
+        const bool decided = !force_gather && fabsf(o1) <= 0x1.fffffep127f
+                             && fabsf(o1) > certified_tau(pt, scale, e - b, D, A);
+        if (active && sub == 0 && decided) correct_acc += ((o1 > 0.f) == (y != 0.f)) ? 1u : 0u;
+        unsigned todo = __ballot_sync(0xffffffffu, active && sub == 0 && !decided);
+        while (todo) {
+            const int src = __ffs(todo) - 1;
+            todo &= todo - 1;
+            const int32_t wb = __shfl_sync(0xffffffffu, b, src), we = __shfl_sync(0xffffffffu, e, src);
+            const float wy = __shfl_sync(0xffffffffu, y, src);
+            float wscale, o;
+            if (VEC > 0) {
+                float4 h[NV];
+                o = rows_logit<NV>(gene, W4, wb, we, lane, reduce_mean, who, h, wscale);
+            } else {
+                o = rows_generic_logit(gene, W_ih, W_ho, wb, we, lane, D, reduce_mean, h_generic, wscale);
+            }
+            if (lane == 0) {
+                correct_acc += ((o > 0.f) == (wy != 0.f)) ? 1u : 0u;
+                ++gathered_acc;
+            }
+        }
+    }
+    correct_acc = __reduce_add_sync(0xffffffffu, correct_acc);
+    if (lane == 0) {
+        atomicAdd(&sh_cnt[0], (unsigned long long)correct_acc);
+        atomicAdd(&sh_cnt[1], (unsigned long long)gathered_acc);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        atomicAdd(n_correct, sh_cnt[0]);
+        if (n_gathered) atomicAdd(n_gathered, sh_cnt[1]);
     }
 }
 
@@ -1137,6 +1213,45 @@ extern "C" int g2v_cbow_eval(const int32_t *rowptr, const int32_t *gene, const u
     if (n_win == 0) return 0;
     return launch_rows<false>(rowptr, gene, label, win, win_begin, n_win, 0.f, W_ih, W_ho, nullptr, nullptr,
                               nullptr, n_correct, D, reduce, (cudaStream_t)stream);
+}
+
+extern "C" int g2v_cbow_eval_certified(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                       const int32_t *win, int64_t win_begin, int64_t n_win, const float *W_ih,
+                                       const float *W_ho, float *st, int64_t *n_correct, int64_t *n_gathered,
+                                       int32_t V, int32_t D, int32_t reduce, int32_t force_gather, void *stream) {
+    G2V_REQUIRE(V > 0 && D > 0 && n_win >= 0 && win_begin >= 0, "g2v_cbow_eval_certified: bad sizes");
+    G2V_REQUIRE(rowptr && label && W_ih && W_ho && st && n_correct, "g2v_cbow_eval_certified: null pointer");
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "g2v_cbow_eval_certified: unknown reduce %d",
+                reduce);
+    if (n_win == 0) return 0;
+    cudaStream_t s = (cudaStream_t)stream;
+    const bool generic = D != 128 && D != 256 && D != 512;
+    const size_t smem = generic ? (size_t)kCbowWarps * D * sizeof(float) : 0;
+    if (generic) {
+        // the D range of g2v_cbow_eval: its generic kernel holds h and the g_ho partial, 2 D floats per warp
+        DeviceProps dp;
+        if (device_props(&dp)) return 1;
+        cudaFuncAttributes fa;
+        G2V_CUDA_OK(cudaFuncGetAttributes(&fa, cbow_rows_generic_kernel<false>));
+        G2V_REQUIRE((size_t)kCbowWarps * 2 * D * sizeof(float) + fa.sharedSizeBytes <= (size_t)dp.max_smem_optin,
+                    "sizeHiddenlayer %d too large for the generic kernel", D);
+        G2V_CUDA_OK(cudaFuncSetAttribute(cbow_eval_certified_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem));
+    }
+    int rc = launch_r1_prepare(W_ih, W_ho, st, V, D, true, s);
+    if (rc) return rc;
+    auto kern = D == 128 ? cbow_eval_certified_kernel<1> : D == 256 ? cbow_eval_certified_kernel<2>
+              : D == 512 ? cbow_eval_certified_kernel<4> : cbow_eval_certified_kernel<0>;
+    int grid = 0;
+    if ((rc = rows_grid((const void *)kern, smem, (n_win + 3) / 4, &grid))) return rc;
+    kern<<<grid, kCbowWarps * 32, smem, s>>>(rowptr, gene, label, win, win_begin, n_win, W_ih, W_ho,
+                                            reinterpret_cast<const float2 *>(st),
+                                            reinterpret_cast<unsigned long long *>(n_correct),
+                                            reinterpret_cast<unsigned long long *>(n_gathered), D,
+                                            reduce == G2V_REDUCE_MEAN, force_gather, loop_skip_flag());
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
 }
 
 __global__ void adam_tick_kernel(float *state, float lr, float beta1, float beta2, const int32_t *skip) {

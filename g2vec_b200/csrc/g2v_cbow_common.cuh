@@ -67,8 +67,74 @@ __device__ __forceinline__ void cta_epilogue(float *sh_gho, CtaAcc &sh_acc, cons
     }
 }
 
+// The row-gather logit of one window, genes gene[b..e), the whole warp: h = sum of the window's W_ih rows (lane owns
+// VEC float4 of the row, D = 128*VEC), scaled by the window's scale (1, or 1/l for the mean), o = <h, W_ho> by a lane
+// partial and warp_sum.  h and scale are left for a backward.  cbow_rows_kernel and the certified accuracy pass's
+// fallback both call this, so a window's o is the same bits in both.
+template <int VEC>
+__device__ __forceinline__ float rows_logit(const int32_t *__restrict__ gene, const float4 *__restrict__ W4, int32_t b,
+                                            int32_t e, int lane, int32_t reduce_mean, const float4 (&who)[VEC],
+                                            float4 (&h)[VEC], float &scale) {
+    constexpr int D4 = 32 * VEC;
+    constexpr int UNR = 8 / VEC;                 // 8 float4 (128 B) in flight per lane
+#pragma unroll
+    for (int v = 0; v < VEC; ++v) h[v] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int32_t base = b; base < e; base += 32) {
+        const int cnt = min(32, e - base);
+        const int32_t g = (lane < cnt) ? __ldg(gene + base + lane) : 0;
+        for (int k = 0; k < cnt; k += UNR) {
+            float4 r[UNR][VEC];
+#pragma unroll
+            for (int u = 0; u < UNR; ++u) {
+                const int32_t gk = __shfl_sync(0xffffffffu, g, (k + u) & 31);
+                const float4 *row = W4 + (size_t)gk * D4 + lane;
+#pragma unroll
+                for (int v = 0; v < VEC; ++v)
+                    r[u][v] = (k + u < cnt) ? ldg4(row + v * 32) : make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+#pragma unroll
+            for (int u = 0; u < UNR; ++u)
+#pragma unroll
+                for (int v = 0; v < VEC; ++v) {
+                    h[v].x += r[u][v].x; h[v].y += r[u][v].y; h[v].z += r[u][v].z; h[v].w += r[u][v].w;
+                }
+        }
+    }
+    scale = (reduce_mean && e > b) ? 1.f / (float)(e - b) : 1.f;
+    float part = 0.f;
+#pragma unroll
+    for (int v = 0; v < VEC; ++v) {
+        if (reduce_mean) { h[v].x *= scale; h[v].y *= scale; h[v].z *= scale; h[v].w *= scale; }
+        part += h[v].x * who[v].x + h[v].y * who[v].y + h[v].z * who[v].z + h[v].w * who[v].w;
+    }
+    return warp_sum(part);
+}
+
+// rows_logit for any D (cbow_rows_generic_kernel): h [D] is the warp's shared-memory row, lane owns h[lane + 32k].
+__device__ __forceinline__ float rows_generic_logit(const int32_t *__restrict__ gene, const float *__restrict__ W_ih,
+                                                    const float *__restrict__ W_ho, int32_t b, int32_t e, int lane,
+                                                    int32_t D, int32_t reduce_mean, float *h, float &scale) {
+    for (int d = lane; d < D; d += 32) h[d] = 0.f;
+    for (int32_t j = b; j < e; ++j) {
+        const float *row = W_ih + (size_t)__ldg(gene + j) * D;
+        for (int d = lane; d < D; d += 32) h[d] += __ldg(row + d);
+    }
+    scale = (reduce_mean && e > b) ? 1.f / (float)(e - b) : 1.f;
+    float part = 0.f;
+    for (int d = lane; d < D; d += 32) {
+        if (reduce_mean) h[d] *= scale;
+        part += h[d] * __ldg(W_ho + d);
+    }
+    return warp_sum(part);
+}
+
 // grid of a one-warp-per-item kernel (window, gene): whole chip resident (SMs x occupancy), never more CTAs than
 // kCbowWarps items each
 int rows_grid(const void *kernel, size_t smem, int64_t n_items, int *grid_out);
+
+// r1_prepare_kernel (g2v_cbow_rank1.cu): s[g] = <W_ih[g,:], W_ho>; with_t: st[g] = {s[g], t[g]} (float2) with
+// t[g] = sum_d |W_ih[g,d] * W_ho[d]|, +inf for a row with an element of magnitude > 2^64 (DESIGN.md §4.16)
+int launch_r1_prepare(const float *W_ih, const float *W_ho, float *s, int32_t V, int32_t D, bool with_t,
+                      cudaStream_t stream);
 
 }  // namespace g2v

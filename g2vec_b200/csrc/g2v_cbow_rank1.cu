@@ -20,6 +20,9 @@
 namespace g2v {
 
 // ---- s = W_ih . W_ho ----------------------------------------------------------------------------
+// WITH_T (the certified accuracy pass of g2v_cbow.cu, DESIGN.md §4.16): also t[g] = sum_d |W_ih[g,d] * W_ho[d]|,
+// +inf when an element of the row has magnitude > 2^64, stored as the float2 {s[g], t[g]}.
+template <bool WITH_T>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 r1_prepare_kernel(const float *__restrict__ W_ih, const float *__restrict__ W_ho, float *__restrict__ s,
                   int32_t V, int32_t D, const int32_t *__restrict__ skip) {
@@ -30,19 +33,38 @@ r1_prepare_kernel(const float *__restrict__ W_ih, const float *__restrict__ W_ho
     const bool vec4 = (D & 3) == 0;
     for (int64_t g = warp; g < V; g += nwarps) {
         const float *row = W_ih + (size_t)g * D;
-        float part = 0.f;
+        float part = 0.f, tpart = 0.f;
+        bool big = false;
         if (vec4) {
             const float4 *r4 = reinterpret_cast<const float4 *>(row);
             const float4 *h4 = reinterpret_cast<const float4 *>(W_ho);
             for (int i = lane; i < (D >> 2); i += 32) {
                 const float4 a = __ldg(r4 + i), b = __ldg(h4 + i);
                 part += a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w;
+                if (WITH_T) {
+                    tpart += fabsf(__fmul_rn(a.x, b.x)) + fabsf(__fmul_rn(a.y, b.y)) + fabsf(__fmul_rn(a.z, b.z))
+                             + fabsf(__fmul_rn(a.w, b.w));
+                    big |= fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))) > 0x1p64f;
+                }
             }
         } else {
-            for (int d = lane; d < D; d += 32) part += __ldg(row + d) * __ldg(W_ho + d);
+            for (int d = lane; d < D; d += 32) {
+                const float a = __ldg(row + d), b = __ldg(W_ho + d);
+                part += a * b;
+                if (WITH_T) {
+                    tpart += fabsf(__fmul_rn(a, b));
+                    big |= fabsf(a) > 0x1p64f;
+                }
+            }
         }
         part = warp_sum(part);
-        if (lane == 0) s[g] = part;
+        if (WITH_T) {
+            tpart = warp_sum(tpart);
+            if (__any_sync(0xffffffffu, big)) tpart = __int_as_float(0x7f800000);
+            if (lane == 0) reinterpret_cast<float2 *>(s)[g] = make_float2(part, tpart);
+        } else if (lane == 0) {
+            s[g] = part;
+        }
     }
 }
 
@@ -250,15 +272,26 @@ r1_update_ho_kernel(float *__restrict__ W_ho, float *__restrict__ m, float *__re
 
 using namespace g2v;
 
-extern "C" int g2v_cbow_r1_prepare(const float *W_ih, const float *W_ho, float *s, int32_t V, int32_t D,
-                                   void *stream) {
-    G2V_REQUIRE(V > 0 && D > 0 && W_ih && W_ho && s, "g2v_cbow_r1_prepare: bad arguments");
+namespace g2v {
+int launch_r1_prepare(const float *W_ih, const float *W_ho, float *s, int32_t V, int32_t D, bool with_t,
+                      cudaStream_t stream) {
+    const void *kern = with_t ? (const void *)r1_prepare_kernel<true> : (const void *)r1_prepare_kernel<false>;
     int grid = 0, rc;
-    if ((rc = rows_grid((const void *)r1_prepare_kernel, 0, V, &grid))) return rc;
-    r1_prepare_kernel<<<grid, kCbowWarps * 32, 0, (cudaStream_t)stream>>>(W_ih, W_ho, s, V, D, loop_skip_flag());
+    if ((rc = rows_grid(kern, 0, V, &grid))) return rc;
+    if (with_t)
+        r1_prepare_kernel<true><<<grid, kCbowWarps * 32, 0, stream>>>(W_ih, W_ho, s, V, D, loop_skip_flag());
+    else
+        r1_prepare_kernel<false><<<grid, kCbowWarps * 32, 0, stream>>>(W_ih, W_ho, s, V, D, loop_skip_flag());
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;
+}
+}  // namespace g2v
+
+extern "C" int g2v_cbow_r1_prepare(const float *W_ih, const float *W_ho, float *s, int32_t V, int32_t D,
+                                   void *stream) {
+    G2V_REQUIRE(V > 0 && D > 0 && W_ih && W_ho && s, "g2v_cbow_r1_prepare: bad arguments");
+    return launch_r1_prepare(W_ih, W_ho, s, V, D, false, (cudaStream_t)stream);
 }
 
 extern "C" int g2v_cbow_r1_windows(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,

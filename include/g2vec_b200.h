@@ -232,6 +232,19 @@ int g2v_cbow_eval(const int32_t *rowptr, const int32_t *gene, const uint8_t *lab
                   const float *W_ho, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce,
                   void *stream);
 
+/* g2v_cbow_eval_certified: adds into *n_correct the same count as g2v_cbow_eval, for every input, mostly without
+ * gathering rows (DESIGN.md §4.16).  A first launch writes st [2*V floats, device scratch] = {s[g], t[g]} per gene,
+ * s = W_ih.W_ho and t[g] = sum_d |W_ih[g,d] W_ho[d]|; the second takes each window's prediction from the collapsed
+ * logit scale * sum_{g in n} s[g] where a float32 error bound shows it has the sign of g2v_cbow_eval's logit, and
+ * computes that logit by g2v_cbow_eval's own row gather for every other window (empty ones included).  Admits the D
+ * range of g2v_cbow_eval.  Test arguments: force_gather != 0 sends every window to the row gather; n_gathered
+ * (nullable) is added the number of windows that took it.  Both launches test the loop's `stopped` word; never
+ * synchronises. */
+int g2v_cbow_eval_certified(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                            const int32_t *win, int64_t win_begin, int64_t n_win, const float *W_ih,
+                            const float *W_ho, float *st, int64_t *n_correct, int64_t *n_gathered, int32_t V,
+                            int32_t D, int32_t reduce, int32_t force_gather, void *stream);
+
 /* ---------------------------------------------------------------------------------------
  * Device-side control of the training loop (SURVEY.md 8f-4; G2Vec.py:262-283), so that several iterations of
  * the reference's loop can be enqueued -- or replayed as ONE CUDA graph -- without a host decision in between.
