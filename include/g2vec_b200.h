@@ -214,7 +214,12 @@ int g2v_cbow_update(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m
  * NVLS multicast addresses of the same buffers, or both NULL (then peer loads/stores are used).  Rank r reduces the
  * slice r of every rank's gradient (multimem.ld_reduce or peer loads), zeroes it everywhere, applies TF1 Adam / SGD
  * to slice r of its m / v / parameters, and stores the new parameters into every rank's buffer.  The caller must
- * place a cross-GPU barrier before the call (all gradients complete) and after it (all parameters delivered). */
+ * place a cross-GPU barrier before the call (all gradients complete) and after it (all parameters delivered).
+ * Slice r is the float4 range [r*c, min(n/4, (r+1)*c)) with c = ceil((n/4) / world) -- empty for the ranks past
+ * n/4 -- and the scalar tail [4*floor(n/4), n) belongs to rank world-1.  m_flat / v_flat are n floats per rank, of
+ * which the call reads and writes only slice r: across steps each rank's m / v hold only its own slice, so `world`
+ * and the partition must stay the same for the whole run.  On the peer path rank r adds the gradients to 0 in the
+ * rank order r, r+1, ..., r-1 (mod world) on its float4 slice and 0, 1, ..., world-1 on the tail. */
 int g2v_cbow_update_nvl(float *const *g_ptrs_dev, float *const *w_ptrs_dev, float *g_multicast, float *w_multicast,
                         float *m_flat, float *v_flat, int64_t n, int32_t rank, int32_t world, int32_t optimizer,
                         float lr, float beta1, float beta2, float eps, int32_t t, const float *alpha_dev, void *stream);
