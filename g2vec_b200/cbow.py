@@ -143,6 +143,8 @@ class CbowModel:
         # Adam's beta1^t / beta2^t / alpha_t live on the device (TF1's beta*_power variables), advanced by
         # g2v_cbow_adam_tick: no launch of a step depends on a host-side value, so a step can be a CUDA graph
         self.hyper = torch.tensor([1.0, 1.0, 0.0, 0.0], dtype=torch.float32, device=dev)
+        # reduce-on-plateau state of g2v_cbow_lr_plateau (set_lr_plateau), else None: the rate is self.lr
+        self.plateau = self._plateau_init = None
         if algo == "rank1":
             self._launch("g2v_cbow_r1_prepare", self.W_ih.data_ptr(), self.W_ho.data_ptr(), self.s.data_ptr(), self.V,
                          self.D)
@@ -355,11 +357,38 @@ class CbowModel:
                      self.v_ih.data_ptr(), self.W_ho.data_ptr(), self.m_ho.data_ptr(), self.v_ho.data_ptr(),
                      self.g_ho.data_ptr(), self.V, self.D, self.lr, self.beta1, self.beta2, self.eps, self.t, adev)
 
+    def set_lr_plateau(self, patience, factor, min_lr, n_steps):
+        """Reduce-on-plateau learning rate (DESIGN.md §4.17): from now on the Adam step size is computed from the rate
+        in ``self.plateau`` (g2v_cbow_adam_tick_lr), which lr_decide() cuts by ``factor`` (not below ``min_lr``) after
+        ``patience`` steps in a row without a validation count above the best.  The rates of the first ``n_steps``
+        decided steps are recorded.  Adam optimizers only."""
+        if self.opt != _capi.OPT_ADAM_TF1:
+            raise ValueError("the reduce-on-plateau learning rate needs an Adam optimizer")
+        cap = max(int(n_steps), 1)
+        head = torch.tensor([int(patience), -1, 0, 0, 0, cap, 0, 0], dtype=torch.int64)
+        rates = torch.zeros(4 + cap + (cap & 1), dtype=torch.float32)
+        rates[:3] = torch.tensor([np.float32(self.lr), np.float32(factor), np.float32(min_lr)])
+        self._plateau_init = torch.cat([head, rates.view(torch.int64)])
+        self.plateau = self._plateau_init.to(self.device)
+
+    def lr_reset(self):
+        """Put the rate state back to its start: best -1, wait 0, no step decided, the initial rate."""
+        if self.plateau is not None:
+            self.plateau.copy_(self._plateau_init)
+
+    def lr_decide(self, counts_ptr, stride=0, n_decided_ptr=None):
+        """g2v_cbow_lr_plateau on the validation counts at ``counts_ptr`` (see include/g2vec_b200.h)."""
+        self._launch("g2v_cbow_lr_plateau", self.plateau.data_ptr(), counts_ptr, int(stride), n_decided_ptr)
+
     def update(self):
         self.t += 1
         adev = 0
         if self.opt == _capi.OPT_ADAM_TF1:
-            self._launch("g2v_cbow_adam_tick", self.hyper.data_ptr(), self.lr, self.beta1, self.beta2)
+            if self.plateau is not None:
+                self._launch("g2v_cbow_adam_tick_lr", self.hyper.data_ptr(), self.plateau.data_ptr() + 64, self.beta1,
+                             self.beta2)
+            else:
+                self._launch("g2v_cbow_adam_tick", self.hyper.data_ptr(), self.lr, self.beta1, self.beta2)
             adev = self.hyper.data_ptr()
         if self.lazy:
             self._lazy_update(adev)
@@ -410,11 +439,25 @@ class CbowModel:
         return float(acc_host[:1].view(torch.float64)[0])
 
 
-def check_config(algo, optimizer, deterministic, several_gpus=False, batch=0, reshuffle=False, patience=1):
+def check_config(algo, optimizer, deterministic, several_gpus=False, batch=0, reshuffle=False, patience=1,
+                 lr_patience=0, lr_factor=0.1, min_lr=0.0):
     """Refuse (ValueError) what train_cbow and CbowModel cannot run, before any device work.  ``several_gpus``: a
-    process group of more than one rank; ``batch``, ``reshuffle`` and ``patience`` as train_cbow takes them."""
+    process group of more than one rank; ``batch``, ``reshuffle``, ``patience``, ``lr_patience``, ``lr_factor`` and
+    ``min_lr`` as train_cbow takes them."""
     if isinstance(patience, bool) or not isinstance(patience, (int, np.integer)) or patience < 1:
         raise ValueError("patience must be an int >= 1 (the number of bad epochs in a row that stops the run)")
+    if isinstance(lr_patience, bool) or not isinstance(lr_patience, (int, np.integer)) or lr_patience < 0:
+        raise ValueError("lr_patience must be an int >= 0 (epochs without improvement before the learning rate is "
+                         "cut; 0 = never)")
+    if (isinstance(lr_factor, bool) or not isinstance(lr_factor, (int, float, np.integer, np.floating))
+            or not 0.0 < float(np.float32(lr_factor)) < 1.0):
+        raise ValueError("lr_factor must be a number in (0, 1) (what the learning rate is multiplied by at a plateau)")
+    if (isinstance(min_lr, bool) or not isinstance(min_lr, (int, float, np.integer, np.floating))
+            or not 0.0 <= float(min_lr) < math.inf):
+        raise ValueError("min_lr must be a finite number >= 0 (the learning rate is never cut below it)")
+    if lr_patience > 0 and optimizer == "sgd":
+        raise ValueError("lr_patience > 0 needs optimizer='adam' or 'lazy_adam': optimizer='sgd' takes its rate from "
+                         "the host")
     if algo not in ("rows", "rank1"):
         raise ValueError("algo must be 'rows' (gather/scatter of embedding rows) or 'rank1' (collapsed)")
     if reshuffle and batch <= 0:
@@ -622,9 +665,17 @@ def _dist():
 def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500, seed=0, optimizer="adam",
                reduce="sum", W_ih0=None, W_ho0=None, split=None, early_stop=True, log=print, return_info=False,
                eval_train="lazy", algo="rows", batch=0, use_graph=True, reshuffle=False, deterministic=False,
-               patience=1):
+               patience=1, lr_patience=0, lr_factor=0.1, min_lr=0.0):
     """Train the modified CBOW on CSR windows and return W_ih (np.float32 [n_genes, hidden]) exactly as
     ``compute_genetovec`` does: the weights after the last step whose validation accuracy did not drop.
+
+    ``lr_patience`` (int >= 0; 0, the default, = off): reduce the learning rate on a plateau, Keras
+    ReduceLROnPlateau(mode="max", min_delta=0, cooldown=0) on the correct validation count of each step (DESIGN.md
+    §4.17).  A count above the best so far is an improvement -- a tie is not, unlike the early-stop rule --; after
+    ``lr_patience`` steps in a row without one the rate becomes max(float32(lr * ``lr_factor``), ``min_lr``) if it is
+    above ``min_lr``, and the count starts again.  A step trains with the rate the decisions of the steps before it
+    left.  The rule runs on the device, independent of early stopping, which still decides the stop and the returned
+    weights.  Adam and lazy_adam only.
 
     ``patience`` (int >= 1, with ``early_stop``): the best validation count so far is tracked, a step whose count is
     >= the best becomes the best (ties: the later step), and the run stops at the ``patience``-th step in a row below
@@ -662,11 +713,13 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     algo="rank1" is already reproducible with a full batch and is accepted unchanged; with ``batch > 0`` it is an error.
 
     ``return_info=True`` also returns a dict: ``history`` [(step, ACC[val], ACC[tr])], ``stop_step`` (the step where
-    the run stopped early, else None), ``best_step`` (the step whose W_ih is returned; None if no step ran), and more.
+    the run stopped early, else None), ``best_step`` (the step whose W_ih is returned; None if no step ran), ``lr``
+    (the float32 learning rate each step trained with), ``lr_reductions`` (the steps whose decision cut the rate;
+    one on the last step has no effect), and more.
     """
     dist = _dist()
     check_config(algo, optimizer, deterministic, several_gpus=dist is not None, batch=batch, reshuffle=reshuffle,
-                 patience=patience)
+                 patience=patience, lr_patience=lr_patience, lr_factor=lr_factor, min_lr=min_lr)
     world, rank = (dist.get_world_size(), dist.get_rank()) if dist else (1, 0)
     rowptr_np = (win_rowptr.cpu().numpy() if isinstance(win_rowptr, torch.Tensor) else np.asarray(win_rowptr))
     N = rowptr_np.shape[0] - 1
@@ -678,6 +731,8 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     model = CbowModel(win_rowptr, win_gene, labels, n_genes, hidden, W_ih0, W_ho0, optimizer, reduce, lr, algo=algo,
                       nvl_group=dist.group.WORLD if (dist and algo == "rows") else None,
                       deterministic=deterministic and algo == "rows")
+    if lr_patience > 0:
+        model.set_lr_plateau(lr_patience, lr_factor, min_lr, max_epoch)
     lens = np.diff(rowptr_np).astype(np.int64)
     n_tr, n_va = len(tr), len(va)
     full_batch = batch <= 0 or batch >= n_tr
@@ -702,24 +757,45 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     if log:
         log("     Start training the modified CBOW with early stopping")
     if max_epoch <= 0:                           # no optimizer step at all: the initial vectors
-        out, hist, stop, best = model.W_ih, [], None, None
+        out, hist, stop, best, plateau = model.W_ih, [], None, None, None
     elif full_batch:
-        out, hist, stop, best = _device_loop(model, dist, tr_d, va_d, n_tr, n_va, len(tr_loc), len(va_loc), max_epoch,
-                                             early_stop, log, eval_train, use_graph, patience=patience)
+        out, hist, stop, best, plateau = _device_loop(model, dist, tr_d, va_d, n_tr, n_va, len(tr_loc), len(va_loc),
+                                                      max_epoch, early_stop, log, eval_train, use_graph,
+                                                      patience=patience)
     else:
-        out, hist, stop, best = _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, len(tr_loc), len(va_loc),
-                                                max_epoch, early_stop, log, batch,
-                                                reshuffle=(tr_all, seed, rank) if reshuffle else None,
-                                                patience=patience)
+        out, hist, stop, best, plateau = _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, len(tr_loc),
+                                                         len(va_loc), max_epoch, early_stop, log, batch,
+                                                         reshuffle=(tr_all, seed, rank) if reshuffle else None,
+                                                         patience=patience)
     if log:
         log("    Optimization Finish")
     out = out.cpu().numpy()
     if return_info:
+        rates, cuts = lr_rates(plateau) if plateau is not None else ([float(np.float32(lr))] * len(hist), [])
         return out, {"history": hist, "stop_step": stop, "best_step": best, "n_train": n_tr, "n_val": n_va,
-                     "model": model,
+                     "lr": rates, "lr_reductions": cuts, "model": model,
                      "windows": (tr_d, va_d),
                      "graph": bool(getattr(model, "loop_used_graph", False)), "exchange": model.exchange() if dist else None}
     return out
+
+
+def lr_rates(state):
+    """From a host copy (int64 tensor) of a g2v_cbow_lr_plateau state: the float32 rate each decided step trained
+    with, as floats, and the steps whose decision cut the rate."""
+    n = int(state[4])
+    f = state.numpy()[8:].view(np.float32)
+    rates = f[4:4 + n]
+    after = np.append(rates[1:], f[0])
+    return [float(r) for r in rates], [s for s in range(n) if after[s] < rates[s]]
+
+
+def lr_cut(state, step):
+    """The rate the decision of ``step`` (already decided in the host copy ``state``) left if it cut the rate, else
+    None."""
+    n = int(state[4])
+    f = state.numpy()[8:].view(np.float32)
+    after = f[4 + step + 1] if step + 1 < n else f[0]
+    return float(after) if after < f[4 + step] else None
 
 
 class _LoopLog:
@@ -735,6 +811,8 @@ class _LoopLog:
         self.hist, self.t0 = [], time.time()
         self.patience = patience
         self.best_val, self.best_step, self.bad = -1, None, 0
+        # reduce-on-plateau: a host copy of the rate state whose decisions step() reports (set by the loop), else None
+        self.plateau = None
 
     def stops(self, acc):
         """Whether a step with counters ``acc`` ends the run under the rule (host-driven loops decide with this)."""
@@ -757,6 +835,10 @@ class _LoopLog:
             t1 = time.time()
             log("    - Epoch: %03d\tACC[val]=%.4f\tACC[tr]=%.4f (%.3f sec)" % (step, acc_val, acc_tr, t1 - self.t0))
             self.t0 = time.time()
+        if self.plateau is not None and log:
+            cut = lr_cut(self.plateau, step)
+            if cut is not None:
+                log("    - Epoch: %03d\tlearning rate -> %g" % (step, cut))
         if stopped_here:
             # the best step's accuracies; its ACC[tr] is in the history by now (step-1's was filled in above)
             if log:
@@ -826,10 +908,14 @@ class DeviceLoop:
         # default path: W_ih before the step being decided (only an early stop ever returns it); keep-best path: W_ih
         # of the best step so far
         self.result = model.W_ih.clone() if (snapshot or self.best is not None) else None
+        # the model's reduce-on-plateau state, read back with the loop's status (model.set_lr_plateau, else None)
+        self.plateau_pin = torch.empty_like(model.plateau, device="cpu").pin_memory() if model.plateau is not None \
+            else None
         self.reset()
 
     def reset(self):
         self.m._launch("g2v_cbow_loop_init", self.ctl.data_ptr(), self.max_epoch, int(self.early_stop))
+        self.m.lr_reset()
         if self.best is not None:
             self.best.copy_(torch.tensor([self.patience, -1, 0, 0], dtype=torch.int64))
         if self.carried:                             # drop a pending carry: its g_ho partial would be added twice
@@ -887,12 +973,16 @@ class DeviceLoop:
                       self.hist_d.data_ptr())
             m._launch("g2v_cbow_loop_keep_best", self.best.data_ptr(), m.W_ih.data_ptr(), self.result.data_ptr(),
                       m.V * m.D)
+        if m.plateau is not None:                # the rate rule on the count the decision just recorded in hist
+            m.lr_decide(self.hist_d.data_ptr() + 16, 4, self.ctl.data_ptr() + 8)
 
     def fetch(self):
         self.ctl_pin.copy_(self.ctl, non_blocking=True)
         self.hist_pin.copy_(self.hist_d, non_blocking=True)
         if self.best is not None:
             self.best_pin.copy_(self.best, non_blocking=True)
+        if self.plateau_pin is not None:
+            self.plateau_pin.copy_(self.m.plateau, non_blocking=True)
 
     def capture(self, pattern):
         """The iterations of `pattern` (list of show flags) + the status read-back as one CUDA graph."""
@@ -914,12 +1004,13 @@ def _device_loop(model, dist, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_ep
     that all have it) -- and synchronises once per printed line instead of once per step.  Iterations enqueued after
     the stop are no-ops (every kernel tests ctl.stopped).  Multi-GPU: the all-reduces are part of the captured graph
     (NCCL is capturable); if capture is refused the same launches run eagerly.  Returns (W_ih to return, history,
-    stop step or None, best step)."""
+    stop step or None, best step, host copy of the model's reduce-on-plateau state or None)."""
     dev = model.device
     loop = DeviceLoop(model, dist, tr_d, va_d, n_tr, max_epoch, early_stop, snapshot=bool(early_stop),
                       patience=patience)
     shown = lambda s: loop.carried or s % 5 == 0 or eval_train == "always"
     info = _LoopLog(n_tr, n_va, log, patience if early_stop else None)
+    info.plateau = loop.plateau_pin
 
     def consume(lo, hi):
         """Host view of steps lo..hi-1 after a sync; True when the loop is over."""
@@ -975,9 +1066,9 @@ def _device_loop(model, dist, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_ep
         loop.detach()
     model.loop_used_graph = graph is not None
     if loop.best is not None:                    # keep-best path: result holds the best step's weights in every case
-        return loop.result, info.hist, stop, int(loop.best_pin[1])
+        return loop.result, info.hist, stop, int(loop.best_pin[1]), info.plateau
     # stopped early: the snapshot taken before the dropping step (G2Vec.py:283,286); else the final weights
-    return (loop.result if stop is not None else model.W_ih), info.hist, stop, info.best_step
+    return (loop.result if stop is not None else model.W_ih), info.hist, stop, info.best_step, info.plateau
 
 
 def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_epoch, early_stop, log, batch,
@@ -987,9 +1078,14 @@ def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_l
     ``reshuffle`` = (global training list on the device, seed, rank): every epoch e >= 1 trains on this rank's share of
     the epoch's order, written into one preallocated buffer (g2v_cbow_epoch_order); lazy_adam then rebuilds the
     buffer's batch plans (one more sync), as does the deterministic mode.  The early-stop rule with ``patience`` is
-    applied on the host after the epoch's sync; the result is copied on the epochs that improve on the best."""
+    applied on the host after the epoch's sync; the result is copied on the epochs that improve on the best.  The
+    reduce-on-plateau rule, if the model has it, is decided on the device after the counters' all-reduce and its state
+    read back with them.  Returns what _device_loop returns."""
     dev = model.device
     info = _LoopLog(n_tr, n_va, log, patience if early_stop else None)
+    if model.plateau is not None:                # read back with each epoch's counters, for the log and the result
+        model.lr_reset()
+        info.plateau = torch.empty_like(model.plateau, device="cpu").pin_memory()
     result = model.W_ih.clone()
     stop = None
     per = -(-batch // world)
@@ -1020,6 +1116,9 @@ def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_l
             model.evaluate(tr_d, 3)                              # acc[1] mixes weights across batches: always evaluate
         if dist:
             dist.all_reduce(model.acc[1:4])
+        if model.plateau is not None:                            # the rate rule on the epoch's (summed) count
+            model.lr_decide(model.acc.data_ptr() + 16)
+            info.plateau.copy_(model.plateau, non_blocking=True)
         acc = model.acc.cpu()                                    # the epoch's only host sync
         if info.step(step, acc, True, info.stops(acc)):
             stop = step
@@ -1028,7 +1127,7 @@ def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_l
             result.copy_(model.W_ih)
     if stop is None:
         info.end()
-    return result, info.hist, stop, info.best_step
+    return result, info.hist, stop, info.best_step, info.plateau
 
 
 def compute_genetovec(pathList, n_genes, hidden_size, learning_rate, max_epoch=500, seed=0, log=print):

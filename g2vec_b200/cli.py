@@ -13,6 +13,11 @@ accuracy is below the best so far, stops at the K-th, and writes the vectors of 
 the ``Epoch(stop)`` line then names the best epoch, and a run that reaches ``--epoch`` with a better earlier epoch
 prints an ``Epoch(best)`` line (DESIGN.md §4.15).
 
+``--lr-patience K`` (default 0: a fixed learning rate) multiplies the learning rate by ``--lr-factor`` (default 0.1), but
+not below ``--min-lr`` (default 0), after K epochs in a row whose validation accuracy is not above the best so far (a
+tie does not count as better), and prints a ``learning rate ->`` line among the epoch lines for every cut (Keras
+ReduceLROnPlateau; DESIGN.md §4.17).  It works with the Adam optimizers only, and is independent of ``--patience``.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle``, at every table size (DESIGN.md §4.13);
@@ -62,9 +67,24 @@ def parse_arguments(argv=None):
                    help="early stopping: stop after this many epochs in a row whose validation accuracy is below the "
                         "best so far, and write the vectors of the best epoch; 1 (default) = the reference's rule, "
                         "stop at the first drop")
+    p.add_argument('--lr-patience', type=int, default=0,
+                   help="reduce the learning rate on a plateau: after this many epochs in a row without a validation "
+                        "accuracy above the best so far, multiply it by --lr-factor; 0 (default) = a fixed rate")
+    p.add_argument('--lr-factor', type=float, default=0.1,
+                   help="with --lr-patience: the factor in (0, 1) the learning rate is multiplied by (default 0.1)")
+    p.add_argument('--min-lr', type=float, default=0.0,
+                   help="with --lr-patience: the learning rate is never cut below this (default 0)")
     args = p.parse_args(argv)
     if args.patience < 1:
         p.error("--patience must be an integer >= 1")
+    if args.lr_patience < 0:
+        p.error("--lr-patience must be an integer >= 0")
+    if not 0.0 < float(np.float32(args.lr_factor)) < 1.0:
+        p.error("--lr-factor must be in (0, 1)")
+    if not 0.0 <= args.min_lr < float("inf"):
+        p.error("--min-lr must be a finite number >= 0")
+    if args.lr_patience > 0 and args.optimizer == 'sgd':
+        p.error("--lr-patience needs --optimizer adam or lazy_adam")
     if args.reshuffle and args.batch <= 0:
         p.error("--reshuffle needs mini-batches (--batch B with B > 0)")
     if args.deterministic and args.algo == 'rank1' and args.batch > 0:
@@ -266,7 +286,8 @@ def main(argv=None):
     mat = cbow.train_cbow(w_rowptr, w_gene, w_label, n_genes, args.sizeHiddenlayer, args.learningRate,
                           max_epoch=args.epoch, seed=args.seed, log=print, algo=args.algo,   # print is silent off rank 0
                           batch=args.batch, optimizer=args.optimizer, reshuffle=args.reshuffle,
-                          deterministic=args.deterministic, patience=args.patience)
+                          deterministic=args.deterministic, patience=args.patience, lr_patience=args.lr_patience,
+                          lr_factor=args.lr_factor, min_lr=args.min_lr)
     genes = data['gene']
     if rank != 0:
         dist.barrier()

@@ -26,7 +26,9 @@
 //                                         c = its segmented dO sum, then TF1 Adam on the W/m/v row with g = c * W_ho;
 //                                         g_ih is never materialised (g2v_cbow_fwd_do + g2v_cbow_lazy_adam)
 //   adam_tick_kernel                      TF1's beta1_power / beta2_power / alpha_t kept on the device so
-//                                         that a whole step can be replayed as one CUDA graph
+//                                         that a whole step can be replayed as one CUDA graph; adam_tick_lr_kernel
+//                                         reads the learning rate from device memory as well
+//   lr_plateau_kernel                     the reduce-on-plateau rule on the step's validation count (one thread)
 //
 // No tensor cores: the 128..512-wide reduction is a memory-bound gather/scatter, not a dense
 // contraction.  Algorithmic bytes per window: l*(8D+4)+5 with the scatter, l*(4D+12)+9 with the CSC backward
@@ -982,6 +984,34 @@ loop_keep_best_kernel(const long long *__restrict__ best, const float4 *__restri
     for (int64_t i = (n4 << 2) + tid; i < n; i += nth) R[i] = W[i];
 }
 
+// ---- reduce-on-plateau learning rate (DESIGN.md §4.17) ---------------------------------------------------------
+// st (int64 x 8, then float32 x (4 + cap)): {K, best, wait, n_reductions, steps, cap, -, -}, then
+//   f = {lr, factor, min_lr, -, rate[0 .. cap-1]}.  Applies the rule to every step from st.steps up to (excluding)
+//   *n_decided -- or to exactly one step if n_decided is NULL -- reading step s's validation count at
+//   counts[s * stride].  rate[s] records the rate step s trained with (the one before its own decision).  It does not
+//   test the loop's `stopped` word: the step that stops the loop is decided like any other, and the no-op steps
+//   enqueued after it find st.steps == *n_decided.
+__global__ void lr_plateau_kernel(long long *__restrict__ st, const long long *__restrict__ counts, int64_t stride,
+                                  const long long *__restrict__ n_decided) {
+    float *f = reinterpret_cast<float *>(st + 8);
+    const long long end = n_decided ? *n_decided : st[4] + 1;
+    for (long long s = st[4]; s < end; ++s) {
+        const long long v = counts[s * stride];
+        const float lr = f[0];
+        if (s < st[5]) f[4 + s] = lr;
+        if (v > st[1]) {                             // strict: a tie is not an improvement
+            st[1] = v; st[2] = 0;
+        } else if (++st[2] >= st[0]) {
+            if (lr > f[2]) {
+                f[0] = fmaxf(__fmul_rn(lr, f[1]), f[2]);
+                st[3] += 1;
+            }
+            st[2] = 0;
+        }
+    }
+    if (end > st[4]) st[4] = end;
+}
+
 }  // namespace g2v
 
 using namespace g2v;
@@ -1059,6 +1089,17 @@ extern "C" int g2v_cbow_loop_keep_best(const int64_t *best, const float *W_ih, f
     loop_keep_best_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
         reinterpret_cast<const long long *>(best), reinterpret_cast<const float4 *>(W_ih),
         reinterpret_cast<float4 *>(result), n >> 2, W_ih, result, n);
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_lr_plateau(int64_t *state, const int64_t *counts, int64_t stride, const int64_t *n_decided,
+                                   void *stream) {
+    G2V_REQUIRE(state && counts && stride >= 0, "g2v_cbow_lr_plateau: bad arguments");
+    lr_plateau_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(
+        reinterpret_cast<long long *>(state), reinterpret_cast<const long long *>(counts), stride,
+        reinterpret_cast<const long long *>(n_decided));
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;
@@ -1265,6 +1306,23 @@ __global__ void adam_tick_kernel(float *state, float lr, float beta1, float beta
 extern "C" int g2v_cbow_adam_tick(float *state, float lr, float beta1, float beta2, void *stream) {
     G2V_REQUIRE(state != nullptr, "g2v_cbow_adam_tick: null pointer");
     adam_tick_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(state, lr, beta1, beta2, loop_skip_flag());
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+// adam_tick_kernel with the learning rate read from device memory (the rate g2v_cbow_lr_plateau keeps)
+__global__ void adam_tick_lr_kernel(float *state, const float *lr_dev, float beta1, float beta2, const int32_t *skip) {
+    G2V_SKIP_IF_STOPPED(skip);
+    const float lr = *lr_dev;
+    const float b1p = state[0] * beta1, b2p = state[1] * beta2;
+    state[0] = b1p; state[1] = b2p;
+    state[2] = lr * sqrtf(1.f - b2p) / (1.f - b1p);
+}
+
+extern "C" int g2v_cbow_adam_tick_lr(float *state, const float *lr_dev, float beta1, float beta2, void *stream) {
+    G2V_REQUIRE(state != nullptr && lr_dev != nullptr, "g2v_cbow_adam_tick_lr: null pointer");
+    adam_tick_lr_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(state, lr_dev, beta1, beta2, loop_skip_flag());
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;

@@ -231,6 +231,10 @@ int g2v_cbow_update_nvl(float *const *g_ptrs_dev, float *const *w_ptrs_dev, floa
  * makes every launch of a training step independent of host-side values, so the whole step can be captured
  * once in a CUDA graph and replayed (g2vec_b200/cbow.py). */
 int g2v_cbow_adam_tick(float *state, float lr, float beta1, float beta2, void *stream);
+/* g2v_cbow_adam_tick with the learning rate read from *lr_dev on the device (the rate of g2v_cbow_lr_plateau's state):
+ * the same arithmetic, so an unchanged rate gives g2v_cbow_adam_tick's bits.  Tests the loop's `stopped` word as
+ * g2v_cbow_adam_tick does. */
+int g2v_cbow_adam_tick_lr(float *state, const float *lr_dev, float beta1, float beta2, void *stream);
 
 int g2v_cbow_eval(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
                   const int32_t *win, int64_t win_begin, int64_t n_win, const float *W_ih,
@@ -294,6 +298,23 @@ int g2v_cbow_loop_decide(int64_t *ctl, const int64_t *acc, int64_t *hist, void *
  * steps or synchronises, so both are captured in the loop's CUDA graphs. */
 int g2v_cbow_loop_decide_best(int64_t *ctl, int64_t *best, const int64_t *acc, int64_t *hist, void *stream);
 int g2v_cbow_loop_keep_best(const int64_t *best, const float *W_ih, float *result, int64_t n, void *stream);
+/* Reduce-on-plateau learning rate (DESIGN.md §4.17): Keras ReduceLROnPlateau(mode="max", min_delta=0, cooldown=0) on
+ * the integer validation count of each step, decided on the device.
+ *   state in device memory, int64 x 8 then float32 x (4 + cap):
+ *        {K, best, wait, n_reductions, steps, cap, -, -}, then {lr, factor, min_lr, -, rate[0 .. cap-1]}.
+ *        The caller sets {K, -1, 0, 0, 0, cap, 0, 0} and {lr, factor, min_lr, 0} (K >= 1, 0 < factor < 1,
+ *        min_lr >= 0); the rate lives at byte offset 64 and is what g2v_cbow_adam_tick_lr reads.
+ *   g2v_cbow_lr_plateau: for every step s not yet decided, v = counts[s * stride]; rate[s] = lr (if s < cap: the rate
+ *        step s trained with); then if v > best: best = v, wait = 0 (a tie is no improvement), else wait += 1 and when
+ *        wait >= K: if lr > min_lr, lr = max(float32(lr * factor), min_lr) and n_reductions += 1; wait = 0.
+ *        The steps it decides are steps .. *n_decided - 1, and exactly one step if n_decided is NULL; steps is then
+ *        advanced past them.  One kernel for both loops:
+ *        - device loop: after g2v_cbow_loop_decide[_best], counts = hist + 2, stride = 4, n_decided = &ctl.step.  The
+ *          decision reads the count that the loop's decision just recorded (summed over the ranks on every exchange),
+ *          and the no-op steps after a stop decide nothing, so it is captured in the loop's CUDA graphs;
+ *        - host-driven loop: after the all-reduce of acc[1..3], counts = acc + 2, stride = 0, n_decided = NULL.
+ *        It does not test the loop's `stopped` word.  One launch of one thread, never synchronises. */
+int g2v_cbow_lr_plateau(int64_t *state, const int64_t *counts, int64_t stride, const int64_t *n_decided, void *stream);
 /* Multi-GPU, hist in symmetric memory (zero-initialised, same size on every rank): add this rank's acc[1..3] into
  * hist[step][1..3] of every rank (multimem.red through hist_multicast, or system-scope atomics on hist_ptrs_dev);
  * after a cross-GPU barrier call g2v_cbow_loop_decide with acc == NULL, which then decides on the summed counters
