@@ -50,6 +50,14 @@ SIGNATURES = {
                                        _f32, _f32, _i32, _vp, _vp]),
     "g2v_cbow_update_nvl": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f32, _f32, _f32,
                                            _f32, _i32, _vp, _vp]),
+    "g2v_cbow_update_wd": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _f32,
+                                          _f32, _f32, _f32, _i32, _vp, _vp]),
+    "g2v_cbow_lazy_adam_wd": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
+                                             _f32, _f32, _f32, _f32, _f32, _i32, _vp, _vp]),
+    "g2v_cbow_update_nvl_wd": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f32, _f32, _f32,
+                                              _f32, _f32, _i32, _vp, _vp]),
+    "g2v_cbow_r1_update_wd": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _f32,
+                                             _f32, _f32, _f32, _i32, _vp, _vp]),
     "g2v_cbow_adam_tick": (ctypes.c_int, [_vp, _f32, _f32, _f32, _vp]),
     "g2v_cbow_adam_tick_lr": (ctypes.c_int, [_vp, _vp, _f32, _f32, _vp]),
     "g2v_cbow_lr_plateau": (ctypes.c_int, [_vp, _vp, _i64, _vp, _vp]),

@@ -63,8 +63,8 @@ class CbowModel:
 
     def __init__(self, rowptr, gene, label, n_genes, hidden, W_ih0, W_ho0, optimizer="adam", reduce="sum",
                  lr=0.005, beta1=0.9, beta2=0.999, eps=1e-8, device=None, algo="rows", nvl_group=None,
-                 deterministic=False):
-        check_config(algo, optimizer, deterministic, several_gpus=nvl_group is not None)
+                 deterministic=False, weight_decay=0.0):
+        check_config(algo, optimizer, deterministic, several_gpus=nvl_group is not None, weight_decay=weight_decay)
         if not torch.cuda.is_available():
             raise RuntimeError("g2vec_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.lib = _capi.load()
@@ -108,6 +108,8 @@ class CbowModel:
         self.opt = {"adam": _capi.OPT_ADAM_TF1, "sgd": _capi.OPT_SGD, "lazy_adam": _capi.OPT_ADAM_TF1}[optimizer]
         self.reduce = {"sum": _capi.REDUCE_SUM, "mean": _capi.REDUCE_MEAN}[reduce]
         self.lr, self.beta1, self.beta2, self.eps = float(lr), float(beta1), float(beta2), float(eps)
+        # decoupled weight decay (DESIGN.md §4.18), fused into every optimizer launch of update(); 0 = off
+        self.wd = float(np.float32(weight_decay))
         z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
         self.algo = algo
         # rows: scratch of the certified accuracy pass, {s[g], t[g]} per gene (g2v_cbow_eval_certified)
@@ -351,11 +353,12 @@ class CbowModel:
     def _lazy_update(self, adev):
         plan, r0, n_rows = self._pending or (None, 0, 0)
         self._pending = None
-        self._launch("g2v_cbow_lazy_adam", plan.rows.data_ptr() + 4 * r0 if n_rows else None,
+        name, wd = self._opt("g2v_cbow_lazy_adam")
+        self._launch(name, plan.rows.data_ptr() + 4 * r0 if n_rows else None,
                      plan.segptr.data_ptr() + 4 * r0 if n_rows else None, plan.pos.data_ptr() if n_rows else None,
                      self._dO.data_ptr() if n_rows else None, n_rows, self.W_ih.data_ptr(), self.m_ih.data_ptr(),
                      self.v_ih.data_ptr(), self.W_ho.data_ptr(), self.m_ho.data_ptr(), self.v_ho.data_ptr(),
-                     self.g_ho.data_ptr(), self.V, self.D, self.lr, self.beta1, self.beta2, self.eps, self.t, adev)
+                     self.g_ho.data_ptr(), self.V, self.D, self.lr, self.beta1, self.beta2, self.eps, *wd, self.t, adev)
 
     def set_lr_plateau(self, patience, factor, min_lr, n_steps):
         """Reduce-on-plateau learning rate (DESIGN.md §4.17): from now on the Adam step size is computed from the rate
@@ -380,7 +383,15 @@ class CbowModel:
         """g2v_cbow_lr_plateau on the validation counts at ``counts_ptr`` (see include/g2vec_b200.h)."""
         self._launch("g2v_cbow_lr_plateau", self.plateau.data_ptr(), counts_ptr, int(stride), n_decided_ptr)
 
+    def _opt(self, name):
+        """The optimizer entry point ``name`` and the arguments it takes between eps and t: its _wd form with the
+        model's weight decay, or with weight decay off the plain entry point (the same launches), so that a run
+        without decay calls exactly what it called before the option existed."""
+        return (name + "_wd", (self.wd,)) if self.wd else (name, ())
+
     def update(self):
+        """One optimizer step; every branch decays the elements it updates by the model's weight decay (self.wd, a
+        launch constant, DESIGN.md §4.18)."""
         self.t += 1
         adev = 0
         if self.opt == _capi.OPT_ADAM_TF1:
@@ -394,25 +405,28 @@ class CbowModel:
             self._lazy_update(adev)
             return
         if self.algo == "rank1":
-            self._launch("g2v_cbow_r1_update", self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._ptr(self.m_ih),
+            name, wd = self._opt("g2v_cbow_r1_update")
+            self._launch(name, self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._ptr(self.m_ih),
                          self._ptr(self.v_ih), self._ptr(self.m_ho), self._ptr(self.v_ho), self.c.data_ptr(),
                          self.g_ho.data_ptr(), self.s.data_ptr(), self.V, self.D, self.opt, self.lr, self.beta1,
-                         self.beta2, self.eps, self.t, adev)
+                         self.beta2, self.eps, *wd, self.t, adev)
             return
         if self.nvl:
             # gradient exchange fused with the optimizer: barrier (every rank's gradient complete) -> reduce-scatter +
             # Adam on the owned slice + all-gather of the new weights in ONE kernel -> barrier (weights delivered)
             nv = self.nvl
             nv["hg"].barrier(channel=0)
-            self._launch("g2v_cbow_update_nvl", nv["hg"].buffer_ptrs_dev, nv["hw"].buffer_ptrs_dev, nv["g_mc"],
+            name, wd = self._opt("g2v_cbow_update_nvl")
+            self._launch(name, nv["hg"].buffer_ptrs_dev, nv["hw"].buffer_ptrs_dev, nv["g_mc"],
                          nv["w_mc"], self._ptr(self.m_flat), self._ptr(self.v_flat), self.V * self.D + self.D,
-                         nv["rank"], nv["world"], self.opt, self.lr, self.beta1, self.beta2, self.eps, self.t, adev)
+                         nv["rank"], nv["world"], self.opt, self.lr, self.beta1, self.beta2, self.eps, *wd, self.t, adev)
             nv["hg"].barrier(channel=1)
             return
-        self._launch("g2v_cbow_update", self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._ptr(self.m_ih),
+        name, wd = self._opt("g2v_cbow_update")
+        self._launch(name, self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._ptr(self.m_ih),
                      self._ptr(self.v_ih), self._ptr(self.m_ho), self._ptr(self.v_ho), self.g_ih.data_ptr(),
-                     self.g_ho.data_ptr(), self.V, self.D, self.opt, self.lr, self.beta1, self.beta2, self.eps, self.t,
-                     adev)
+                     self.g_ho.data_ptr(), self.V, self.D, self.opt, self.lr, self.beta1, self.beta2, self.eps, *wd,
+                     self.t, adev)
 
     def evaluate(self, win, slot, win_begin=0, n_win=None):
         """Add the number of correctly classified listed windows into acc[slot]."""
@@ -440,10 +454,14 @@ class CbowModel:
 
 
 def check_config(algo, optimizer, deterministic, several_gpus=False, batch=0, reshuffle=False, patience=1,
-                 lr_patience=0, lr_factor=0.1, min_lr=0.0):
+                 lr_patience=0, lr_factor=0.1, min_lr=0.0, weight_decay=0.0):
     """Refuse (ValueError) what train_cbow and CbowModel cannot run, before any device work.  ``several_gpus``: a
-    process group of more than one rank; ``batch``, ``reshuffle``, ``patience``, ``lr_patience``, ``lr_factor`` and
-    ``min_lr`` as train_cbow takes them."""
+    process group of more than one rank; ``batch``, ``reshuffle``, ``patience``, ``lr_patience``, ``lr_factor``,
+    ``min_lr`` and ``weight_decay`` as train_cbow takes them."""
+    if (isinstance(weight_decay, bool) or not isinstance(weight_decay, (int, float, np.integer, np.floating))
+            or not 0.0 <= float(np.float32(weight_decay)) < 1.0):
+        raise ValueError("weight_decay must be a finite number with 0 <= weight_decay < 1 in float32 (the fraction of "
+                         "every weight removed per optimizer step; 0 = off)")
     if isinstance(patience, bool) or not isinstance(patience, (int, np.integer)) or patience < 1:
         raise ValueError("patience must be an int >= 1 (the number of bad epochs in a row that stops the run)")
     if isinstance(lr_patience, bool) or not isinstance(lr_patience, (int, np.integer)) or lr_patience < 0:
@@ -665,9 +683,16 @@ def _dist():
 def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500, seed=0, optimizer="adam",
                reduce="sum", W_ih0=None, W_ho0=None, split=None, early_stop=True, log=print, return_info=False,
                eval_train="lazy", algo="rows", batch=0, use_graph=True, reshuffle=False, deterministic=False,
-               patience=1, lr_patience=0, lr_factor=0.1, min_lr=0.0):
+               patience=1, lr_patience=0, lr_factor=0.1, min_lr=0.0, weight_decay=0.0):
     """Train the modified CBOW on CSR windows and return W_ih (np.float32 [n_genes, hidden]) exactly as
     ``compute_genetovec`` does: the weights after the last step whose validation accuracy did not drop.
+
+    ``weight_decay`` (λ, finite, 0 <= λ < 1 in float32; 0, the default, = off): decoupled weight decay, AdamW / SGDW
+    as TF1's DecoupledWeightDecayExtension applies it (DESIGN.md §4.18).  Every optimizer step first sets each element
+    it updates to fl(w - fl(λ w)), then takes the unchanged Adam / SGD step on that value with the gradient of the
+    weights before the step.  adam, sgd and rank1 decay all of W_ih and W_ho every step; lazy_adam decays the rows its
+    batch gathered, once each, and all of W_ho.  λ is a constant: the learning-rate schedule does not scale it, and
+    the logged loss has no penalty term.
 
     ``lr_patience`` (int >= 0; 0, the default, = off): reduce the learning rate on a plateau, Keras
     ReduceLROnPlateau(mode="max", min_delta=0, cooldown=0) on the correct validation count of each step (DESIGN.md
@@ -696,8 +721,9 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
 
     ``optimizer``: "adam" (TF1 AdamOptimizer, the reference's), "sgd", or "lazy_adam": TF1 LazyAdam on the
     embedding-lookup form of the model -- a step updates W_ih / m / v only on the rows of the genes its batch
-    gathered (dense Adam on W_ho).  Full batch it computes what "adam" computes (rows outside the training list
-    keep zero gradient and zero moments); with ``batch`` it is the usual sparse mini-batch embedding update.
+    gathered (dense Adam on W_ho).  Full batch and without ``weight_decay`` it computes what "adam" computes (rows
+    outside the training list keep zero gradient and zero moments; with decay "adam" shrinks them and lazy_adam does
+    not); with ``batch`` it is the usual sparse mini-batch embedding update.
     Only with algo="rows", on one GPU.
 
     ``reshuffle`` (with 0 < ``batch`` < n_train): epoch 0 trains on the split's order, epoch e >= 1 on tr[P(seed, e)],
@@ -719,8 +745,9 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     """
     dist = _dist()
     check_config(algo, optimizer, deterministic, several_gpus=dist is not None, batch=batch, reshuffle=reshuffle,
-                 patience=patience, lr_patience=lr_patience, lr_factor=lr_factor, min_lr=min_lr)
-    world, rank = (dist.get_world_size(), dist.get_rank()) if dist else (1, 0)
+                 patience=patience, lr_patience=lr_patience, lr_factor=lr_factor, min_lr=min_lr,
+                 weight_decay=weight_decay)
+    world, rank =(dist.get_world_size(), dist.get_rank()) if dist else (1, 0)
     rowptr_np = (win_rowptr.cpu().numpy() if isinstance(win_rowptr, torch.Tensor) else np.asarray(win_rowptr))
     N = rowptr_np.shape[0] - 1
     if N < 2:
@@ -730,7 +757,7 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
         W_ih0, W_ho0 = init_weights(n_genes, hidden, seed)
     model = CbowModel(win_rowptr, win_gene, labels, n_genes, hidden, W_ih0, W_ho0, optimizer, reduce, lr, algo=algo,
                       nvl_group=dist.group.WORLD if (dist and algo == "rows") else None,
-                      deterministic=deterministic and algo == "rows")
+                      deterministic=deterministic and algo == "rows", weight_decay=weight_decay)
     if lr_patience > 0:
         model.set_lr_plateau(lr_patience, lr_factor, min_lr, max_epoch)
     lens = np.diff(rowptr_np).astype(np.int64)

@@ -18,6 +18,12 @@ not below ``--min-lr`` (default 0), after K epochs in a row whose validation acc
 tie does not count as better), and prints a ``learning rate ->`` line among the epoch lines for every cut (Keras
 ReduceLROnPlateau; DESIGN.md §4.17).  It works with the Adam optimizers only, and is independent of ``--patience``.
 
+``--weight-decay λ`` (default 0: off; finite, 0 <= λ < 1) is decoupled weight decay, AdamW / SGDW: every optimizer
+step first shrinks each weight it updates to w - λ·w, then takes the usual step (DESIGN.md §4.18).  It acts per
+optimizer step (once per batch with ``--batch``), is not scaled by the learning rate or ``--lr-patience``, and adds
+nothing to the logged loss.  ``adam``, ``sgd`` and ``--algo rank1`` decay every gene vector every step; ``lazy_adam``
+decays only the vectors of the genes a batch gathered.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle``, at every table size (DESIGN.md §4.13);
@@ -74,7 +80,12 @@ def parse_arguments(argv=None):
                    help="with --lr-patience: the factor in (0, 1) the learning rate is multiplied by (default 0.1)")
     p.add_argument('--min-lr', type=float, default=0.0,
                    help="with --lr-patience: the learning rate is never cut below this (default 0)")
+    p.add_argument('--weight-decay', type=float, default=0.0,
+                   help="decoupled weight decay (AdamW / SGDW): every optimizer step first shrinks each weight it "
+                        "updates by this fraction, in [0, 1); 0 (default) = off")
     args = p.parse_args(argv)
+    if not 0.0 <= float(np.float32(args.weight_decay)) < 1.0:
+        p.error("--weight-decay must be a finite number with 0 <= weight-decay < 1")
     if args.patience < 1:
         p.error("--patience must be an integer >= 1")
     if args.lr_patience < 0:
@@ -287,7 +298,7 @@ def main(argv=None):
                           max_epoch=args.epoch, seed=args.seed, log=print, algo=args.algo,   # print is silent off rank 0
                           batch=args.batch, optimizer=args.optimizer, reshuffle=args.reshuffle,
                           deterministic=args.deterministic, patience=args.patience, lr_patience=args.lr_patience,
-                          lr_factor=args.lr_factor, min_lr=args.min_lr)
+                          lr_factor=args.lr_factor, min_lr=args.min_lr, weight_decay=args.weight_decay)
     genes = data['gene']
     if rank != 0:
         dist.barrier()

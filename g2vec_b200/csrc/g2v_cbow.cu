@@ -25,6 +25,8 @@
 //   cbow_lazy_adam_rows_kernel            lazy (touched-row) Adam of a batch: one warp per gene the batch gathered,
 //                                         c = its segmented dO sum, then TF1 Adam on the W/m/v row with g = c * W_ho;
 //                                         g_ih is never materialised (g2v_cbow_fwd_do + g2v_cbow_lazy_adam)
+//                                         The optimizer kernels take a bool WD: decoupled weight decay of every
+//                                         element they update, fused before the step (the *_wd entry points)
 //   adam_tick_kernel                      TF1's beta1_power / beta2_power / alpha_t kept on the device so
 //                                         that a whole step can be replayed as one CUDA graph; adam_tick_lr_kernel
 //                                         reads the learning rate from device memory as well
@@ -582,12 +584,14 @@ cbow_batch_expand_kernel(const int32_t *__restrict__ rows, const int32_t *__rest
 }
 
 // ---- optimizer epilogue --------------------------------------------------------------------
-template <int OPT>
+// WD: decoupled weight decay wd on every element before the step (decay1); WD = false is the plain update.
+template <int OPT, bool WD>
 __global__ void __launch_bounds__(256)
 cbow_update_kernel(float *__restrict__ W, float *__restrict__ M, float *__restrict__ Vv,
                    float *__restrict__ G, int64_t n, float *__restrict__ W2, float *__restrict__ M2,
                    float *__restrict__ V2, float *__restrict__ G2, int64_t n2, float alpha_host, float omb1,
-                   float omb2, float eps, const float *__restrict__ alpha_dev, const int32_t *__restrict__ skip) {
+                   float omb2, float eps, const float *__restrict__ alpha_dev, const int32_t *__restrict__ skip,
+                   float wd) {
     G2V_SKIP_IF_STOPPED(skip);
     // alpha_dev != NULL: the step size lives on the device (g2v_cbow_adam_tick), so the launch can be replayed
     const float alpha = alpha_dev ? __ldg(alpha_dev + 2) : alpha_host;
@@ -599,6 +603,7 @@ cbow_update_kernel(float *__restrict__ W, float *__restrict__ M, float *__restri
     for (int64_t i = tid; i < n4; i += nthreads) {
         float4 w = W4[i];
         const float4 g = G4[i];
+        decay4<WD>(w, wd);
         if (OPT == G2V_OPT_ADAM_TF1) {
             float4 m = M4[i], v = V4[i];
             adam1(w.x, m.x, v.x, g.x, alpha, omb1, omb2, eps);
@@ -617,6 +622,7 @@ cbow_update_kernel(float *__restrict__ W, float *__restrict__ M, float *__restri
         float *w, *m, *v, *g;
         if (i < n) { w = W + i; m = M + i; v = Vv + i; g = G + i; }
         else { const int64_t j = i - n; w = W2 + j; m = M2 + j; v = V2 + j; g = G2 + j; }
+        decay1<WD>(*w, wd);
         if (OPT == G2V_OPT_ADAM_TF1) adam1(*w, *m, *v, *g, alpha, omb1, omb2, eps);
         else *w -= alpha * *g;
         *g = 0.f;
@@ -631,12 +637,15 @@ cbow_update_kernel(float *__restrict__ W, float *__restrict__ M, float *__restri
 // Rows outside the list keep W, m and v bit for bit.  W_ho must be the value before this step: its own update is a
 // second launch (cbow_update_kernel with n = 0).  The gradient is rounded on its own (__fmul_rn, never contracted
 // into Adam's first subtraction), as the stored g_ih of the CSC backward is, so the step is the dense one bit for bit.
+// WD: each listed row is decayed once (rows are distinct) before its step, as TF1 decays the deduplicated indices.
+template <bool WD>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 cbow_lazy_adam_rows_kernel(const int32_t *__restrict__ rows, const int32_t *__restrict__ segptr,
                            const int32_t *__restrict__ pos, const float *__restrict__ dO, int64_t n_rows,
                            float *__restrict__ W, float *__restrict__ M, float *__restrict__ Vv,
                            const float *__restrict__ W_ho, int32_t D, float alpha_host, float omb1, float omb2,
-                           float eps, const float *__restrict__ alpha_dev, const int32_t *__restrict__ skip) {
+                           float eps, const float *__restrict__ alpha_dev, const int32_t *__restrict__ skip,
+                           float wd) {
     G2V_SKIP_IF_STOPPED(skip);
     const float alpha = alpha_dev ? __ldg(alpha_dev + 2) : alpha_host;
     const int lane = threadIdx.x & 31;
@@ -651,6 +660,7 @@ cbow_lazy_adam_rows_kernel(const int32_t *__restrict__ rows, const int32_t *__re
             for (int k = lane; k < (D >> 2); k += 32) {
                 const float4 h = ldg4(reinterpret_cast<const float4 *>(W_ho) + k);
                 float4 w = w4[k], m = m4[k], v = v4[k];
+                decay4<WD>(w, wd);
                 adam1(w.x, m.x, v.x, __fmul_rn(c, h.x), alpha, omb1, omb2, eps);
                 adam1(w.y, m.y, v.y, __fmul_rn(c, h.y), alpha, omb1, omb2, eps);
                 adam1(w.z, m.z, v.z, __fmul_rn(c, h.z), alpha, omb1, omb2, eps);
@@ -658,8 +668,10 @@ cbow_lazy_adam_rows_kernel(const int32_t *__restrict__ rows, const int32_t *__re
                 w4[k] = w; m4[k] = m; v4[k] = v;
             }
         } else {
-            for (int d = lane; d < D; d += 32)
+            for (int d = lane; d < D; d += 32) {
+                decay1<WD>(W[off + d], wd);
                 adam1(W[off + d], M[off + d], Vv[off + d], __fmul_rn(c, __ldg(W_ho + d)), alpha, omb1, omb2, eps);
+            }
         }
     }
 }
@@ -696,12 +708,13 @@ __device__ __forceinline__ void st_peer4(float *p, float4 v) {
                  : "memory");
 }
 
-template <int OPT, bool MC>
+// WD: the owned slice is decayed (decay1) after the reduce and before Adam / SGD, then all-gathered as before.
+template <int OPT, bool MC, bool WD>
 __global__ void __launch_bounds__(256)
 cbow_update_nvl_kernel(float *const *__restrict__ g_ptrs, float *const *__restrict__ w_ptrs, float *__restrict__ g_mc,
                        float *__restrict__ w_mc, float *__restrict__ M, float *__restrict__ Vv, int64_t n, int32_t rank,
                        int32_t world, float alpha_host, float omb1, float omb2, float eps,
-                       const float *__restrict__ alpha_dev, const int32_t *__restrict__ skip) {
+                       const float *__restrict__ alpha_dev, const int32_t *__restrict__ skip, float wd) {
     G2V_SKIP_IF_STOPPED(skip);
     const float alpha = alpha_dev ? __ldg(alpha_dev + 2) : alpha_host;
     const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, nth = (int64_t)gridDim.x * blockDim.x;
@@ -724,6 +737,7 @@ cbow_update_nvl_kernel(float *const *__restrict__ g_ptrs, float *const *__restri
             }
         }
         float4 w = reinterpret_cast<const float4 *>(Wl)[i];
+        decay4<WD>(w, wd);
         if (OPT == G2V_OPT_ADAM_TF1) {
             float4 m = reinterpret_cast<float4 *>(M)[i], v = reinterpret_cast<float4 *>(Vv)[i];
             adam1(w.x, m.x, v.x, g.x, alpha, omb1, omb2, eps);
@@ -749,6 +763,7 @@ cbow_update_nvl_kernel(float *const *__restrict__ g_ptrs, float *const *__restri
                 g += *gp; *gp = 0.f;
             }
             float w = Wl[i];
+            decay1<WD>(w, wd);
             if (OPT == G2V_OPT_ADAM_TF1) adam1(w, M[i], Vv[i], g, alpha, omb1, omb2, eps);
             else w -= alpha * g;
             for (int p = 0; p < world; ++p) { volatile float *wp = w_ptrs[p] + i; *wp = w; }
@@ -1328,14 +1343,25 @@ extern "C" int g2v_cbow_adam_tick_lr(float *state, const float *lr_dev, float be
     return 0;
 }
 
-extern "C" int g2v_cbow_update(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m_ho, float *v_ho,
-                               float *g_ih, float *g_ho, int32_t V, int32_t D, int32_t optimizer, float lr,
-                               float beta1, float beta2, float eps, int32_t t, const float *alpha_dev,
-                               void *stream) {
+// The template arguments <OPT, WD> of an optimizer kernel as runtime values: WD = weight_decay > 0, so that 0 launches
+// the plain instantiation.
+#define G2V_OPT_WD_DISPATCH(optimizer, weight_decay, MACRO)                                                            \
+    do {                                                                                                               \
+        if ((optimizer) == G2V_OPT_ADAM_TF1) { if ((weight_decay) > 0.f) MACRO(G2V_OPT_ADAM_TF1, true);              \
+                                               else MACRO(G2V_OPT_ADAM_TF1, false); }                                 \
+        else { if ((weight_decay) > 0.f) MACRO(G2V_OPT_SGD, true); else MACRO(G2V_OPT_SGD, false); }                  \
+    } while (0)
+
+extern "C" int g2v_cbow_update_wd(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m_ho, float *v_ho,
+                                  float *g_ih, float *g_ho, int32_t V, int32_t D, int32_t optimizer, float lr,
+                                  float beta1, float beta2, float eps, float weight_decay, int32_t t,
+                                  const float *alpha_dev, void *stream) {
     G2V_REQUIRE(V > 0 && D > 0 && (t >= 1 || alpha_dev), "g2v_cbow_update: bad sizes (V=%d D=%d t=%d)", V, D, t);
     G2V_REQUIRE(W_ih && W_ho && g_ih && g_ho, "g2v_cbow_update: null pointer");
     G2V_REQUIRE(optimizer == G2V_OPT_ADAM_TF1 || optimizer == G2V_OPT_SGD, "g2v_cbow_update: unknown optimizer %d", optimizer);
     G2V_REQUIRE(optimizer == G2V_OPT_SGD || (m_ih && v_ih && m_ho && v_ho), "g2v_cbow_update: Adam needs m/v buffers");
+    G2V_REQUIRE(weight_decay_ok(weight_decay), "g2v_cbow_update_wd: weight_decay must be finite with 0 <= wd < 1 (got %g)",
+                (double)weight_decay);
     DeviceProps dp;
     if (device_props(&dp)) return 1;
     const int64_t n = (int64_t)V * D;
@@ -1344,17 +1370,59 @@ extern "C" int g2v_cbow_update(float *W_ih, float *W_ho, float *m_ih, float *v_i
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
     cudaStream_t st = (cudaStream_t)stream;
-    if (optimizer == G2V_OPT_ADAM_TF1) {
-        const float alpha = alpha_dev ? 0.f : adam_tf1_alpha(lr, beta1, beta2, t);
-        cbow_update_kernel<G2V_OPT_ADAM_TF1><<<(unsigned)blocks, 256, 0, st>>>(
-            W_ih, m_ih, v_ih, g_ih, n, W_ho, m_ho, v_ho, g_ho, (int64_t)D, alpha, 1.f - beta1, 1.f - beta2, eps,
-            alpha_dev, loop_skip_flag());
-    } else {
-        cbow_update_kernel<G2V_OPT_SGD><<<(unsigned)blocks, 256, 0, st>>>(
-            W_ih, nullptr, nullptr, g_ih, n, W_ho, nullptr, nullptr, g_ho, (int64_t)D, lr, 0.f, 0.f, 0.f, nullptr, loop_skip_flag());
-    }
+    const bool adam = optimizer == G2V_OPT_ADAM_TF1;
+    const float alpha = !adam ? lr : alpha_dev ? 0.f : adam_tf1_alpha(lr, beta1, beta2, t);
+    const float omb1 = adam ? 1.f - beta1 : 0.f, omb2 = adam ? 1.f - beta2 : 0.f, eps_ = adam ? eps : 0.f;
+    if (!adam) { m_ih = v_ih = m_ho = v_ho = nullptr; alpha_dev = nullptr; }
+#define G2V_UPDATE(OPT, WD)                                                                                           \
+    cbow_update_kernel<OPT, WD><<<(unsigned)blocks, 256, 0, st>>>(W_ih, m_ih, v_ih, g_ih, n, W_ho, m_ho, v_ho, g_ho,   \
+                                                                  (int64_t)D, alpha, omb1, omb2, eps_, alpha_dev,     \
+                                                                  loop_skip_flag(), weight_decay)
+    G2V_OPT_WD_DISPATCH(optimizer, weight_decay, G2V_UPDATE);
+#undef G2V_UPDATE
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_update(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m_ho, float *v_ho,
+                               float *g_ih, float *g_ho, int32_t V, int32_t D, int32_t optimizer, float lr,
+                               float beta1, float beta2, float eps, int32_t t, const float *alpha_dev,
+                               void *stream) {
+    return g2v_cbow_update_wd(W_ih, W_ho, m_ih, v_ih, m_ho, v_ho, g_ih, g_ho, V, D, optimizer, lr, beta1, beta2, eps, 0.f,
+                              t, alpha_dev, stream);
+}
+
+extern "C" int g2v_cbow_lazy_adam_wd(const int32_t *rows, const int32_t *segptr, const int32_t *pos, const float *dO,
+                                     int64_t n_rows, float *W_ih, float *m_ih, float *v_ih, float *W_ho, float *m_ho,
+                                     float *v_ho, float *g_ho, int32_t V, int32_t D, float lr, float beta1, float beta2,
+                                     float eps, float weight_decay, int32_t t, const float *alpha_dev, void *stream) {
+    G2V_REQUIRE(V > 0 && D > 0 && n_rows >= 0 && n_rows <= V && (t >= 1 || alpha_dev),
+                "g2v_cbow_lazy_adam: bad sizes (V=%d D=%d n_rows=%lld t=%d)", V, D, (long long)n_rows, t);
+    G2V_REQUIRE(W_ih && m_ih && v_ih && W_ho && m_ho && v_ho && g_ho, "g2v_cbow_lazy_adam: null pointer");
+    G2V_REQUIRE(n_rows == 0 || (rows && segptr && pos && dO), "g2v_cbow_lazy_adam: null row list");
+    G2V_REQUIRE(weight_decay_ok(weight_decay),
+                "g2v_cbow_lazy_adam_wd: weight_decay must be finite with 0 <= wd < 1 (got %g)", (double)weight_decay);
+    cudaStream_t st = (cudaStream_t)stream;
+    const float alpha = alpha_dev ? 0.f : adam_tf1_alpha(lr, beta1, beta2, t);
+    const bool wd = weight_decay > 0.f;
+    int rc, launches = 1;
+    if (n_rows > 0) {
+        int grid = 0;
+        auto kern = wd ? cbow_lazy_adam_rows_kernel<true> : cbow_lazy_adam_rows_kernel<false>;
+        if ((rc = rows_grid((const void *)kern, 0, n_rows, &grid))) return rc;
+        kern<<<grid, kCbowWarps * 32, 0, st>>>(rows, segptr, pos, dO, n_rows, W_ih, m_ih, v_ih, W_ho, D, alpha,
+                                               1.f - beta1, 1.f - beta2, eps, alpha_dev, loop_skip_flag(), weight_decay);
+        G2V_CUDA_OK(cudaGetLastError());
+        ++launches;
+    }
+    // W_ho (dense TF1 Adam from g_ho, which it zeroes) after every row has read the pre-step W_ho
+    auto ho = wd ? cbow_update_kernel<G2V_OPT_ADAM_TF1, true> : cbow_update_kernel<G2V_OPT_ADAM_TF1, false>;
+    ho<<<(unsigned)((D + 255) / 256), 256, 0, st>>>(nullptr, nullptr, nullptr, nullptr, 0, W_ho, m_ho, v_ho, g_ho,
+                                                    (int64_t)D, alpha, 1.f - beta1, 1.f - beta2, eps, alpha_dev,
+                                                    loop_skip_flag(), weight_decay);
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch(launches);
     return 0;
 }
 
@@ -1362,40 +1430,21 @@ extern "C" int g2v_cbow_lazy_adam(const int32_t *rows, const int32_t *segptr, co
                                   int64_t n_rows, float *W_ih, float *m_ih, float *v_ih, float *W_ho, float *m_ho,
                                   float *v_ho, float *g_ho, int32_t V, int32_t D, float lr, float beta1, float beta2,
                                   float eps, int32_t t, const float *alpha_dev, void *stream) {
-    G2V_REQUIRE(V > 0 && D > 0 && n_rows >= 0 && n_rows <= V && (t >= 1 || alpha_dev),
-                "g2v_cbow_lazy_adam: bad sizes (V=%d D=%d n_rows=%lld t=%d)", V, D, (long long)n_rows, t);
-    G2V_REQUIRE(W_ih && m_ih && v_ih && W_ho && m_ho && v_ho && g_ho, "g2v_cbow_lazy_adam: null pointer");
-    G2V_REQUIRE(n_rows == 0 || (rows && segptr && pos && dO), "g2v_cbow_lazy_adam: null row list");
-    cudaStream_t st = (cudaStream_t)stream;
-    const float alpha = alpha_dev ? 0.f : adam_tf1_alpha(lr, beta1, beta2, t);
-    int rc, launches = 1;
-    if (n_rows > 0) {
-        int grid = 0;
-        if ((rc = rows_grid((const void *)cbow_lazy_adam_rows_kernel, 0, n_rows, &grid))) return rc;
-        cbow_lazy_adam_rows_kernel<<<grid, kCbowWarps * 32, 0, st>>>(rows, segptr, pos, dO, n_rows, W_ih, m_ih, v_ih,
-                                                                     W_ho, D, alpha, 1.f - beta1, 1.f - beta2, eps,
-                                                                     alpha_dev, loop_skip_flag());
-        G2V_CUDA_OK(cudaGetLastError());
-        ++launches;
-    }
-    // W_ho (dense TF1 Adam from g_ho, which it zeroes) after every row has read the pre-step W_ho
-    cbow_update_kernel<G2V_OPT_ADAM_TF1><<<(unsigned)((D + 255) / 256), 256, 0, st>>>(
-        nullptr, nullptr, nullptr, nullptr, 0, W_ho, m_ho, v_ho, g_ho, (int64_t)D, alpha, 1.f - beta1, 1.f - beta2, eps,
-        alpha_dev, loop_skip_flag());
-    G2V_CUDA_OK(cudaGetLastError());
-    count_launch(launches);
-    return 0;
+    return g2v_cbow_lazy_adam_wd(rows, segptr, pos, dO, n_rows, W_ih, m_ih, v_ih, W_ho, m_ho, v_ho, g_ho, V, D, lr, beta1,
+                                 beta2, eps, 0.f, t, alpha_dev, stream);
 }
 
-extern "C" int g2v_cbow_update_nvl(float *const *g_ptrs_dev, float *const *w_ptrs_dev, float *g_multicast,
-                                   float *w_multicast, float *m_flat, float *v_flat, int64_t n, int32_t rank,
-                                   int32_t world, int32_t optimizer, float lr, float beta1, float beta2, float eps,
-                                   int32_t t, const float *alpha_dev, void *stream) {
+extern "C" int g2v_cbow_update_nvl_wd(float *const *g_ptrs_dev, float *const *w_ptrs_dev, float *g_multicast,
+                                      float *w_multicast, float *m_flat, float *v_flat, int64_t n, int32_t rank,
+                                      int32_t world, int32_t optimizer, float lr, float beta1, float beta2, float eps,
+                                      float weight_decay, int32_t t, const float *alpha_dev, void *stream) {
     G2V_REQUIRE(n > 0 && world >= 1 && rank >= 0 && rank < world && (t >= 1 || alpha_dev), "g2v_cbow_update_nvl: bad sizes");
     G2V_REQUIRE(g_ptrs_dev && w_ptrs_dev, "g2v_cbow_update_nvl: null pointer tables");
     G2V_REQUIRE((g_multicast == nullptr) == (w_multicast == nullptr), "g2v_cbow_update_nvl: both or neither multicast pointer");
     G2V_REQUIRE(optimizer == G2V_OPT_ADAM_TF1 || optimizer == G2V_OPT_SGD, "g2v_cbow_update_nvl: unknown optimizer %d", optimizer);
     G2V_REQUIRE(optimizer == G2V_OPT_SGD || (m_flat && v_flat), "g2v_cbow_update_nvl: Adam needs m/v buffers");
+    G2V_REQUIRE(weight_decay_ok(weight_decay),
+                "g2v_cbow_update_nvl_wd: weight_decay must be finite with 0 <= wd < 1 (got %g)", (double)weight_decay);
     DeviceProps dp;
     if (device_props(&dp)) return 1;
     const int64_t own = ((n >> 2) + world - 1) / world;
@@ -1412,16 +1461,26 @@ extern "C" int g2v_cbow_update_nvl(float *const *g_ptrs_dev, float *const *w_ptr
     } else {
         alpha_dev = nullptr;
     }
-#define G2V_NVL(OPT, MC)                                                                                              \
-    cbow_update_nvl_kernel<OPT, MC><<<(unsigned)blocks, 256, 0, st>>>(g_ptrs_dev, w_ptrs_dev, g_multicast, w_multicast, \
-                                                                      m_flat, v_flat, n, rank, world, alpha, omb1, omb2, \
-                                                                      eps, alpha_dev, loop_skip_flag())
-    if (optimizer == G2V_OPT_ADAM_TF1) { if (mc) G2V_NVL(G2V_OPT_ADAM_TF1, true); else G2V_NVL(G2V_OPT_ADAM_TF1, false); }
-    else { if (mc) G2V_NVL(G2V_OPT_SGD, true); else G2V_NVL(G2V_OPT_SGD, false); }
+#define G2V_NVL(OPT, WD)                                                                                              \
+    do {                                                                                                              \
+        auto kern = mc ? cbow_update_nvl_kernel<OPT, true, WD> : cbow_update_nvl_kernel<OPT, false, WD>;              \
+        kern<<<(unsigned)blocks, 256, 0, st>>>(g_ptrs_dev, w_ptrs_dev, g_multicast, w_multicast, m_flat, v_flat, n,   \
+                                               rank, world, alpha, omb1, omb2, eps, alpha_dev, loop_skip_flag(),      \
+                                               weight_decay);                                                         \
+    } while (0)
+    G2V_OPT_WD_DISPATCH(optimizer, weight_decay, G2V_NVL);
 #undef G2V_NVL
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;
+}
+
+extern "C" int g2v_cbow_update_nvl(float *const *g_ptrs_dev, float *const *w_ptrs_dev, float *g_multicast,
+                                   float *w_multicast, float *m_flat, float *v_flat, int64_t n, int32_t rank,
+                                   int32_t world, int32_t optimizer, float lr, float beta1, float beta2, float eps,
+                                   int32_t t, const float *alpha_dev, void *stream) {
+    return g2v_cbow_update_nvl_wd(g_ptrs_dev, w_ptrs_dev, g_multicast, w_multicast, m_flat, v_flat, n, rank, world,
+                                  optimizer, lr, beta1, beta2, eps, 0.f, t, alpha_dev, stream);
 }
 
 extern "C" int g2v_cbow_step_host(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,

@@ -27,6 +27,20 @@ __device__ __forceinline__ void adam1(float &w, float &m, float &v, float g, flo
     w -= (m * alpha) / (sqrtf(v) + eps);
 }
 
+// Decoupled weight decay (DESIGN.md §4.18), TF1's DecoupledWeightDecayExtension: var -= weight_decay * var before the
+// optimizer step.  Both operations are rounded on their own (never one FMA), so a kernel that decays in a register
+// computes what a separate decay pass followed by the undecayed kernel computes, bit for bit.
+template <bool WD>
+__device__ __forceinline__ void decay1(float &w, float wd) {
+    if (WD) w = __fsub_rn(w, __fmul_rn(wd, w));
+}
+template <bool WD>
+__device__ __forceinline__ void decay4(float4 &w, float wd) {
+    decay1<WD>(w.x, wd); decay1<WD>(w.y, wd); decay1<WD>(w.z, wd); decay1<WD>(w.w, wd);
+}
+// weight_decay as the *_wd entry points admit it: finite, 0 <= wd < 1 (NaN fails both comparisons)
+inline bool weight_decay_ok(float wd) { return wd >= 0.f && wd < 1.f; }
+
 // alpha of step t >= 1, with beta^t by repeated float32 multiplication, as TF1's beta1_power / beta2_power variables
 inline float adam_tf1_alpha(float lr, float beta1, float beta2, int32_t t) {
     float b1p = 1.f, b2p = 1.f;

@@ -152,12 +152,13 @@ r1_csc_reduce_kernel(const int32_t *__restrict__ cscptr, const int32_t *__restri
 
 // ---- dense optimizer pass over the rows -----------------------------------------------------------
 // VEC > 0: D = 128*VEC, register accumulators for g_ho.  VEC == 0: any D, shared-memory accumulators.
-template <int VEC, int OPT>
+// WD: every row is decayed (decay1) before its step, rows with c[g] = 0 included; g_ho takes the pre-decay row.
+template <int VEC, int OPT, bool WD>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 r1_update_kernel(float *__restrict__ W_ih, float *__restrict__ M, float *__restrict__ Vv,
                  const float *__restrict__ W_ho, float *__restrict__ c, float *__restrict__ g_part, int32_t V,
                  int32_t D, float alpha_host, float omb1, float omb2, float eps,
-                 const float *__restrict__ alpha_dev, const int32_t *__restrict__ skip) {
+                 const float *__restrict__ alpha_dev, const int32_t *__restrict__ skip, float wd) {
     G2V_SKIP_IF_STOPPED(skip);
     const float alpha = alpha_dev ? __ldg(alpha_dev + 2) : alpha_host;
     // g_ho = W_ih^T . c is reduced WITHOUT atomics so that the step is bit-reproducible: every warp owns a
@@ -187,6 +188,7 @@ r1_update_kernel(float *__restrict__ W_ih, float *__restrict__ M, float *__restr
             for (int v = 0; v < NV; ++v) {
                 float4 w = w4[v * 32];
                 acc[v].x += cg * w.x; acc[v].y += cg * w.y; acc[v].z += cg * w.z; acc[v].w += cg * w.w;
+                decay4<WD>(w, wd);
                 if (OPT == G2V_OPT_ADAM_TF1) {
                     float4 m = m4[v * 32], vv = v4[v * 32];
                     adam1(w.x, m.x, vv.x, cg * who[v].x, alpha, omb1, omb2, eps);
@@ -195,10 +197,13 @@ r1_update_kernel(float *__restrict__ W_ih, float *__restrict__ M, float *__restr
                     adam1(w.w, m.w, vv.w, cg * who[v].w, alpha, omb1, omb2, eps);
                     m4[v * 32] = m; v4[v * 32] = vv;
                     w4[v * 32] = w;
-                } else if (cg != 0.f) {
-                    w.x -= alpha * cg * who[v].x; w.y -= alpha * cg * who[v].y;
-                    w.z -= alpha * cg * who[v].z; w.w -= alpha * cg * who[v].w;
-                    w4[v * 32] = w;
+                } else {
+                    // SGD skips the arithmetic of a row with c[g] = 0; with WD the decayed row is still stored
+                    if (cg != 0.f) {
+                        w.x -= alpha * cg * who[v].x; w.y -= alpha * cg * who[v].y;
+                        w.z -= alpha * cg * who[v].z; w.w -= alpha * cg * who[v].w;
+                    }
+                    if (WD || cg != 0.f) w4[v * 32] = w;
                 }
             }
             __syncwarp();
@@ -213,6 +218,7 @@ r1_update_kernel(float *__restrict__ W_ih, float *__restrict__ M, float *__restr
             for (int d = lane; d < D; d += 32) {
                 float x = w[d];
                 if (cg != 0.f) my[d] += cg * x;            // lane-owned element of the warp's row
+                decay1<WD>(x, wd);
                 if (OPT == G2V_OPT_ADAM_TF1) {
                     float m = M[(size_t)g * D + d], vv = Vv[(size_t)g * D + d];
                     adam1(x, m, vv, cg * __ldg(W_ho + d), alpha, omb1, omb2, eps);
@@ -237,11 +243,12 @@ r1_update_kernel(float *__restrict__ W_ih, float *__restrict__ M, float *__restr
 
 // W_ho step: g_ho[i] = sum over the update kernel's blocks of g_part[p][i], in a fixed order (32 interleaved
 // slices, then the slices in order) so the result is bit-reproducible, then TF1 Adam / SGD.
-template <int OPT>
+template <int OPT, bool WD>
 __global__ void __launch_bounds__(1024)
 r1_update_ho_kernel(float *__restrict__ W_ho, float *__restrict__ m, float *__restrict__ v,
                     const float *__restrict__ g_part, int32_t n_part, int32_t D, float alpha_host, float omb1,
-                    float omb2, float eps, const float *__restrict__ alpha_dev, const int32_t *__restrict__ skip) {
+                    float omb2, float eps, const float *__restrict__ alpha_dev, const int32_t *__restrict__ skip,
+                    float wd) {
     G2V_SKIP_IF_STOPPED(skip);
     const float alpha = alpha_dev ? __ldg(alpha_dev + 2) : alpha_host;
     __shared__ float sh[32][33];
@@ -257,6 +264,7 @@ r1_update_ho_kernel(float *__restrict__ W_ho, float *__restrict__ m, float *__re
 #pragma unroll
         for (int q = 0; q < 32; ++q) g += sh[q][lane];
         float w = W_ho[i];
+        decay1<WD>(w, wd);
         if (OPT == G2V_OPT_ADAM_TF1) {
             float mm = m[i], vv = v[i];
             adam1(w, mm, vv, g, alpha, omb1, omb2, eps);
@@ -344,21 +352,22 @@ extern "C" int g2v_cbow_r1_windows_csc(const int32_t *rowptr, const int32_t *gen
 
 constexpr int kR1MaxParts = 1024;   // upper bound on the update kernel's grid (scratch = kR1MaxParts * D floats)
 
-template <int VEC, int OPT>
+template <int VEC, int OPT, bool WD>
 static int launch_r1_update(float *W_ih, float *M, float *Vv, const float *W_ho, float *c, float *g_ho, int32_t V,
                             int32_t D, float alpha, float omb1, float omb2, float eps, const float *alpha_dev,
-                            cudaStream_t st, int *grid_out) {
+                            float wd, cudaStream_t st, int *grid_out) {
     const size_t smem = (size_t)kCbowWarps * D * sizeof(float);
     DeviceProps dp;
     if (device_props(&dp)) return 1;
     G2V_REQUIRE(smem <= (size_t)dp.max_smem_optin, "sizeHiddenlayer %d too large", D);
     if (smem > 48 * 1024)
-        G2V_CUDA_OK(cudaFuncSetAttribute(r1_update_kernel<VEC, OPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        G2V_CUDA_OK(cudaFuncSetAttribute(r1_update_kernel<VEC, OPT, WD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem));
     int grid = 0, rc;
-    if ((rc = rows_grid((const void *)r1_update_kernel<VEC, OPT>, smem, V, &grid))) return rc;
+    if ((rc = rows_grid((const void *)r1_update_kernel<VEC, OPT, WD>, smem, V, &grid))) return rc;
     if (grid > kR1MaxParts) grid = kR1MaxParts;
-    r1_update_kernel<VEC, OPT><<<grid, kCbowWarps * 32, smem, st>>>(W_ih, M, Vv, W_ho, c, g_ho, V, D, alpha, omb1, omb2, eps,
-                                                                    alpha_dev, loop_skip_flag());
+    r1_update_kernel<VEC, OPT, WD><<<grid, kCbowWarps * 32, smem, st>>>(W_ih, M, Vv, W_ho, c, g_ho, V, D, alpha, omb1,
+                                                                        omb2, eps, alpha_dev, loop_skip_flag(), wd);
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     *grid_out = grid;
@@ -367,37 +376,54 @@ static int launch_r1_update(float *W_ih, float *M, float *Vv, const float *W_ho,
 
 extern "C" size_t g2v_cbow_r1_scratch_bytes(int32_t D) { return (size_t)kR1MaxParts * (size_t)(D > 0 ? D : 1) * sizeof(float); }
 
-extern "C" int g2v_cbow_r1_update(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m_ho, float *v_ho,
-                                  float *c, float *g_ho, float *s, int32_t V, int32_t D, int32_t optimizer,
-                                  float lr, float beta1, float beta2, float eps, int32_t t, const float *alpha_dev,
-                                  void *stream) {
+extern "C" int g2v_cbow_r1_update_wd(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m_ho, float *v_ho,
+                                     float *c, float *g_ho, float *s, int32_t V, int32_t D, int32_t optimizer,
+                                     float lr, float beta1, float beta2, float eps, float weight_decay, int32_t t,
+                                     const float *alpha_dev, void *stream) {
     G2V_REQUIRE(V > 0 && D > 0 && (t >= 1 || alpha_dev), "g2v_cbow_r1_update: bad sizes (V=%d D=%d t=%d)", V, D, t);
     if (optimizer != G2V_OPT_ADAM_TF1) alpha_dev = nullptr;
     G2V_REQUIRE(W_ih && W_ho && c && g_ho && s, "g2v_cbow_r1_update: null pointer");
     G2V_REQUIRE(optimizer == G2V_OPT_ADAM_TF1 || optimizer == G2V_OPT_SGD, "g2v_cbow_r1_update: unknown optimizer %d", optimizer);
     G2V_REQUIRE(optimizer == G2V_OPT_SGD || (m_ih && v_ih && m_ho && v_ho), "g2v_cbow_r1_update: Adam needs m/v buffers");
+    G2V_REQUIRE(weight_decay_ok(weight_decay),
+                "g2v_cbow_r1_update_wd: weight_decay must be finite with 0 <= wd < 1 (got %g)", (double)weight_decay);
     cudaStream_t st = (cudaStream_t)stream;
+    const bool adam = optimizer == G2V_OPT_ADAM_TF1;
     float alpha = lr, omb1 = 0.f, omb2 = 0.f;
-    if (optimizer == G2V_OPT_ADAM_TF1) {
+    if (adam) {
         alpha = adam_tf1_alpha(lr, beta1, beta2, t);
         omb1 = 1.f - beta1; omb2 = 1.f - beta2;
+    } else {
+        m_ih = v_ih = m_ho = v_ho = nullptr;
     }
-    int rc, parts = 0;
-#define G2V_R1(VEC)                                                                                             \
-    rc = optimizer == G2V_OPT_ADAM_TF1                                                                          \
-             ? launch_r1_update<VEC, G2V_OPT_ADAM_TF1>(W_ih, m_ih, v_ih, W_ho, c, g_ho, V, D, alpha, omb1, omb2, eps, alpha_dev, st, &parts) \
-             : launch_r1_update<VEC, G2V_OPT_SGD>(W_ih, nullptr, nullptr, W_ho, c, g_ho, V, D, alpha, omb1, omb2, eps, alpha_dev, st, &parts)
-    if (D == 128) { G2V_R1(1); }
-    else if (D == 256) { G2V_R1(2); }
-    else if (D == 512) { G2V_R1(4); }
-    else { G2V_R1(0); }
+    int rc = 0, parts = 0;
+#define G2V_R1(OPT, WD)                                                                                               \
+    do {                                                                                                              \
+        if (D == 128) rc = launch_r1_update<1, OPT, WD>(W_ih, m_ih, v_ih, W_ho, c, g_ho, V, D, alpha, omb1, omb2, eps, \
+                                                        alpha_dev, weight_decay, st, &parts);                         \
+        else if (D == 256) rc = launch_r1_update<2, OPT, WD>(W_ih, m_ih, v_ih, W_ho, c, g_ho, V, D, alpha, omb1, omb2, \
+                                                             eps, alpha_dev, weight_decay, st, &parts);               \
+        else if (D == 512) rc = launch_r1_update<4, OPT, WD>(W_ih, m_ih, v_ih, W_ho, c, g_ho, V, D, alpha, omb1, omb2, \
+                                                             eps, alpha_dev, weight_decay, st, &parts);               \
+        else rc = launch_r1_update<0, OPT, WD>(W_ih, m_ih, v_ih, W_ho, c, g_ho, V, D, alpha, omb1, omb2, eps,          \
+                                               alpha_dev, weight_decay, st, &parts);                                  \
+        if (rc) return rc;                                                                                            \
+        r1_update_ho_kernel<OPT, WD><<<(D + 31) / 32, 1024, 0, st>>>(W_ho, m_ho, v_ho, g_ho, parts, D, alpha, omb1,    \
+                                                                     omb2, eps, alpha_dev, loop_skip_flag(),          \
+                                                                     weight_decay);                                   \
+    } while (0)
+    if (adam) { if (weight_decay > 0.f) G2V_R1(G2V_OPT_ADAM_TF1, true); else G2V_R1(G2V_OPT_ADAM_TF1, false); }
+    else { if (weight_decay > 0.f) G2V_R1(G2V_OPT_SGD, true); else G2V_R1(G2V_OPT_SGD, false); }
 #undef G2V_R1
-    if (rc) return rc;
-    if (optimizer == G2V_OPT_ADAM_TF1)
-        r1_update_ho_kernel<G2V_OPT_ADAM_TF1><<<(D + 31) / 32, 1024, 0, st>>>(W_ho, m_ho, v_ho, g_ho, parts, D, alpha, omb1, omb2, eps, alpha_dev, loop_skip_flag());
-    else
-        r1_update_ho_kernel<G2V_OPT_SGD><<<(D + 31) / 32, 1024, 0, st>>>(W_ho, nullptr, nullptr, g_ho, parts, D, alpha, omb1, omb2, eps, nullptr, loop_skip_flag());
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     return g2v_cbow_r1_prepare(W_ih, W_ho, s, V, D, stream);
+}
+
+extern "C" int g2v_cbow_r1_update(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m_ho, float *v_ho,
+                                  float *c, float *g_ho, float *s, int32_t V, int32_t D, int32_t optimizer,
+                                  float lr, float beta1, float beta2, float eps, int32_t t, const float *alpha_dev,
+                                  void *stream) {
+    return g2v_cbow_r1_update_wd(W_ih, W_ho, m_ih, v_ih, m_ho, v_ho, c, g_ho, s, V, D, optimizer, lr, beta1, beta2, eps,
+                                 0.f, t, alpha_dev, stream);
 }

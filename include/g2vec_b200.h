@@ -207,6 +207,37 @@ int g2v_cbow_update(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m
                     float *g_ih, float *g_ho, int32_t V, int32_t D, int32_t optimizer, float lr,
                     float beta1, float beta2, float eps, int32_t t, const float *alpha_dev, void *stream);
 
+/* Decoupled weight decay (DESIGN.md §4.18; TF1 DecoupledWeightDecayExtension, AdamW / SGDW): the *_wd entry points
+ * take the arguments of their counterparts plus `weight_decay` (lambda) after `eps`, and apply
+ *     w <- fl(w - fl(lambda * w))     (two separately rounded operations, never one FMA)
+ * to every parameter element the step updates, before the unchanged Adam / SGD arithmetic on that value.  m and v are
+ * not touched by the decay, the gradients are those of the weights before the step, and lambda is not scaled by the
+ * learning rate.  lambda = 0 launches the same kernels as the counterpart (which is that call with 0), so the results
+ * and the launch count are the counterpart's; lambda must be finite with 0 <= lambda < 1, else the call fails with
+ * g2v_last_error() set and nothing launched.  Elements decayed:
+ *   g2v_cbow_update_wd      every element of W_ih and W_ho;
+ *   g2v_cbow_lazy_adam_wd   the listed rows of W_ih, each once, and all of W_ho; the other rows keep W, m and v;
+ *   g2v_cbow_update_nvl_wd  rank r's slice (and the scalar tail on rank world-1), after the reduce and before the
+ *                           step; the all-gather then delivers the decayed and updated values to every rank;
+ *   g2v_cbow_r1_update_wd   every element of W_ih, rows with c[g] = 0 included (SGD too), and W_ho; g_ho = W_ih^T.c
+ *                           uses W_ih before the decay. */
+int g2v_cbow_update_wd(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m_ho, float *v_ho,
+                       float *g_ih, float *g_ho, int32_t V, int32_t D, int32_t optimizer, float lr,
+                       float beta1, float beta2, float eps, float weight_decay, int32_t t, const float *alpha_dev,
+                       void *stream);
+int g2v_cbow_lazy_adam_wd(const int32_t *rows, const int32_t *segptr, const int32_t *pos, const float *dO,
+                          int64_t n_rows, float *W_ih, float *m_ih, float *v_ih, float *W_ho, float *m_ho, float *v_ho,
+                          float *g_ho, int32_t V, int32_t D, float lr, float beta1, float beta2, float eps,
+                          float weight_decay, int32_t t, const float *alpha_dev, void *stream);
+int g2v_cbow_update_nvl_wd(float *const *g_ptrs_dev, float *const *w_ptrs_dev, float *g_multicast, float *w_multicast,
+                           float *m_flat, float *v_flat, int64_t n, int32_t rank, int32_t world, int32_t optimizer,
+                           float lr, float beta1, float beta2, float eps, float weight_decay, int32_t t,
+                           const float *alpha_dev, void *stream);
+int g2v_cbow_r1_update_wd(float *W_ih, float *W_ho, float *m_ih, float *v_ih, float *m_ho, float *v_ho,
+                          float *c, float *g_ho, float *s, int32_t V, int32_t D, int32_t optimizer,
+                          float lr, float beta1, float beta2, float eps, float weight_decay, int32_t t,
+                          const float *alpha_dev, void *stream);
+
 /* Multi-GPU optimizer epilogue fused with the gradient exchange (one process per GPU, one node): replaces
  * ncclAllReduce(gradient) + g2v_cbow_update.  All buffers are flat [W_ih (V*D) | W_ho (D)] = n floats, the gradient
  * and the parameters in symmetric memory (same size on every rank, peer-mapped): g_ptrs_dev / w_ptrs_dev are DEVICE
