@@ -73,6 +73,11 @@ SIGNATURES = {
     "g2v_cbow_loop_decide_best": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp]),
     "g2v_cbow_loop_keep_best": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp]),
     "g2v_cbow_loop_counters_nvl": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _vp]),
+    "g2v_cbow_val_loss": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _vp, _i32, _vp, _i32, _i32, _vp]),
+    "g2v_cbow_st_prepare": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _vp]),
+    "g2v_cbow_loop_decide_score": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
+    "g2v_cbow_loop_decide_best_score": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "g2v_cbow_loop_score_nvl": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp]),
     "g2v_cbow_slab_plan": (ctypes.c_int, [_i32, _i32, _vp]),
     "g2v_cbow_slab_workspace_bytes": (ctypes.c_size_t, [_i64, _i32, _i32]),
     "g2v_cbow_slab_setup": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _i32, _i32, _vp, _vp]),

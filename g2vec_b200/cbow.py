@@ -141,6 +141,8 @@ class CbowModel:
         # [loss_sum (f64 bits), n_correct_train_fwd, n_correct_val, n_correct_train] as 4 x 8 bytes, then the carry
         # slots a DeviceLoop's tail pass fills for the next step: [carried loss_sum (f64 bits), carried n_correct]
         self.acc = torch.zeros(6, dtype=torch.int64, device=dev)
+        # Q of the validation-loss pass (evaluate(..., loss=True), DESIGN.md §4.19): an exact uint64 fixed-point sum
+        self.q = torch.zeros(1, dtype=torch.int64, device=dev)
         self.t = 0
         # Adam's beta1^t / beta2^t / alpha_t live on the device (TF1's beta*_power variables), advanced by
         # g2v_cbow_adam_tick: no launch of a step depends on a host-side value, so a step can be a CUDA graph
@@ -428,8 +430,10 @@ class CbowModel:
                      self.g_ho.data_ptr(), self.V, self.D, self.opt, self.lr, self.beta1, self.beta2, self.eps, *wd,
                      self.t, adev)
 
-    def evaluate(self, win, slot, win_begin=0, n_win=None):
-        """Add the number of correctly classified listed windows into acc[slot]."""
+    def evaluate(self, win, slot, win_begin=0, n_win=None, loss=False):
+        """Add the number of correctly classified listed windows into acc[slot].  ``loss``: then also add the windows'
+        validation loss Q (g2v_cbow_val_loss, DESIGN.md §4.19) into self.q, from the s = W_ih.W_ho of the weights the
+        count was taken at: rank1's s, the certified pass's st, or on the gene-slab route a fresh st."""
         lo = int(win_begin)
         n = int((win.shape[0] - win_begin) if n_win is None else n_win)
         rec = self.prepared(win)
@@ -448,16 +452,42 @@ class CbowModel:
             self._launch("g2v_cbow_eval_certified", self.rowptr.data_ptr(), self.gene.data_ptr(),
                          self.label.data_ptr(), self._ptr(win), lo, n, self.W_ih.data_ptr(), self.W_ho.data_ptr(),
                          self.st.data_ptr(), acc, None, self.V, self.D, self.reduce, 0)
+        if not loss:
+            return
+        if r in ("r1", "r1_csc"):
+            s, stride = self.s, 1
+        else:
+            if r == "slabs":                     # the slab passes do not write st
+                self._launch("g2v_cbow_st_prepare", self.W_ih.data_ptr(), self.W_ho.data_ptr(), self.st.data_ptr(),
+                             self.V, self.D)
+            s, stride = self.st, 2
+        self._launch("g2v_cbow_val_loss", self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+                     self._ptr(win), lo, n, s.data_ptr(), stride, self.q.data_ptr(), self.V, self.reduce)
 
     def loss_sum(self, acc_host):
         return float(acc_host[:1].view(torch.float64)[0])
 
 
+# what early stopping and the reduce-on-plateau rate can decide on (train_cbow's ``monitor``)
+MONITORS = ("val_acc", "val_loss")
+# the validation-loss pass's fixed point (DESIGN.md §4.19): q_n = rint(min(l_n, LOSS_CAP) * 2^LOSS_BITS), and the
+# monitored score 2^62 - Q, non-negative and higher-is-better like a count
+LOSS_CAP, LOSS_BITS, SCORE_TOP = 64.0, 24, 1 << 62
+
+
+def val_loss_mean(Q, n_val):
+    """The mean validation loss Q 2^-24 / n_val of an integer Q over n_val windows (0 for none)."""
+    return int(Q) / (max(int(n_val), 1) << LOSS_BITS)         # integer true division: correctly rounded
+
+
 def check_config(algo, optimizer, deterministic, several_gpus=False, batch=0, reshuffle=False, patience=1,
-                 lr_patience=0, lr_factor=0.1, min_lr=0.0, weight_decay=0.0):
+                 lr_patience=0, lr_factor=0.1, min_lr=0.0, weight_decay=0.0, monitor="val_acc"):
     """Refuse (ValueError) what train_cbow and CbowModel cannot run, before any device work.  ``several_gpus``: a
     process group of more than one rank; ``batch``, ``reshuffle``, ``patience``, ``lr_patience``, ``lr_factor``,
-    ``min_lr`` and ``weight_decay`` as train_cbow takes them."""
+    ``min_lr``, ``weight_decay`` and ``monitor`` as train_cbow takes them."""
+    if not isinstance(monitor, str) or monitor not in MONITORS:
+        raise ValueError("monitor must be 'val_acc' (the correct validation count) or 'val_loss' (the validation "
+                         "loss): the value early stopping and the reduce-on-plateau rate decide on")
     if (isinstance(weight_decay, bool) or not isinstance(weight_decay, (int, float, np.integer, np.floating))
             or not 0.0 <= float(np.float32(weight_decay)) < 1.0):
         raise ValueError("weight_decay must be a finite number with 0 <= weight_decay < 1 in float32 (the fraction of "
@@ -683,9 +713,18 @@ def _dist():
 def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500, seed=0, optimizer="adam",
                reduce="sum", W_ih0=None, W_ho0=None, split=None, early_stop=True, log=print, return_info=False,
                eval_train="lazy", algo="rows", batch=0, use_graph=True, reshuffle=False, deterministic=False,
-               patience=1, lr_patience=0, lr_factor=0.1, min_lr=0.0, weight_decay=0.0):
+               patience=1, lr_patience=0, lr_factor=0.1, min_lr=0.0, weight_decay=0.0, monitor="val_acc"):
     """Train the modified CBOW on CSR windows and return W_ih (np.float32 [n_genes, hidden]) exactly as
     ``compute_genetovec`` does: the weights after the last step whose validation accuracy did not drop.
+
+    ``monitor``: what early stopping (``patience``) and the reduce-on-plateau rate (``lr_patience``) decide on.
+    "val_acc" (the default): the correct validation count, the reference's rule.  "val_loss": the validation loss
+    (DESIGN.md §4.19), the mean sigmoid BCE of the collapsed logits z = scale * sum_{g in n} (W_ih W_ho)[g] over the
+    validation windows, each term capped at 64 and summed as the exact integer Q = sum rint(min(l, 64) 2^24) (the same
+    for every launch grid and split over the ranks).  Both rules are the ones above with the count replaced by -Q: a
+    step whose Q is <= the best so far becomes the best (ties: the later step) and the ``patience``-th step in a row
+    with a higher Q stops the run; for the rate, only a Q below the best is an improvement.  The epoch lines then show
+    ``LOSS[val]`` = Q 2^-24 / n_val after ``ACC[tr]``.
 
     ``weight_decay`` (λ, finite, 0 <= λ < 1 in float32; 0, the default, = off): decoupled weight decay, AdamW / SGDW
     as TF1's DecoupledWeightDecayExtension applies it (DESIGN.md §4.18).  Every optimizer step first sets each element
@@ -741,12 +780,13 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     ``return_info=True`` also returns a dict: ``history`` [(step, ACC[val], ACC[tr])], ``stop_step`` (the step where
     the run stopped early, else None), ``best_step`` (the step whose W_ih is returned; None if no step ran), ``lr``
     (the float32 learning rate each step trained with), ``lr_reductions`` (the steps whose decision cut the rate;
-    one on the last step has no effect), and more.
+    one on the last step has no effect), ``val_loss`` (with monitor="val_loss": the mean validation loss of every step),
+    and more.
     """
     dist = _dist()
     check_config(algo, optimizer, deterministic, several_gpus=dist is not None, batch=batch, reshuffle=reshuffle,
                  patience=patience, lr_patience=lr_patience, lr_factor=lr_factor, min_lr=min_lr,
-                 weight_decay=weight_decay)
+                 weight_decay=weight_decay, monitor=monitor)
     world, rank =(dist.get_world_size(), dist.get_rank()) if dist else (1, 0)
     rowptr_np = (win_rowptr.cpu().numpy() if isinstance(win_rowptr, torch.Tensor) else np.asarray(win_rowptr))
     N = rowptr_np.shape[0] - 1
@@ -784,25 +824,28 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     if log:
         log("     Start training the modified CBOW with early stopping")
     if max_epoch <= 0:                           # no optimizer step at all: the initial vectors
-        out, hist, stop, best, plateau = model.W_ih, [], None, None, None
+        out, hist, stop, best, plateau, info = model.W_ih, [], None, None, None, None
     elif full_batch:
-        out, hist, stop, best, plateau = _device_loop(model, dist, tr_d, va_d, n_tr, n_va, len(tr_loc), len(va_loc),
-                                                      max_epoch, early_stop, log, eval_train, use_graph,
-                                                      patience=patience)
+        out, hist, stop, best, plateau, info = _device_loop(model, dist, tr_d, va_d, n_tr, n_va, len(tr_loc),
+                                                            len(va_loc), max_epoch, early_stop, log, eval_train,
+                                                            use_graph, patience=patience, monitor=monitor)
     else:
-        out, hist, stop, best, plateau = _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, len(tr_loc),
-                                                         len(va_loc), max_epoch, early_stop, log, batch,
-                                                         reshuffle=(tr_all, seed, rank) if reshuffle else None,
-                                                         patience=patience)
+        out, hist, stop, best, plateau, info = _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, len(tr_loc),
+                                                               len(va_loc), max_epoch, early_stop, log, batch,
+                                                               reshuffle=(tr_all, seed, rank) if reshuffle else None,
+                                                               patience=patience, monitor=monitor)
     if log:
         log("    Optimization Finish")
     out = out.cpu().numpy()
     if return_info:
         rates, cuts = lr_rates(plateau) if plateau is not None else ([float(np.float32(lr))] * len(hist), [])
-        return out, {"history": hist, "stop_step": stop, "best_step": best, "n_train": n_tr, "n_val": n_va,
-                     "lr": rates, "lr_reductions": cuts, "model": model,
-                     "windows": (tr_d, va_d),
-                     "graph": bool(getattr(model, "loop_used_graph", False)), "exchange": model.exchange() if dist else None}
+        res = {"history": hist, "stop_step": stop, "best_step": best, "n_train": n_tr, "n_val": n_va,
+               "lr": rates, "lr_reductions": cuts, "model": model,
+               "windows": (tr_d, va_d),
+               "graph": bool(getattr(model, "loop_used_graph", False)), "exchange": model.exchange() if dist else None}
+        if monitor == "val_loss":
+            res["val_loss"] = list(info.losses) if info is not None else []
+        return out, res
     return out
 
 
@@ -831,21 +874,34 @@ class _LoopLog:
 
     It also follows the early-stop rule with ``patience`` (DESIGN.md §4.15) on the integer validation counts, as
     g2v_cbow_loop_decide[_best] do: ``best_step`` is the step whose weights the loop returns.  ``patience=None``: no
-    early stopping, every step is the new best (the loop returns the last weights)."""
+    early stopping, every step is the new best (the loop returns the last weights).
 
-    def __init__(self, n_tr, n_va, log, patience=1):
+    ``monitor="val_loss"`` (DESIGN.md §4.19): the rule decides on the score 2^62 - Q of the step's validation loss Q
+    (passed as ``q``) instead of the count, as g2v_cbow_loop_decide[_best]_score do, and every epoch line shows the mean
+    loss as ``LOSS[val]`` after ``ACC[tr]``; ``losses`` holds it for every step."""
+
+    def __init__(self, n_tr, n_va, log, patience=1, monitor="val_acc"):
         self.n_tr, self.n_va, self.log = n_tr, n_va, log
         self.hist, self.t0 = [], time.time()
         self.patience = patience
         self.best_val, self.best_step, self.bad = -1, None, 0
         # reduce-on-plateau: a host copy of the rate state whose decisions step() reports (set by the loop), else None
         self.plateau = None
+        self.loss = monitor == "val_loss"
+        self.losses = []
 
-    def stops(self, acc):
-        """Whether a step with counters ``acc`` ends the run under the rule (host-driven loops decide with this)."""
-        return self.patience is not None and int(acc[2]) < self.best_val and self.bad + 1 >= self.patience
+    def _value(self, acc, q):
+        return SCORE_TOP - int(q) if self.loss else int(acc[2])
 
-    def step(self, step, acc, shown, stopped_here):
+    def _loss_txt(self, step):
+        return "\tLOSS[val]=%.6f" % self.losses[step] if self.loss else ""
+
+    def stops(self, acc, q=0):
+        """Whether a step with counters ``acc`` (and validation loss ``q``) ends the run under the rule (host-driven
+        loops decide with this)."""
+        return self.patience is not None and self._value(acc, q) < self.best_val and self.bad + 1 >= self.patience
+
+    def step(self, step, acc, shown, stopped_here, q=0):
         f32 = np.float32
         acc_val = f32(int(acc[2])) / f32(max(self.n_va, 1))
         acc_tr_prev = f32(int(acc[1])) / f32(max(self.n_tr, 1))      # = ACC[tr] of step-1 (SURVEY 3.2-5)
@@ -854,13 +910,17 @@ class _LoopLog:
         if hist and hist[-1][2] is None:
             hist[-1] = (hist[-1][0], hist[-1][1], float(acc_tr_prev))
         hist.append((step, float(acc_val), None if acc_tr is None else float(acc_tr)))
-        if self.patience is None or int(acc[2]) >= self.best_val:
-            self.best_val, self.best_step, self.bad = int(acc[2]), step, 0
+        if self.loss:
+            self.losses.append(val_loss_mean(q, self.n_va))
+        v = self._value(acc, q)
+        if self.patience is None or v >= self.best_val:
+            self.best_val, self.best_step, self.bad = v, step, 0
         else:
             self.bad += 1
         if step % 5 == 0 and log:
             t1 = time.time()
-            log("    - Epoch: %03d\tACC[val]=%.4f\tACC[tr]=%.4f (%.3f sec)" % (step, acc_val, acc_tr, t1 - self.t0))
+            log("    - Epoch: %03d\tACC[val]=%.4f\tACC[tr]=%.4f%s (%.3f sec)" % (step, acc_val, acc_tr,
+                                                                          self._loss_txt(step), t1 - self.t0))
             self.t0 = time.time()
         if self.plateau is not None and log:
             cut = lr_cut(self.plateau, step)
@@ -870,8 +930,8 @@ class _LoopLog:
             # the best step's accuracies; its ACC[tr] is in the history by now (step-1's was filled in above)
             if log:
                 b = hist[self.best_step]
-                log("    - Epoch(stop): %03d\tACC[val]=%.4f\tACC[tr]=%.4f (%.3f sec)"
-                    % (b[0], b[1], b[2], time.time() - self.t0))
+                log("    - Epoch(stop): %03d\tACC[val]=%.4f\tACC[tr]=%.4f%s (%.3f sec)"
+                    % (b[0], b[1], b[2], self._loss_txt(b[0]), time.time() - self.t0))
             return True
         return False
 
@@ -880,7 +940,7 @@ class _LoopLog:
         patience > 1 allows.  Call it once the last step's ACC[tr] is in the history."""
         if self.log and self.hist and self.best_step != self.hist[-1][0]:
             b = self.hist[self.best_step]
-            self.log("    - Epoch(best): %03d\tACC[val]=%.4f\tACC[tr]=%.4f" % b)
+            self.log("    - Epoch(best): %03d\tACC[val]=%.4f\tACC[tr]=%.4f" % b + self._loss_txt(b[0]))
 
 
 class DeviceLoop:
@@ -897,33 +957,42 @@ class DeviceLoop:
 
     Patience (``early_stop`` with ``patience`` > 1, DESIGN.md §4.15): no snapshot at the start of a step; the decision
     is g2v_cbow_loop_decide_best, followed by g2v_cbow_loop_keep_best, which copies W_ih into ``result`` on the steps
-    that improve on the best validation count.  ``result`` then holds the best step's weights however the loop ends."""
+    that improve on the best validation count.  ``result`` then holds the best step's weights however the loop ends.
+
+    ``monitor="val_loss"`` (DESIGN.md §4.19): the validation pass also computes the loss Q, and both rules decide on the
+    score 2^62 - Q (g2v_cbow_loop_decide[_best]_score), recorded per step in ``score_d`` (host copy ``score_pin``)."""
 
     # the smallest patience that takes the keep-best kernels; tests lower it to 1 to check them against the default rule
     keep_best_from = 2
 
-    def __init__(self, model, dist, tr_d, va_d, n_tr, max_epoch, early_stop, snapshot=True, patience=1):
+    def __init__(self, model, dist, tr_d, va_d, n_tr, max_epoch, early_stop, snapshot=True, patience=1,
+                 monitor="val_acc"):
         self.m, self.dist, self.tr_d, self.va_d, self.n_tr = model, dist, tr_d, va_d, n_tr
         self.n_tr_loc, self.n_va_loc = int(tr_d.shape[0]), int(va_d.shape[0])
         self.carried = (dist is None and not model.lazy and self.n_tr_loc > 0
                         and model.route(tr_d) in ("csc", "csc_det"))
+        self.loss = monitor == "val_loss"
         dev = model.device
         self.ctl = torch.zeros(8, dtype=torch.int64, device=dev)
         n_hist = max(max_epoch, 1) * 4
+        # val_loss: one score per step, after the counters in the same allocation (symmetric memory with NVLink)
+        n_score = max(max_epoch, 1) if self.loss else 0
         # with the NVLink exchange the history lives in symmetric memory and the accuracy counters of all ranks are
         # added into it by the ranks themselves (g2v_cbow_loop_counters_nvl): no NCCL call is left in the step
         self.hist_nvl = None
         if dist and model.nvl:
             try:
                 import torch.distributed._symmetric_memory as symm
-                h = symm.empty(n_hist, dtype=torch.int64, device=dev)
+                h = symm.empty(n_hist + n_score, dtype=torch.int64, device=dev)
                 hh = symm.rendezvous(h, dist.group.WORLD)
                 self.hist_nvl = {"h": hh, "mc": int(hh.multicast_ptr or 0) if model.nvl["g_mc"] else 0}
-                self.hist_d = h
+                self.hist_all = h
             except Exception:
                 self.hist_nvl = None
         if self.hist_nvl is None:
-            self.hist_d = torch.zeros(n_hist, dtype=torch.int64, device=dev)
+            self.hist_all = torch.zeros(n_hist + n_score, dtype=torch.int64, device=dev)
+        self.hist_d, self.score_d = self.hist_all[:n_hist], self.hist_all[n_hist:]
+        self.score_pin = torch.zeros(n_score, dtype=torch.int64).pin_memory() if self.loss else None
         self.ctl_pin = torch.zeros(8, dtype=torch.int64).pin_memory()
         self.hist_pin = torch.zeros(max(max_epoch, 1) * 4, dtype=torch.int64).pin_memory()
         self.max_epoch, self.early_stop, self.patience = int(max_epoch), bool(early_stop), int(patience)
@@ -948,9 +1017,11 @@ class DeviceLoop:
         if self.carried:                             # drop a pending carry: its g_ho partial would be added twice
             self.m.g_ho.zero_()
             self.m.acc[4:].zero_()
+        if self.loss:                                # each decision clears Q; drop one a caller left pending
+            self.m.q.zero_()
         if self.hist_nvl:
             self.hist_nvl["h"].barrier(channel=2)    # no rank is still adding into the history of the previous loop
-            self.hist_d.zero_()
+            self.hist_all.zero_()
             self.hist_nvl["h"].barrier(channel=2)    # ... and no rank adds before every history is zero
 
     def attach(self):
@@ -977,7 +1048,10 @@ class DeviceLoop:
         if m_upd is not None:
             m_upd.record()
         if self.n_va_loc:
-            m.evaluate(self.va_d, 2)
+            if self.loss:
+                m.evaluate(self.va_d, 2, loss=True)
+            else:
+                m.evaluate(self.va_d, 2)
         if m_val is not None:
             m_val.record()
         if self.carried:
@@ -985,27 +1059,46 @@ class DeviceLoop:
         elif show and self.n_tr_loc:
             m.evaluate(self.tr_d, 3)
         acc_ptr = m.acc.data_ptr()
+        q_ptr = m.q.data_ptr() if self.loss else None
         if self.hist_nvl:
             hn = self.hist_nvl
             m._launch("g2v_cbow_loop_counters_nvl", self.ctl.data_ptr(), acc_ptr, hn["h"].buffer_ptrs_dev, hn["mc"],
                       m.nvl["world"])
+            if self.loss:                            # Q of every rank into score[step] of every rank
+                m._launch("g2v_cbow_loop_score_nvl", self.ctl.data_ptr(), q_ptr, hn["h"].buffer_ptrs_dev, hn["mc"],
+                          self.hist_d.numel(), m.nvl["world"])
             hn["h"].barrier(channel=3)
-            acc_ptr = None                           # decide on the sums already in hist[step]
+            acc_ptr = q_ptr = None                   # decide on the sums already in hist[step] (and score[step])
         elif dist:
             dist.all_reduce(m.acc[1:4])
+            if self.loss:
+                dist.all_reduce(m.q)
         if self.best is None:
-            m._launch("g2v_cbow_loop_decide", self.ctl.data_ptr(), acc_ptr, self.hist_d.data_ptr())
+            if self.loss:
+                m._launch("g2v_cbow_loop_decide_score", self.ctl.data_ptr(), acc_ptr, self.hist_d.data_ptr(), q_ptr,
+                          self.score_d.data_ptr())
+            else:
+                m._launch("g2v_cbow_loop_decide", self.ctl.data_ptr(), acc_ptr, self.hist_d.data_ptr())
         else:
-            m._launch("g2v_cbow_loop_decide_best", self.ctl.data_ptr(), self.best.data_ptr(), acc_ptr,
-                      self.hist_d.data_ptr())
+            if self.loss:
+                m._launch("g2v_cbow_loop_decide_best_score", self.ctl.data_ptr(), self.best.data_ptr(), acc_ptr,
+                          self.hist_d.data_ptr(), q_ptr, self.score_d.data_ptr())
+            else:
+                m._launch("g2v_cbow_loop_decide_best", self.ctl.data_ptr(), self.best.data_ptr(), acc_ptr,
+                          self.hist_d.data_ptr())
             m._launch("g2v_cbow_loop_keep_best", self.best.data_ptr(), m.W_ih.data_ptr(), self.result.data_ptr(),
                       m.V * m.D)
-        if m.plateau is not None:                # the rate rule on the count the decision just recorded in hist
-            m.lr_decide(self.hist_d.data_ptr() + 16, 4, self.ctl.data_ptr() + 8)
+        if m.plateau is not None:                # the rate rule on the value the decision just recorded
+            if self.loss:
+                m.lr_decide(self.score_d.data_ptr(), 1, self.ctl.data_ptr() + 8)
+            else:
+                m.lr_decide(self.hist_d.data_ptr() + 16, 4, self.ctl.data_ptr() + 8)
 
     def fetch(self):
         self.ctl_pin.copy_(self.ctl, non_blocking=True)
         self.hist_pin.copy_(self.hist_d, non_blocking=True)
+        if self.score_pin is not None:
+            self.score_pin.copy_(self.score_d, non_blocking=True)
         if self.best is not None:
             self.best_pin.copy_(self.best, non_blocking=True)
         if self.plateau_pin is not None:
@@ -1024,26 +1117,27 @@ class DeviceLoop:
 
 
 def _device_loop(model, dist, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_epoch, early_stop, log, eval_train,
-                 use_graph, chunk=5, patience=1):
+                 use_graph, chunk=5, patience=1, monitor="val_acc"):
     """Full-batch loop of G2Vec.py:262-283 with the early-stop rule, the result snapshot and the step counter on
     the DEVICE (g2v_cbow_loop_*): the host enqueues `chunk` iterations at a time -- one CUDA-graph replay of
     4 plain iterations + 1 that also runs the training-accuracy pass (in carried mode, five identical iterations
     that all have it) -- and synchronises once per printed line instead of once per step.  Iterations enqueued after
     the stop are no-ops (every kernel tests ctl.stopped).  Multi-GPU: the all-reduces are part of the captured graph
     (NCCL is capturable); if capture is refused the same launches run eagerly.  Returns (W_ih to return, history,
-    stop step or None, best step, host copy of the model's reduce-on-plateau state or None)."""
+    stop step or None, best step, host copy of the model's reduce-on-plateau state or None, the _LoopLog)."""
     dev = model.device
     loop = DeviceLoop(model, dist, tr_d, va_d, n_tr, max_epoch, early_stop, snapshot=bool(early_stop),
-                      patience=patience)
+                      patience=patience, monitor=monitor)
     shown = lambda s: loop.carried or s % 5 == 0 or eval_train == "always"
-    info = _LoopLog(n_tr, n_va, log, patience if early_stop else None)
+    info = _LoopLog(n_tr, n_va, log, patience if early_stop else None, monitor=monitor)
     info.plateau = loop.plateau_pin
 
     def consume(lo, hi):
         """Host view of steps lo..hi-1 after a sync; True when the loop is over."""
         decided, stop_step = int(loop.ctl_pin[1]), int(loop.ctl_pin[2])
         for s in range(lo, min(hi, decided)):
-            if info.step(s, loop.hist_pin[4 * s:4 * s + 4], shown(s), s == stop_step):
+            q = SCORE_TOP - int(loop.score_pin[s]) if loop.loss else 0
+            if info.step(s, loop.hist_pin[4 * s:4 * s + 4], shown(s), s == stop_step, q):
                 return True
         return bool(int(loop.ctl_pin[0]))
 
@@ -1093,13 +1187,13 @@ def _device_loop(model, dist, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_ep
         loop.detach()
     model.loop_used_graph = graph is not None
     if loop.best is not None:                    # keep-best path: result holds the best step's weights in every case
-        return loop.result, info.hist, stop, int(loop.best_pin[1]), info.plateau
+        return loop.result, info.hist, stop, int(loop.best_pin[1]), info.plateau, info
     # stopped early: the snapshot taken before the dropping step (G2Vec.py:283,286); else the final weights
-    return (loop.result if stop is not None else model.W_ih), info.hist, stop, info.best_step, info.plateau
+    return (loop.result if stop is not None else model.W_ih), info.hist, stop, info.best_step, info.plateau, info
 
 
 def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_loc, max_epoch, early_stop, log, batch,
-                    reshuffle=None, patience=1):
+                    reshuffle=None, patience=1, monitor="val_acc"):
     """north_star's mini-batch variant: one optimizer step (and one gradient all-reduce) per batch of the shuffled
     training list, the reference's per-epoch accuracies and early stop around it; host-driven, one sync per epoch.
     ``reshuffle`` = (global training list on the device, seed, rank): every epoch e >= 1 trains on this rank's share of
@@ -1107,9 +1201,13 @@ def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_l
     buffer's batch plans (one more sync), as does the deterministic mode.  The early-stop rule with ``patience`` is
     applied on the host after the epoch's sync; the result is copied on the epochs that improve on the best.  The
     reduce-on-plateau rule, if the model has it, is decided on the device after the counters' all-reduce and its state
-    read back with them.  Returns what _device_loop returns."""
+    read back with them.  ``monitor="val_loss"``: the validation pass also adds the loss Q into model.q (all-reduced
+    right after the counters), both rules decide on the score 2^62 - Q, and the rate rule reads the score on the device.
+    Returns what _device_loop returns."""
     dev = model.device
-    info = _LoopLog(n_tr, n_va, log, patience if early_stop else None)
+    info = _LoopLog(n_tr, n_va, log, patience if early_stop else None, monitor=monitor)
+    loss = monitor == "val_loss"
+    score_d = torch.zeros(1, dtype=torch.int64, device=dev) if loss else None
     if model.plateau is not None:                # read back with each epoch's counters, for the log and the result
         model.lr_reset()
         info.plateau = torch.empty_like(model.plateau, device="cpu").pin_memory()
@@ -1126,6 +1224,8 @@ def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_l
                 model.prepare_batches(ep_d, batch)
             win = ep_d
         model.acc.zero_()
+        if loss:
+            model.q.zero_()
         for lo in range(0, -(-n_tr // world), per):             # same trip count on every rank (collectives inside)
             nb = max(0, min(per, n_tr_loc - lo))
             nb_tot = nb
@@ -1138,23 +1238,31 @@ def _minibatch_loop(model, dist, world, tr_d, va_d, n_tr, n_va, n_tr_loc, n_va_l
                     dist.all_reduce(g)
             model.update()
         if n_va_loc:
-            model.evaluate(va_d, 2)
+            if loss:
+                model.evaluate(va_d, 2, loss=True)
+            else:
+                model.evaluate(va_d, 2)
         if n_tr_loc:
             model.evaluate(tr_d, 3)                              # acc[1] mixes weights across batches: always evaluate
         if dist:
             dist.all_reduce(model.acc[1:4])
-        if model.plateau is not None:                            # the rate rule on the epoch's (summed) count
-            model.lr_decide(model.acc.data_ptr() + 16)
+            if loss:
+                dist.all_reduce(model.q)
+        if loss:                                                 # score = 2^62 - Q, for the rate rule on the device
+            torch.neg(model.q, out=score_d).add_(SCORE_TOP)
+        if model.plateau is not None:                            # the rate rule on the epoch's (summed) count or score
+            model.lr_decide(score_d.data_ptr() if loss else model.acc.data_ptr() + 16)
             info.plateau.copy_(model.plateau, non_blocking=True)
         acc = model.acc.cpu()                                    # the epoch's only host sync
-        if info.step(step, acc, True, info.stops(acc)):
+        q = int(model.q.cpu()[0]) if loss else 0
+        if info.step(step, acc, True, info.stops(acc, q), q):
             stop = step
             break
         if info.best_step == step:
             result.copy_(model.W_ih)
     if stop is None:
         info.end()
-    return result, info.hist, stop, info.best_step, info.plateau
+    return result, info.hist, stop, info.best_step, info.plateau, info
 
 
 def compute_genetovec(pathList, n_genes, hidden_size, learning_rate, max_epoch=500, seed=0, log=print):

@@ -24,6 +24,12 @@ optimizer step (once per batch with ``--batch``), is not scaled by the learning 
 nothing to the logged loss.  ``adam``, ``sgd`` and ``--algo rank1`` decay every gene vector every step; ``lazy_adam``
 decays only the vectors of the genes a batch gathered.
 
+``--monitor val_loss`` (default ``val_acc``) makes ``--patience`` and ``--lr-patience`` decide on the validation loss
+instead of the validation accuracy: an epoch whose loss is not above the best so far is the new best (ties: the later
+one), and only a loss below the best counts as an improvement for the learning rate.  The loss is the mean sigmoid
+cross-entropy of the validation windows, each term capped at 64, summed exactly in fixed point (2^-24), so for given
+vectors it does not depend on how the windows are split over the GPUs; the epoch lines then show it as ``LOSS[val]`` after ``ACC[tr]`` (DESIGN.md §4.19).
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle``, at every table size (DESIGN.md §4.13);
@@ -83,6 +89,10 @@ def parse_arguments(argv=None):
     p.add_argument('--weight-decay', type=float, default=0.0,
                    help="decoupled weight decay (AdamW / SGDW): every optimizer step first shrinks each weight it "
                         "updates by this fraction, in [0, 1); 0 (default) = off")
+    p.add_argument('--monitor', choices=['val_acc', 'val_loss'], default='val_acc',
+                   help="what --patience and --lr-patience decide on: 'val_acc' (default) = the validation accuracy, "
+                        "'val_loss' = the validation loss (lower is better), also printed as LOSS[val] on the epoch "
+                        "lines")
     args = p.parse_args(argv)
     if not 0.0 <= float(np.float32(args.weight_decay)) < 1.0:
         p.error("--weight-decay must be a finite number with 0 <= weight-decay < 1")
@@ -298,7 +308,8 @@ def main(argv=None):
                           max_epoch=args.epoch, seed=args.seed, log=print, algo=args.algo,   # print is silent off rank 0
                           batch=args.batch, optimizer=args.optimizer, reshuffle=args.reshuffle,
                           deterministic=args.deterministic, patience=args.patience, lr_patience=args.lr_patience,
-                          lr_factor=args.lr_factor, min_lr=args.min_lr, weight_decay=args.weight_decay)
+                          lr_factor=args.lr_factor, min_lr=args.min_lr, weight_decay=args.weight_decay,
+                          monitor=args.monitor)
     genes = data['gene']
     if rank != 0:
         dist.barrier()

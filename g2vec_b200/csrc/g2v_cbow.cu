@@ -31,6 +31,8 @@
 //                                         that a whole step can be replayed as one CUDA graph; adam_tick_lr_kernel
 //                                         reads the learning rate from device memory as well
 //   lr_plateau_kernel                     the reduce-on-plateau rule on the step's validation count (one thread)
+//   val_loss_kernel                       the validation loss as an exact fixed-point integer Q from the collapsed
+//                                         logits (s gathered, no rows); loop_decide[_best]_score_kernel decide on it
 //
 // No tensor cores: the 128..512-wide reduction is a memory-bound gather/scatter, not a dense
 // contraction.  Algorithmic bytes per window: l*(8D+4)+5 with the scatter, l*(4D+12)+9 with the CSC backward
@@ -1027,6 +1029,135 @@ __global__ void lr_plateau_kernel(long long *__restrict__ st, const long long *_
     if (end > st[4]) st[4] = end;
 }
 
+// ---- validation loss (DESIGN.md §4.19) -------------------------------------------------------------------------
+// Q = sum over the listed windows of q_n = rint(min(l_n, 64) 2^24), l_n = max(z,0) - z y + log1p(exp(-|z|)) in float64
+// (64 for a z that is not finite), z = scale * sum_{g in n} s[g] in float32.  The sum over g is r1_windows_kernel's
+// order: lane `sub` of the window's 8 lanes adds s of its genes j = b + sub, b + sub + 8, ... in turn, then the 8
+// partials are combined by the xor-shuffle tree 4, 2, 1.  z therefore depends only on s and the window, and Q, an
+// integer sum, on nothing but the list: not on the grid, the order of the windows or a split of the list.
+// q_n <= 2^30, so a list of fewer than 2^32 windows sums to Q < 2^62 without overflow.
+constexpr double kValLossCap = 64.0, kValLossUnit = 0x1p24;
+constexpr long long kScoreTop = 1ll << 62;
+
+__device__ __forceinline__ unsigned long long val_loss_term(float z, float y) {
+    double l = kValLossCap;
+    if (isfinite(z)) {
+        const double zd = (double)z;
+        l = fmin(fmax(zd, 0.0) - zd * (double)y + log1p(exp(-fabs(zd))), kValLossCap);
+    }
+    return (unsigned long long)rint(l * kValLossUnit);
+}
+
+// s[g] at s[g * s_stride]: 2 for the certified pass's st = {s, t}, 1 for the rank-1 model's s
+__global__ void __launch_bounds__(kCbowWarps * 32)
+val_loss_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
+                const uint8_t *__restrict__ label, const int32_t *__restrict__ win, int64_t win_begin, int64_t n_win,
+                const float *__restrict__ s, int32_t s_stride, unsigned long long *__restrict__ q_sum,
+                int32_t reduce_mean, const int32_t *__restrict__ skip) {
+    G2V_SKIP_IF_STOPPED(skip);
+    __shared__ unsigned long long sh_q;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int sub = lane & 7, slot = lane >> 3;          // 8 lanes per window, 4 windows per warp
+    if (threadIdx.x == 0) sh_q = 0ull;
+    __syncthreads();
+    unsigned long long q_acc = 0ull;
+    const int64_t stride = (int64_t)gridDim.x * kCbowWarps * 4;
+    for (int64_t base = ((int64_t)blockIdx.x * kCbowWarps + warp) * 4; base < n_win; base += stride) {
+        const int64_t i = base + slot;
+        const bool active = i < n_win;
+        int32_t b = 0, e = 0;
+        float y = 0.f;
+        if (active) {
+            const int64_t n = win ? (int64_t)__ldg(win + win_begin + i) : win_begin + i;
+            b = __ldg(rowptr + n); e = __ldg(rowptr + n + 1);
+            y = (float)__ldg(label + n);
+        }
+        float part = 0.f;
+        for (int32_t j = b + sub; j < e; j += 8) part += __ldg(s + (int64_t)__ldg(gene + j) * s_stride);
+        part += __shfl_xor_sync(0xffffffffu, part, 4);
+        part += __shfl_xor_sync(0xffffffffu, part, 2);
+        part += __shfl_xor_sync(0xffffffffu, part, 1);
+        const float scale = (reduce_mean && e > b) ? 1.f / (float)(e - b) : 1.f;
+        if (active && sub == 0) q_acc += val_loss_term(part * scale, y);
+    }
+    q_acc = warp_sum_u64(q_acc);
+    if (lane == 0) atomicAdd(&sh_q, q_acc);
+    __syncthreads();
+    if (threadIdx.x == 0 && sh_q) atomicAdd(q_sum, sh_q);
+}
+
+// The monitored score of a step is 2^62 - Q (Q summed over the ranks): non-negative and higher-is-better, like a
+// validation count, so ctl.before_val = -1 and the plateau state's best = -1 stay "worse than any step".  q != NULL:
+// Q is *q, which is cleared for the next step; q == NULL: score[step] holds the Q the ranks added (loop_score_nvl).
+// score[step] is left holding the score.
+__device__ __forceinline__ long long take_score(long long *__restrict__ score, long long step,
+                                                unsigned long long *__restrict__ q) {
+    const unsigned long long Q = q ? *q : (unsigned long long)score[step];
+    if (q) *q = 0ull;
+    const long long v = kScoreTop - (long long)Q;
+    score[step] = v;
+    return v;
+}
+
+// loop_decide_kernel / loop_decide_best_kernel deciding on score[step] instead of the validation count hist[step][2]
+__global__ void loop_decide_score_kernel(long long *__restrict__ ctl, const long long *__restrict__ acc,
+                                         long long *__restrict__ hist, unsigned long long *__restrict__ q,
+                                         long long *__restrict__ score) {
+    if (ctl[0] != 0) return;
+    const long long step = ctl[1];
+    if (acc)
+        for (int k = 0; k < 4; ++k) hist[step * 4 + k] = acc[k];
+    const long long val = take_score(score, step, q);
+    if (ctl[5] != 0 && val < ctl[3]) {
+        ctl[0] = 1; ctl[2] = step;
+    } else {
+        ctl[3] = val;
+        if (step + 1 >= ctl[4]) ctl[0] = 1;
+    }
+    ctl[1] = step + 1;
+}
+
+__global__ void loop_decide_best_score_kernel(long long *__restrict__ ctl, long long *__restrict__ best,
+                                              const long long *__restrict__ acc, long long *__restrict__ hist,
+                                              unsigned long long *__restrict__ q, long long *__restrict__ score) {
+    if (ctl[0] != 0) {
+        best[3] = 0;
+        return;
+    }
+    const long long step = ctl[1];
+    if (acc)
+        for (int k = 0; k < 4; ++k) hist[step * 4 + k] = acc[k];
+    const long long val = take_score(score, step, q);
+    if (val >= ctl[3]) {
+        ctl[3] = val; best[1] = step; best[2] = 0; best[3] = 1;
+    } else {
+        best[2] += 1; best[3] = 0;
+        if (ctl[5] != 0 && best[2] >= best[0]) {
+            ctl[0] = 1; ctl[2] = step;
+        }
+    }
+    if (step + 1 >= ctl[4]) ctl[0] = 1;
+    ctl[1] = step + 1;
+}
+
+// Multi-GPU: add this rank's Q into score[step] of every rank's symmetric-memory buffer (at element `offset` of it),
+// as loop_counters_nvl_kernel adds the counters, and clear Q.  The caller puts a cross-GPU barrier before the decision.
+__global__ void loop_score_nvl_kernel(const long long *__restrict__ ctl, unsigned long long *__restrict__ q,
+                                      long long *const *__restrict__ ptrs, long long *__restrict__ mc, int64_t offset,
+                                      int32_t world) {
+    if (ctl[0] != 0) return;
+    const long long step = ctl[1];
+    const unsigned long long v = *q;
+    *q = 0ull;
+    if (mc) {
+        asm volatile("multimem.red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(mc + offset + step), "l"(v) : "memory");
+    } else {
+        for (int p = 0; p < world; ++p)
+            atomicAdd_system(reinterpret_cast<unsigned long long *>(ptrs[p] + offset + step), v);
+    }
+    __threadfence_system();
+}
+
 }  // namespace g2v
 
 using namespace g2v;
@@ -1115,6 +1246,66 @@ extern "C" int g2v_cbow_lr_plateau(int64_t *state, const int64_t *counts, int64_
     lr_plateau_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(
         reinterpret_cast<long long *>(state), reinterpret_cast<const long long *>(counts), stride,
         reinterpret_cast<const long long *>(n_decided));
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_val_loss(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                                 int64_t win_begin, int64_t n_win, const float *s, int32_t s_stride, uint64_t *q_sum,
+                                 int32_t V, int32_t reduce, void *stream) {
+    G2V_REQUIRE(V > 0 && n_win >= 0 && win_begin >= 0 && n_win < (1ll << 32) && (s_stride == 1 || s_stride == 2),
+                "g2v_cbow_val_loss: bad sizes (V=%d n_win=%lld s_stride=%d)", V, (long long)n_win, s_stride);
+    G2V_REQUIRE(rowptr && label && s && q_sum, "g2v_cbow_val_loss: null pointer");
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "g2v_cbow_val_loss: unknown reduce %d", reduce);
+    if (n_win == 0) return 0;
+    int grid = 0, rc;
+    if ((rc = rows_grid((const void *)val_loss_kernel, 0, (n_win + 3) / 4, &grid))) return rc;
+    val_loss_kernel<<<grid, kCbowWarps * 32, 0, (cudaStream_t)stream>>>(
+        rowptr, gene, label, win, win_begin, n_win, s, s_stride, reinterpret_cast<unsigned long long *>(q_sum),
+        reduce == G2V_REDUCE_MEAN, loop_skip_flag());
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_st_prepare(const float *W_ih, const float *W_ho, float *st, int32_t V, int32_t D,
+                                   void *stream) {
+    G2V_REQUIRE(V > 0 && D > 0, "g2v_cbow_st_prepare: bad sizes (V=%d D=%d)", V, D);
+    G2V_REQUIRE(W_ih && W_ho && st, "g2v_cbow_st_prepare: null pointer");
+    return launch_r1_prepare(W_ih, W_ho, st, V, D, true, (cudaStream_t)stream);
+}
+
+extern "C" int g2v_cbow_loop_decide_score(int64_t *ctl, const int64_t *acc, int64_t *hist, uint64_t *q,
+                                          int64_t *score, void *stream) {
+    G2V_REQUIRE(ctl && hist && score, "g2v_cbow_loop_decide_score: null pointer");
+    loop_decide_score_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(
+        reinterpret_cast<long long *>(ctl), reinterpret_cast<const long long *>(acc),
+        reinterpret_cast<long long *>(hist), reinterpret_cast<unsigned long long *>(q),
+        reinterpret_cast<long long *>(score));
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_loop_decide_best_score(int64_t *ctl, int64_t *best, const int64_t *acc, int64_t *hist,
+                                               uint64_t *q, int64_t *score, void *stream) {
+    G2V_REQUIRE(ctl && best && hist && score, "g2v_cbow_loop_decide_best_score: null pointer");
+    loop_decide_best_score_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(
+        reinterpret_cast<long long *>(ctl), reinterpret_cast<long long *>(best),
+        reinterpret_cast<const long long *>(acc), reinterpret_cast<long long *>(hist),
+        reinterpret_cast<unsigned long long *>(q), reinterpret_cast<long long *>(score));
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_loop_score_nvl(const int64_t *ctl, uint64_t *q, int64_t *const *ptrs_dev, int64_t *multicast,
+                                       int64_t offset, int32_t world, void *stream) {
+    G2V_REQUIRE(ctl && q && ptrs_dev && offset >= 0 && world >= 1, "g2v_cbow_loop_score_nvl: bad arguments");
+    loop_score_nvl_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(
+        reinterpret_cast<const long long *>(ctl), reinterpret_cast<unsigned long long *>(q),
+        reinterpret_cast<long long *const *>(ptrs_dev), reinterpret_cast<long long *>(multicast), offset, world);
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;

@@ -353,6 +353,38 @@ int g2v_cbow_lr_plateau(int64_t *state, const int64_t *counts, int64_t stride, c
 int g2v_cbow_loop_counters_nvl(const int64_t *ctl, const int64_t *acc, int64_t *const *hist_ptrs_dev,
                                int64_t *hist_multicast, int32_t world, void *stream);
 
+/* Validation-loss monitor (DESIGN.md §4.19): the early-stop and reduce-on-plateau rules decided on the validation
+ * loss instead of the validation count.
+ *   g2v_cbow_val_loss: adds into *q_sum  Q = sum over windows n of the list of q_n = rint(min(l_n, 64) * 2^24), with
+ *        l_n = max(z,0) - z*y + log1p(exp(-|z|)) in float64 (64 when z is not finite) and the collapsed logit
+ *        z = scale_n * sum_{g in n} s[g] in float32 (scale_n = 1 for REDUCE_SUM, 1/len for REDUCE_MEAN).  s[g] is read at
+ *        s[g * s_stride]: s_stride = 2 on the st = {s, t} that g2v_cbow_eval_certified or g2v_cbow_st_prepare wrote,
+ *        1 on the rank-1 model's s.  The sum over g is taken in one fixed order per window (8 lanes, lane k adding
+ *        genes k, k+8, ... of the window, then a shuffle tree 4, 2, 1), so Q is the same integer for any launch grid,
+ *        any order of the windows and any split of the list (the parts' Q add up to the whole's).  q_n <= 2^30 and
+ *        n_win < 2^32, so Q < 2^62 never overflows.  Tests the loop's `stopped` word; one launch, never synchronises.
+ *   g2v_cbow_st_prepare: the first launch of g2v_cbow_eval_certified alone (st = {s, t} per gene, 2*V floats), for a
+ *        list whose count came from another route (the gene slabs).  Tests the loop's `stopped` word.
+ *   The monitored score of a step is 2^62 - Q (non-negative, higher is better), so the loop's sentinels (-1) and
+ *   g2v_cbow_lr_plateau (counts = score, stride = 1) apply to it unchanged.
+ *   g2v_cbow_loop_decide_score / g2v_cbow_loop_decide_best_score: g2v_cbow_loop_decide / g2v_cbow_loop_decide_best
+ *        (same ctl, best, acc, hist forms) deciding on score[step] = 2^62 - Q instead of the validation count.
+ *        q != NULL: Q = *q (summed over the ranks), which is then zeroed for the next step; q == NULL: score[step]
+ *        holds the Q g2v_cbow_loop_score_nvl added.  score[step] is left holding the score.
+ *   g2v_cbow_loop_score_nvl: unless stopped, adds *q into element offset + step of every rank's symmetric buffer
+ *        (multimem.red through multicast, else system-scope atomics on ptrs_dev) and zeroes *q; a cross-GPU barrier
+ *        then precedes the decision with q == NULL on score = buffer + offset. */
+int g2v_cbow_val_loss(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                      int64_t win_begin, int64_t n_win, const float *s, int32_t s_stride, uint64_t *q_sum, int32_t V,
+                      int32_t reduce, void *stream);
+int g2v_cbow_st_prepare(const float *W_ih, const float *W_ho, float *st, int32_t V, int32_t D, void *stream);
+int g2v_cbow_loop_decide_score(int64_t *ctl, const int64_t *acc, int64_t *hist, uint64_t *q, int64_t *score,
+                               void *stream);
+int g2v_cbow_loop_decide_best_score(int64_t *ctl, int64_t *best, const int64_t *acc, int64_t *hist, uint64_t *q,
+                                    int64_t *score, void *stream);
+int g2v_cbow_loop_score_nvl(const int64_t *ctl, uint64_t *q, int64_t *const *ptrs_dev, int64_t *multicast,
+                            int64_t offset, int32_t world, void *stream);
+
 /* ---------------------------------------------------------------------------------------
  * HOT PATH 2 for tables larger than the L2 (csrc/g2v_cbow_slab.cu): the same step as g2v_cbow_fwdbwd /
  * g2v_cbow_eval, processed gene slab by gene slab so that the gathered rows and the gradient rows stay
