@@ -56,8 +56,8 @@ class WalkGraph:
         lib = _capi.load()
         self._ws = torch.zeros(max(int(lib.g2v_walk_workspace_bytes()), 64), dtype=torch.uint8, device=device)
         # packed layouts, built once per graph by g2v_walk_prepare: rows = {begin, end} pairs, edges = {col, qw}
-        # pairs (layout 1) or 16+16-bit words, two neighbours per 8-byte load (layout 2: V <= 65536 and weights in
-        # the |PCC| range [0.5, 1])
+        # pairs (layout 1) or 16+16-bit words, two neighbours per 8-byte load (layout 2: V <= 65535, so that node
+        # ids and the sentinel id V fit 16 bits, and weights in the |PCC| range [0.5, 1])
         import ctypes
         rb, eb = ctypes.c_size_t(0), ctypes.c_size_t(0)
         _capi.check(lib.g2v_walk_packed_bytes(self.V, self.E, ctypes.byref(rb), ctypes.byref(eb)), "g2v_walk_packed_bytes")

@@ -76,7 +76,7 @@ int g2v_walk_launch(const int32_t *rowptr, const int32_t *col, const uint32_t *q
  *   rows  [V]  int32 pairs {begin, end} of each node's out-edges                (g2v_walk_packed_bytes: rows_bytes)
  *   edges      layout 1: uint32 pairs {col, qw}, rows starting at even indices: one 16-byte load brings two
  *              neighbours per lane;
- *              layout 2: uint32 col | (qw - 32768) << 16 [E] -- chosen when V <= 65536 and every
+ *              layout 2: uint32 col | (qw - 32768) << 16 [E] -- chosen when V <= 65535 and every
  *              32768 <= qw <= 65536 (weights |PCC| in [0.5, 1], G2Vec.py:389): one 8-byte load brings two
  *              neighbours per lane                                              (edges_bytes covers both)
  * and returns the layout chosen through *layout_out (a host int; the call synchronises the stream once).
