@@ -58,6 +58,27 @@ SIGNATURES = {
                                               _f32, _f32, _i32, _vp, _vp]),
     "g2v_cbow_r1_update_wd": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _f32, _f32,
                                              _f32, _f32, _f32, _i32, _vp, _vp]),
+    # class-weighted forms (DESIGN.md §4.20): the counterpart's arguments, then w0, w1 before the stream
+    "g2v_cbow_fwdbwd_cw": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                          _i32, _i32, _i32, _f32, _f32, _vp]),
+    "g2v_cbow_fwdbwd_csc_cw": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                              _vp, _i32, _i32, _i32, _f32, _f32, _vp]),
+    "g2v_cbow_fwd_do_cw": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
+                                          _i32, _f32, _f32, _vp]),
+    "g2v_cbow_fwdbwd_csc_det_cw": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                  _vp, _vp, _i32, _i32, _i32, _vp, _i32, _f32, _f32, _vp]),
+    "g2v_cbow_fwd_do_det_cw": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
+                                              _i32, _vp, _i32, _f32, _f32, _vp]),
+    "g2v_cbow_loop_tail_cw": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _i32, _i32,
+                                             _i32, _f32, _f32, _vp]),
+    "g2v_cbow_loop_tail_det_cw": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _i32,
+                                                 _i32, _i32, _vp, _i32, _f32, _f32, _vp]),
+    "g2v_cbow_fwdbwd_slabs_cw": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                _i32, _i32, _i32, _i32, _vp, _f32, _f32, _vp]),
+    "g2v_cbow_r1_windows_cw": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _vp, _vp, _i32, _i32,
+                                              _f32, _f32, _vp]),
+    "g2v_cbow_r1_windows_csc_cw": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                  _i32, _i32, _f32, _f32, _vp]),
     "g2v_cbow_adam_tick": (ctypes.c_int, [_vp, _f32, _f32, _f32, _vp]),
     "g2v_cbow_adam_tick_lr": (ctypes.c_int, [_vp, _vp, _f32, _f32, _vp]),
     "g2v_cbow_lr_plateau": (ctypes.c_int, [_vp, _vp, _i64, _vp, _vp]),

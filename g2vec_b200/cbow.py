@@ -63,8 +63,11 @@ class CbowModel:
 
     def __init__(self, rowptr, gene, label, n_genes, hidden, W_ih0, W_ho0, optimizer="adam", reduce="sum",
                  lr=0.005, beta1=0.9, beta2=0.999, eps=1e-8, device=None, algo="rows", nvl_group=None,
-                 deterministic=False, weight_decay=0.0):
-        check_config(algo, optimizer, deterministic, several_gpus=nvl_group is not None, weight_decay=weight_decay)
+                 deterministic=False, weight_decay=0.0, class_weight=None):
+        check_config(algo, optimizer, deterministic, several_gpus=nvl_group is not None, weight_decay=weight_decay,
+                     class_weight=class_weight)
+        if isinstance(class_weight, str):
+            raise ValueError("CbowModel takes class_weight=None or a pair (w0, w1); train_cbow resolves 'balanced'")
         if not torch.cuda.is_available():
             raise RuntimeError("g2vec_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.lib = _capi.load()
@@ -110,6 +113,9 @@ class CbowModel:
         self.lr, self.beta1, self.beta2, self.eps = float(lr), float(beta1), float(beta2), float(eps)
         # decoupled weight decay (DESIGN.md §4.18), fused into every optimizer launch of update(); 0 = off
         self.wd = float(np.float32(weight_decay))
+        # class weights (w0, w1) of the training loss as float32 values (DESIGN.md §4.20), folded into dO by every
+        # launch that forms it; None = off
+        self.cw = class_weight_pair(class_weight)
         z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
         self.algo = algo
         # rows: scratch of the certified accuracy pass, {s[g], t[g]} per gene (g2v_cbow_eval_certified)
@@ -276,15 +282,18 @@ class CbowModel:
         getattr(self, "_fwdbwd_" + r)(win, rec, 1.0 / float(n_total), int(win_begin), int(n))
 
     def _fwdbwd_scatter(self, win, rec, scale, lo, n):
-        self._launch("g2v_cbow_fwdbwd", self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+        name, cw = self._cw("g2v_cbow_fwdbwd")
+        self._launch(name, self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
                      self._ptr(win), lo, n, scale, self.W_ih.data_ptr(), self.W_ho.data_ptr(), self.g_ih.data_ptr(),
-                     self.g_ho.data_ptr(), self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D, self.reduce)
+                     self.g_ho.data_ptr(), self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D, self.reduce,
+                     *cw)
 
     def _fwdbwd_slabs(self, win, rec, scale, lo, n):
-        self._launch("g2v_cbow_fwdbwd_slabs", self.gene.data_ptr(), self.label.data_ptr(), self._ptr(win), lo, n, scale,
+        name, cw = self._cw("g2v_cbow_fwdbwd_slabs")
+        self._launch(name, self.gene.data_ptr(), self.label.data_ptr(), self._ptr(win), lo, n, scale,
                      self.W_ih.data_ptr(), self.W_ho.data_ptr(), self.g_ih.data_ptr(), self.g_ho.data_ptr(),
                      self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D, self.reduce, self._n_slabs,
-                     rec.slabs[(lo, n)].data_ptr())
+                     rec.slabs[(lo, n)].data_ptr(), *cw)
 
     def _csc_args(self, win, rec, scale, n):
         return (self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(), win.data_ptr(), n, scale,
@@ -293,10 +302,12 @@ class CbowModel:
                 self.acc.data_ptr() + 8, self.V, self.D, self.reduce)
 
     def _fwdbwd_csc(self, win, rec, scale, lo, n):
-        self._launch("g2v_cbow_fwdbwd_csc", *self._csc_args(win, rec, scale, n))
+        name, cw = self._cw("g2v_cbow_fwdbwd_csc")
+        self._launch(name, *self._csc_args(win, rec, scale, n), *cw)
 
     def _fwdbwd_csc_det(self, win, rec, scale, lo, n):
-        self._launch("g2v_cbow_fwdbwd_csc_det", *self._csc_args(win, rec, scale, n), self.det_workspace(n).data_ptr(), 0)
+        name, cw = self._cw("g2v_cbow_fwdbwd_csc_det")
+        self._launch(name, *self._csc_args(win, rec, scale, n), self.det_workspace(n).data_ptr(), 0, *cw)
 
     def _fwdbwd_batch_lazy(self, win, rec, scale, lo, n):
         """dO*scale per position of the batch; update() then applies the lazy step to the batch's rows."""
@@ -312,15 +323,17 @@ class CbowModel:
                      self._dO.data_ptr(), n_rows, self.W_ho.data_ptr(), self.g_ih.data_ptr(), self.V, self.D, 0)
 
     def _fwdbwd_r1(self, win, rec, scale, lo, n):
-        self._launch("g2v_cbow_r1_windows", self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+        name, cw = self._cw("g2v_cbow_r1_windows")
+        self._launch(name, self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
                      self._ptr(win), lo, n, scale, self.s.data_ptr(), self.c.data_ptr(), self.acc.data_ptr(),
-                     self.acc.data_ptr() + 8, self.V, self.reduce)
+                     self.acc.data_ptr() + 8, self.V, self.reduce, *cw)
 
     def _fwdbwd_r1_csc(self, win, rec, scale, lo, n):
-        self._launch("g2v_cbow_r1_windows_csc", self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+        name, cw = self._cw("g2v_cbow_r1_windows_csc")
+        self._launch(name, self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
                      win.data_ptr(), n, scale, self.s.data_ptr(), rec.cscptr.data_ptr(), rec.pos.data_ptr(),
                      rec.dO.data_ptr(), self.c.data_ptr(), self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V,
-                     self.reduce)
+                     self.reduce, *cw)
 
     def det_workspace(self, n):
         """The tile workspace of a deterministic forward over n windows (g2v_cbow_det_workspace_bytes), grown on
@@ -336,9 +349,11 @@ class CbowModel:
                 self.W_ih.data_ptr(), self.W_ho.data_ptr(), self._dO.data_ptr(), self.g_ho.data_ptr(),
                 self.acc.data_ptr(), self.acc.data_ptr() + 8, self.V, self.D, self.reduce)
         if self.det:
-            self._launch("g2v_cbow_fwd_do_det", *args, self.det_workspace(n).data_ptr(), 0)
+            name, cw = self._cw("g2v_cbow_fwd_do_det")
+            self._launch(name, *args, self.det_workspace(n).data_ptr(), 0, *cw)
         else:
-            self._launch("g2v_cbow_fwd_do", *args)
+            name, cw = self._cw("g2v_cbow_fwd_do")
+            self._launch(name, *args, *cw)
 
     def loop_tail(self, ctl, win, n_total):
         """A carried DeviceLoop's training-accuracy pass over ``win``, whose fwdbwd routes to csc or csc_det
@@ -348,9 +363,11 @@ class CbowModel:
                 rec.n, 1.0 / float(n_total), self.W_ih.data_ptr(), self.W_ho.data_ptr(), rec.dO.data_ptr(),
                 self.g_ho.data_ptr(), self.acc.data_ptr(), self.V, self.D, self.reduce)
         if self.det:
-            self._launch("g2v_cbow_loop_tail_det", *args, self.det_workspace(rec.n).data_ptr(), 0)
+            name, cw = self._cw("g2v_cbow_loop_tail_det")
+            self._launch(name, *args, self.det_workspace(rec.n).data_ptr(), 0, *cw)
         else:
-            self._launch("g2v_cbow_loop_tail", *args)
+            name, cw = self._cw("g2v_cbow_loop_tail")
+            self._launch(name, *args, *cw)
 
     def _lazy_update(self, adev):
         plan, r0, n_rows = self._pending or (None, 0, 0)
@@ -390,6 +407,12 @@ class CbowModel:
         model's weight decay, or with weight decay off the plain entry point (the same launches), so that a run
         without decay calls exactly what it called before the option existed."""
         return (name + "_wd", (self.wd,)) if self.wd else (name, ())
+
+    def _cw(self, name):
+        """The dO-forming entry point ``name`` and the arguments it takes before the stream: its _cw form with the
+        model's class weights (w0, w1), or without class weights the plain entry point, so that a run without them
+        calls exactly what it called before the option existed (DESIGN.md §4.20)."""
+        return (name + "_cw", self.cw) if self.cw is not None else (name, ())
 
     def update(self):
         """One optimizer step; every branch decays the elements it updates by the model's weight decay (self.wd, a
@@ -480,11 +503,46 @@ def val_loss_mean(Q, n_val):
     return int(Q) / (max(int(n_val), 1) << LOSS_BITS)         # integer true division: correctly rounded
 
 
+def class_weight_pair(class_weight):
+    """The float32 class weights (w0, w1) of a pair of finite numbers > 0 that stay so in float32, as Python floats;
+    None for None.  Anything else raises ValueError ("balanced" too: train_cbow resolves it from the labels)."""
+    if class_weight is None:
+        return None
+    msg = ("class_weight must be None, 'balanced' or a pair (w0, w1) of finite numbers > 0 that stay finite and > 0 "
+           "in float32 (the weights of the label-0 and label-1 windows in the training loss)")
+    if isinstance(class_weight, (str, bytes)) or not hasattr(class_weight, "__len__") or len(class_weight) != 2:
+        raise ValueError(msg)
+    out = []
+    for w in class_weight:
+        if isinstance(w, (bool, np.bool_)) or not isinstance(w, (int, float, np.integer, np.floating)):
+            raise ValueError(msg)
+        with np.errstate(over="ignore", under="ignore"):
+            w32 = np.float32(w)
+        if not (math.isfinite(float(w32)) and float(w32) > 0.0):
+            raise ValueError(msg)
+        out.append(float(w32))
+    return tuple(out)
+
+
+def balanced_class_weight(labels, tr):
+    """sklearn's compute_class_weight("balanced") on the training split ``tr`` (indices into ``labels``):
+    w_y = float32(n_tr / (2 n_tr,y)), computed in float64.  A split without both labels raises ValueError."""
+    y = np.asarray(labels.cpu() if isinstance(labels, torch.Tensor) else labels).reshape(-1)[np.asarray(tr, np.int64)]
+    n1 = int(np.count_nonzero(y))
+    n = int(y.shape[0])
+    if n1 == 0 or n1 == n:
+        raise ValueError("class_weight='balanced' needs both labels in the training split (it has %d windows of label "
+                         "0 and %d of label 1)" % (n - n1, n1))
+    return (float(np.float32(n / (2.0 * (n - n1)))), float(np.float32(n / (2.0 * n1))))
+
+
 def check_config(algo, optimizer, deterministic, several_gpus=False, batch=0, reshuffle=False, patience=1,
-                 lr_patience=0, lr_factor=0.1, min_lr=0.0, weight_decay=0.0, monitor="val_acc"):
+                 lr_patience=0, lr_factor=0.1, min_lr=0.0, weight_decay=0.0, monitor="val_acc", class_weight=None):
     """Refuse (ValueError) what train_cbow and CbowModel cannot run, before any device work.  ``several_gpus``: a
     process group of more than one rank; ``batch``, ``reshuffle``, ``patience``, ``lr_patience``, ``lr_factor``,
-    ``min_lr``, ``weight_decay`` and ``monitor`` as train_cbow takes them."""
+    ``min_lr``, ``weight_decay``, ``monitor`` and ``class_weight`` as train_cbow takes them."""
+    if not (isinstance(class_weight, str) and class_weight == "balanced"):
+        class_weight_pair(class_weight)
     if not isinstance(monitor, str) or monitor not in MONITORS:
         raise ValueError("monitor must be 'val_acc' (the correct validation count) or 'val_loss' (the validation "
                          "loss): the value early stopping and the reduce-on-plateau rate decide on")
@@ -713,9 +771,18 @@ def _dist():
 def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500, seed=0, optimizer="adam",
                reduce="sum", W_ih0=None, W_ho0=None, split=None, early_stop=True, log=print, return_info=False,
                eval_train="lazy", algo="rows", batch=0, use_graph=True, reshuffle=False, deterministic=False,
-               patience=1, lr_patience=0, lr_factor=0.1, min_lr=0.0, weight_decay=0.0, monitor="val_acc"):
+               patience=1, lr_patience=0, lr_factor=0.1, min_lr=0.0, weight_decay=0.0, monitor="val_acc",
+               class_weight=None):
     """Train the modified CBOW on CSR windows and return W_ih (np.float32 [n_genes, hidden]) exactly as
     ``compute_genetovec`` does: the weights after the last step whose validation accuracy did not drop.
+
+    ``class_weight`` (None, the default, = off; "balanced"; or a pair (w0, w1) of finite numbers > 0): per-class
+    weights of the training loss, Keras ``fit(class_weight=...)`` (DESIGN.md §4.20).  A window of label y counts with
+    w_y: the step's cost is (1/N) sum_n w_{y_n} l_n over its N windows (not normalised by the weights), so
+    dO = fl(fl(fl(sigmoid(o) - y) / N) * w_y), and the logged training loss is the weighted sum.  "balanced" is
+    sklearn's: w_y = float32(n_tr / (2 n_tr,y)) from the labels of the whole training split (the same on every rank);
+    a split without both labels is an error.  The accuracy counts, the validation loss and every early-stop and
+    learning-rate decision keep their definitions.  w = (1, 1) gives the bits of an unweighted run.
 
     ``monitor``: what early stopping (``patience``) and the reduce-on-plateau rate (``lr_patience``) decide on.
     "val_acc" (the default): the correct validation count, the reference's rule.  "val_loss": the validation loss
@@ -781,23 +848,26 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
     the run stopped early, else None), ``best_step`` (the step whose W_ih is returned; None if no step ran), ``lr``
     (the float32 learning rate each step trained with), ``lr_reductions`` (the steps whose decision cut the rate;
     one on the last step has no effect), ``val_loss`` (with monitor="val_loss": the mean validation loss of every step),
-    and more.
+    ``class_weight`` (the float32 weights (w0, w1) the training loss used, None without), and more.
     """
     dist = _dist()
     check_config(algo, optimizer, deterministic, several_gpus=dist is not None, batch=batch, reshuffle=reshuffle,
                  patience=patience, lr_patience=lr_patience, lr_factor=lr_factor, min_lr=min_lr,
-                 weight_decay=weight_decay, monitor=monitor)
+                 weight_decay=weight_decay, monitor=monitor, class_weight=class_weight)
     world, rank =(dist.get_world_size(), dist.get_rank()) if dist else (1, 0)
     rowptr_np = (win_rowptr.cpu().numpy() if isinstance(win_rowptr, torch.Tensor) else np.asarray(win_rowptr))
     N = rowptr_np.shape[0] - 1
     if N < 2:
         raise ValueError("need at least two context windows")
     tr, va = split_indices(N, seed) if split is None else split
+    if isinstance(class_weight, str):            # "balanced", from the global training split
+        class_weight = balanced_class_weight(labels, tr)
     if W_ih0 is None or W_ho0 is None:
         W_ih0, W_ho0 = init_weights(n_genes, hidden, seed)
     model = CbowModel(win_rowptr, win_gene, labels, n_genes, hidden, W_ih0, W_ho0, optimizer, reduce, lr, algo=algo,
                       nvl_group=dist.group.WORLD if (dist and algo == "rows") else None,
-                      deterministic=deterministic and algo == "rows", weight_decay=weight_decay)
+                      deterministic=deterministic and algo == "rows", weight_decay=weight_decay,
+                      class_weight=class_weight)
     if lr_patience > 0:
         model.set_lr_plateau(lr_patience, lr_factor, min_lr, max_epoch)
     lens = np.diff(rowptr_np).astype(np.int64)
@@ -823,6 +893,8 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
         model.prepare_csc(tr_d)
     if log:
         log("     Start training the modified CBOW with early stopping")
+        if model.cw is not None:
+            log("     class weights: w0=%.9g w1=%.9g" % model.cw)
     if max_epoch <= 0:                           # no optimizer step at all: the initial vectors
         out, hist, stop, best, plateau, info = model.W_ih, [], None, None, None, None
     elif full_batch:
@@ -842,7 +914,8 @@ def train_cbow(win_rowptr, win_gene, labels, n_genes, hidden, lr, max_epoch=500,
         res = {"history": hist, "stop_step": stop, "best_step": best, "n_train": n_tr, "n_val": n_va,
                "lr": rates, "lr_reductions": cuts, "model": model,
                "windows": (tr_d, va_d),
-               "graph": bool(getattr(model, "loop_used_graph", False)), "exchange": model.exchange() if dist else None}
+               "graph": bool(getattr(model, "loop_used_graph", False)), "exchange": model.exchange() if dist else None,
+               "class_weight": model.cw}
         if monitor == "val_loss":
             res["val_loss"] = list(info.losses) if info is not None else []
         return out, res

@@ -30,9 +30,17 @@ one), and only a loss below the best counts as an improvement for the learning r
 cross-entropy of the validation windows, each term capped at 64, summed exactly in fixed point (2^-24), so for given
 vectors it does not depend on how the windows are split over the GPUs; the epoch lines then show it as ``LOSS[val]`` after ``ACC[tr]`` (DESIGN.md §4.19).
 
+``--class-weight balanced`` or ``--class-weight W0,W1`` (default off) weights the training loss per label, Keras
+``fit(class_weight=...)``: a window of label y counts W_y times in the step's mean (DESIGN.md §4.20).  ``balanced`` is
+sklearn's rule, W_y = n / (2 n_y) over the training windows, so each label carries half of the loss however the paths
+fall between the groups; a training split with one label only is an error.  The weights must be finite and > 0.  The
+run prints a ``class weights:`` line after ``Start training``; the accuracies, ``LOSS[val]``, ``--patience`` and
+``--lr-patience`` keep their meanings, and the logged training loss is the weighted one.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
-  ``--reshuffle``, at every table size (DESIGN.md §4.13);
+  ``--reshuffle`` or ``--class-weight``, at every table size (DESIGN.md §4.13); ``--class-weight 1,1`` writes the
+  files of the same run without it;
 - ``--algo rank1`` with a full batch.
 Without ``--deterministic`` the rows trainer adds some floating-point values in an order the GPU picks (the
 output-layer gradient every step; the gradient rows with ``--batch`` and adam/sgd, or on tables larger than the
@@ -93,7 +101,12 @@ def parse_arguments(argv=None):
                    help="what --patience and --lr-patience decide on: 'val_acc' (default) = the validation accuracy, "
                         "'val_loss' = the validation loss (lower is better), also printed as LOSS[val] on the epoch "
                         "lines")
+    p.add_argument('--class-weight', type=str, default=None, metavar='{balanced | W0,W1}',
+                   help="weights of the label-0 and label-1 windows in the training loss: 'balanced' = n / (2 n_y) "
+                        "from the training windows, or two finite numbers > 0; default off")
     args = p.parse_args(argv)
+    if args.class_weight is not None:
+        args.class_weight = _parse_class_weight(args.class_weight, p)
     if not 0.0 <= float(np.float32(args.weight_decay)) < 1.0:
         p.error("--weight-decay must be a finite number with 0 <= weight-decay < 1")
     if args.patience < 1:
@@ -111,6 +124,23 @@ def parse_arguments(argv=None):
     if args.deterministic and args.algo == 'rank1' and args.batch > 0:
         p.error("--deterministic with --algo rank1 needs a full batch (--batch 0)")
     return args
+
+
+def _parse_class_weight(text, p):
+    """'balanced', or 'W0,W1' as the pair of float32 weights (finite, > 0 in float32); anything else is p.error."""
+    if text == 'balanced':
+        return text
+    parts = text.split(',')
+    try:
+        if len(parts) != 2:
+            raise ValueError
+        with np.errstate(over='ignore', under='ignore'):
+            w = tuple(np.float32(float(x)) for x in parts)
+    except ValueError:
+        w = None
+    if w is None or not all(np.isfinite(x) and x > 0 for x in w):
+        p.error("--class-weight must be 'balanced' or W0,W1: two numbers that are finite and > 0 in float32")
+    return tuple(float(x) for x in w)
 
 
 # ----------------------------------------------------------------------------------- step 1: I/O
@@ -309,7 +339,7 @@ def main(argv=None):
                           batch=args.batch, optimizer=args.optimizer, reshuffle=args.reshuffle,
                           deterministic=args.deterministic, patience=args.patience, lr_patience=args.lr_patience,
                           lr_factor=args.lr_factor, min_lr=args.min_lr, weight_decay=args.weight_decay,
-                          monitor=args.monitor)
+                          monitor=args.monitor, class_weight=args.class_weight)
     genes = data['gene']
     if rank != 0:
         dist.barrier()

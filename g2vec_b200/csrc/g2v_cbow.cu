@@ -47,7 +47,8 @@ namespace g2v {
 constexpr int kRowsEval = 0, kRowsScatter = 1, kRowsCsc = 2;
 
 // carried != NULL and set: the loop's tail pass already ran this forward at these weights (g2v_cbow_loop_tail).
-template <int VEC, int MODE>
+// CW: the training term of a window of label y is weighted by cw.{x,y}[y] (class_weighted, DESIGN.md §4.20).
+template <int VEC, int MODE, bool CW>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
                  const uint8_t *__restrict__ label, const int32_t *__restrict__ win,
@@ -55,7 +56,7 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
                  const float *__restrict__ W_ho, float *__restrict__ g_ih, float *__restrict__ g_ho,
                  double *__restrict__ loss_sum, unsigned long long *__restrict__ n_correct,
                  int32_t reduce_mean, const int32_t *__restrict__ skip, float *__restrict__ dO_pos,
-                 const int32_t *__restrict__ carried) {
+                 const int32_t *__restrict__ carried, float2 cw) {
     G2V_SKIP_IF_STOPPED(skip);
     G2V_SKIP_IF_STOPPED(carried);
     constexpr bool BACKWARD = MODE != kRowsEval;
@@ -87,17 +88,17 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
         const float o = rows_logit<VEC>(gene, W4, b, e, lane, reduce_mean, who, h, scale);
         if (lane == 0) {
             correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
-            if (BACKWARD) loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
+            if (BACKWARD) loss_acc += class_weighted<CW>(fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o))), y, cw);
         }
         if (MODE == kRowsCsc) {
-            const float dO = (sigmoid_stable(o) - y) * inv_n;
+            const float dO = class_weighted<CW>((sigmoid_stable(o) - y) * inv_n, y, cw);
 #pragma unroll
             for (int v = 0; v < VEC; ++v) {
                 gho[v].x += h[v].x * dO; gho[v].y += h[v].y * dO; gho[v].z += h[v].z * dO; gho[v].w += h[v].w * dO;
             }
             if (lane == 0) dO_pos[i] = dO * scale;
         } else if (MODE == kRowsScatter) {
-            const float dO = (sigmoid_stable(o) - y) * inv_n;
+            const float dO = class_weighted<CW>((sigmoid_stable(o) - y) * inv_n, y, cw);
             float4 gv[VEC];
 #pragma unroll
             for (int v = 0; v < VEC; ++v) {
@@ -122,7 +123,7 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
 
 // Any D (not a multiple of 128): h and the g_ho partial live in shared memory per warp.
 // dO_pos != NULL: the CSC backward of cbow_rows_kernel (dO*scale stored per list position, no scatter).
-template <bool BACKWARD>
+template <bool BACKWARD, bool CW>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 cbow_rows_generic_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
                          const uint8_t *__restrict__ label, const int32_t *__restrict__ win,
@@ -131,7 +132,7 @@ cbow_rows_generic_kernel(const int32_t *__restrict__ rowptr, const int32_t *__re
                          float *__restrict__ g_ho, double *__restrict__ loss_sum,
                          unsigned long long *__restrict__ n_correct, int32_t D, int32_t reduce_mean,
                          const int32_t *__restrict__ skip, float *__restrict__ dO_pos,
-                         const int32_t *__restrict__ carried) {
+                         const int32_t *__restrict__ carried, float2 cw) {
     G2V_SKIP_IF_STOPPED(skip);
     G2V_SKIP_IF_STOPPED(carried);
     extern __shared__ float shf[];
@@ -153,10 +154,10 @@ cbow_rows_generic_kernel(const int32_t *__restrict__ rowptr, const int32_t *__re
         const float o = rows_generic_logit(gene, W_ih, W_ho, b, e, lane, D, reduce_mean, h, scale);
         if (lane == 0) {
             correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
-            if (BACKWARD) loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
+            if (BACKWARD) loss_acc += class_weighted<CW>(fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o))), y, cw);
         }
         if (BACKWARD) {
-            const float dO = (sigmoid_stable(o) - y) * inv_n;
+            const float dO = class_weighted<CW>((sigmoid_stable(o) - y) * inv_n, y, cw);
             for (int d = lane; d < D; d += 32) gho[d] += h[d] * dO;
             const float s = dO * scale;
             if (dO_pos) {
@@ -343,14 +344,14 @@ __host__ __device__ __forceinline__ size_t det_ws_loss_bytes(int64_t n_tiles) {
     return ((size_t)n_tiles * sizeof(double) + 255) & ~(size_t)255;
 }
 
-template <int VEC>
+template <int VEC, bool CW>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 cbow_rows_det_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
                      const uint8_t *__restrict__ label, const int32_t *__restrict__ win, int64_t n_win, float inv_n,
                      const float *__restrict__ W_ih, const float *__restrict__ W_ho, float *__restrict__ dO_pos,
                      double *__restrict__ tile_loss, float *__restrict__ tile_gho,
                      unsigned long long *__restrict__ n_correct, int32_t reduce_mean, const int32_t *__restrict__ skip,
-                     const int32_t *__restrict__ carried) {
+                     const int32_t *__restrict__ carried, float2 cw) {
     G2V_SKIP_IF_STOPPED(skip);
     G2V_SKIP_IF_STOPPED(carried);
     constexpr int D = 128 * VEC;
@@ -412,9 +413,9 @@ cbow_rows_det_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restri
             const float o = warp_sum(part);
             if (lane == 0) {
                 correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
-                loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
+                loss_acc += class_weighted<CW>(fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o))), y, cw);
             }
-            const float dO = (sigmoid_stable(o) - y) * inv_n;
+            const float dO = class_weighted<CW>((sigmoid_stable(o) - y) * inv_n, y, cw);
 #pragma unroll
             for (int v = 0; v < VEC; ++v) {
                 gho[v].x += h[v].x * dO; gho[v].y += h[v].y * dO; gho[v].z += h[v].z * dO; gho[v].w += h[v].w * dO;
@@ -448,13 +449,14 @@ cbow_rows_det_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restri
 }
 
 // Any D: cbow_rows_generic_kernel's CSC mode with the tiles of cbow_rows_det_kernel.
+template <bool CW>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 cbow_rows_generic_det_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
                              const uint8_t *__restrict__ label, const int32_t *__restrict__ win, int64_t n_win,
                              float inv_n, const float *__restrict__ W_ih, const float *__restrict__ W_ho,
                              float *__restrict__ dO_pos, double *__restrict__ tile_loss, float *__restrict__ tile_gho,
                              unsigned long long *__restrict__ n_correct, int32_t D, int32_t reduce_mean,
-                             const int32_t *__restrict__ skip, const int32_t *__restrict__ carried) {
+                             const int32_t *__restrict__ skip, const int32_t *__restrict__ carried, float2 cw) {
     G2V_SKIP_IF_STOPPED(skip);
     G2V_SKIP_IF_STOPPED(carried);
     extern __shared__ float shf[];
@@ -489,9 +491,9 @@ cbow_rows_generic_det_kernel(const int32_t *__restrict__ rowptr, const int32_t *
             const float o = warp_sum(part);
             if (lane == 0) {
                 correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
-                loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
+                loss_acc += class_weighted<CW>(fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o))), y, cw);
             }
-            const float dO = (sigmoid_stable(o) - y) * inv_n;
+            const float dO = class_weighted<CW>((sigmoid_stable(o) - y) * inv_n, y, cw);
             for (int d = lane; d < D; d += 32) gho[d] += h[d] * dO;
             if (lane == 0) dO_pos[i] = dO * scale;
         }
@@ -788,20 +790,23 @@ int rows_grid(const void *kernel, size_t smem, int64_t n_items, int *grid_out) {
 
 // dO_pos != NULL (backward only): the CSC backward -- dO*scale per list position instead of the scatter into g_ih.
 // carried: the word that makes the launched kernel return at once when set (besides `stopped`), or NULL.
-template <bool BACKWARD>
+// CW (backward only): the class-weighted kernels with weights cw (DESIGN.md §4.20).
+template <bool BACKWARD, bool CW = false>
 static int launch_rows(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
                        int64_t win_begin, int64_t n_win, float inv_n, const float *W_ih, const float *W_ho,
                        float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t D,
-                       int32_t reduce, cudaStream_t st, float *dO_pos = nullptr, const int32_t *carried = nullptr) {
+                       int32_t reduce, cudaStream_t st, float *dO_pos = nullptr, const int32_t *carried = nullptr,
+                       float2 cw = float2{1.f, 1.f}) {
+    static_assert(BACKWARD || !CW, "the accuracy pass has no class weights");
     unsigned long long *nc = reinterpret_cast<unsigned long long *>(n_correct);
     int grid = 0, rc;
 #define G2V_LAUNCH_VEC(VEC)                                                                                            \
     {                                                                                                                  \
-        auto kern = !BACKWARD ? cbow_rows_kernel<VEC, kRowsEval>                                                       \
-                              : dO_pos ? cbow_rows_kernel<VEC, kRowsCsc> : cbow_rows_kernel<VEC, kRowsScatter>;        \
+        auto kern = !BACKWARD ? cbow_rows_kernel<VEC, kRowsEval, false>                                                \
+                    : dO_pos  ? cbow_rows_kernel<VEC, kRowsCsc, CW> : cbow_rows_kernel<VEC, kRowsScatter, CW>;         \
         if ((rc = rows_grid((const void *)kern, 0, n_win, &grid))) return rc;                                          \
         kern<<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, win_begin, n_win, inv_n, W_ih, W_ho, g_ih, \
-                                               g_ho, loss_sum, nc, reduce, loop_skip_flag(), dO_pos, carried); \
+                                               g_ho, loss_sum, nc, reduce, loop_skip_flag(), dO_pos, carried, cw); \
     }
     if (D == 128) G2V_LAUNCH_VEC(1)
     else if (D == 256) G2V_LAUNCH_VEC(2)
@@ -812,14 +817,14 @@ static int launch_rows(const int32_t *rowptr, const int32_t *gene, const uint8_t
         if (device_props(&dp)) return 1;
         // the opt-in limit covers the kernel's static shared memory (sh_acc) as well as the dynamic part
         cudaFuncAttributes fa;
-        G2V_CUDA_OK(cudaFuncGetAttributes(&fa, cbow_rows_generic_kernel<BACKWARD>));
+        G2V_CUDA_OK(cudaFuncGetAttributes(&fa, cbow_rows_generic_kernel<BACKWARD, CW>));
         G2V_REQUIRE(smem + fa.sharedSizeBytes <= (size_t)dp.max_smem_optin,
                     "sizeHiddenlayer %d too large for the generic kernel", D);
-        G2V_CUDA_OK(cudaFuncSetAttribute(cbow_rows_generic_kernel<BACKWARD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if ((rc = rows_grid((const void *)cbow_rows_generic_kernel<BACKWARD>, smem, n_win, &grid))) return rc;
-        cbow_rows_generic_kernel<BACKWARD><<<grid, kCbowWarps * 32, smem, st>>>(
+        G2V_CUDA_OK(cudaFuncSetAttribute(cbow_rows_generic_kernel<BACKWARD, CW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        if ((rc = rows_grid((const void *)cbow_rows_generic_kernel<BACKWARD, CW>, smem, n_win, &grid))) return rc;
+        cbow_rows_generic_kernel<BACKWARD, CW><<<grid, kCbowWarps * 32, smem, st>>>(
             rowptr, gene, label, win, win_begin, n_win, inv_n, W_ih, W_ho, g_ih, g_ho, loss_sum, nc, D, reduce, loop_skip_flag(),
-            dO_pos, carried);
+            dO_pos, carried, cw);
     }
 #undef G2V_LAUNCH_VEC
     G2V_CUDA_OK(cudaGetLastError());
@@ -837,10 +842,13 @@ static int det_grid(const void *kernel, size_t smem, int64_t n_items, int32_t ma
 
 // The deterministic forward over win[0..n_win-1] (cbow_rows_det_kernel / cbow_rows_generic_det_kernel) and the fixed-
 // order sum of its tiles into g_ho and loss_sum (cbow_det_sum_kernel).  Both launches also test `carried` (nullable).
+// CW: the class-weighted forward kernels with weights cw (DESIGN.md §4.20).
+template <bool CW = false>
 static int launch_rows_det(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
                            int64_t n_win, float inv_n, const float *W_ih, const float *W_ho, float *dO_pos,
                            float *g_ho, double *loss_sum, int64_t *n_correct, int32_t D, int32_t reduce,
-                           void *workspace, int32_t max_ctas, cudaStream_t st, const int32_t *carried) {
+                           void *workspace, int32_t max_ctas, cudaStream_t st, const int32_t *carried,
+                           float2 cw = float2{1.f, 1.f}) {
     unsigned long long *nc = reinterpret_cast<unsigned long long *>(n_correct);
     const int64_t n_tiles = (n_win + kDetTile - 1) / kDetTile;
     double *tile_loss = reinterpret_cast<double *>(workspace);
@@ -848,11 +856,11 @@ static int launch_rows_det(const int32_t *rowptr, const int32_t *gene, const uin
     int grid = 0, rc;
 #define G2V_LAUNCH_DET(VEC)                                                                                            \
     {                                                                                                                  \
-        if ((rc = det_grid((const void *)cbow_rows_det_kernel<VEC>, 0, n_tiles * kCbowWarps, max_ctas, &grid)))      \
+        if ((rc = det_grid((const void *)cbow_rows_det_kernel<VEC, CW>, 0, n_tiles * kCbowWarps, max_ctas, &grid)))  \
             return rc;                                                                                                 \
-        cbow_rows_det_kernel<VEC><<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, n_win, inv_n, W_ih,     \
-                                                                    W_ho, dO_pos, tile_loss, tile_gho, nc, reduce,     \
-                                                                    loop_skip_flag(), carried);                        \
+        cbow_rows_det_kernel<VEC, CW><<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, n_win, inv_n, W_ih, \
+                                                                        W_ho, dO_pos, tile_loss, tile_gho, nc, reduce, \
+                                                                        loop_skip_flag(), carried, cw);                \
     }
     if (D == 128) G2V_LAUNCH_DET(1)
     else if (D == 256) G2V_LAUNCH_DET(2)
@@ -862,12 +870,12 @@ static int launch_rows_det(const int32_t *rowptr, const int32_t *gene, const uin
         DeviceProps dp;
         if (device_props(&dp)) return 1;
         G2V_REQUIRE(smem + 1024 <= (size_t)dp.max_smem_optin, "sizeHiddenlayer %d too large for the generic kernel", D);
-        G2V_CUDA_OK(cudaFuncSetAttribute(cbow_rows_generic_det_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if ((rc = det_grid((const void *)cbow_rows_generic_det_kernel, smem, n_tiles * kCbowWarps, max_ctas, &grid)))
+        G2V_CUDA_OK(cudaFuncSetAttribute(cbow_rows_generic_det_kernel<CW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        if ((rc = det_grid((const void *)cbow_rows_generic_det_kernel<CW>, smem, n_tiles * kCbowWarps, max_ctas, &grid)))
             return rc;
-        cbow_rows_generic_det_kernel<<<grid, kCbowWarps * 32, smem, st>>>(rowptr, gene, label, win, n_win, inv_n, W_ih,
-                                                                          W_ho, dO_pos, tile_loss, tile_gho, nc, D,
-                                                                          reduce, loop_skip_flag(), carried);
+        cbow_rows_generic_det_kernel<CW><<<grid, kCbowWarps * 32, smem, st>>>(rowptr, gene, label, win, n_win, inv_n,
+                                                                              W_ih, W_ho, dO_pos, tile_loss, tile_gho,
+                                                                              nc, D, reduce, loop_skip_flag(), carried, cw);
     }
 #undef G2V_LAUNCH_DET
     G2V_CUDA_OK(cudaGetLastError());
@@ -1311,32 +1319,57 @@ extern "C" int g2v_cbow_loop_score_nvl(const int64_t *ctl, uint64_t *q, int64_t 
     return 0;
 }
 
+// ---- the entry points that form dO and their class-weighted *_cw forms (DESIGN.md §4.20) ------------------------
+// One body per entry point, a template on CW: the plain form launches the unweighted kernels, the _cw form checks its
+// weights (G2V_CW_CHECK) and launches the weighted instantiations with cw = {w0, w1}.  `name` is the entry point's,
+// for errors.
+
+template <bool CW>
+static int fwdbwd_impl(const char *name, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                       const int32_t *win, int64_t win_begin, int64_t n_win, float inv_n_total, const float *W_ih,
+                       const float *W_ho, float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
+                       int32_t D, int32_t reduce, float2 cw, void *stream) {
+    G2V_REQUIRE(V > 0 && D > 0 && n_win >= 0 && win_begin >= 0, "%s: bad sizes (V=%d D=%d n_win=%lld)", name, V, D, (long long)n_win);
+    G2V_REQUIRE(rowptr && label && W_ih && W_ho && g_ih && g_ho, "%s: null pointer", name);
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "%s: unknown reduce %d", name, reduce);
+    if (n_win == 0) return 0;
+    return launch_rows<true, CW>(rowptr, gene, label, win, win_begin, n_win, inv_n_total, W_ih, W_ho, g_ih, g_ho,
+                                 loss_sum, n_correct, D, reduce, (cudaStream_t)stream, nullptr, nullptr, cw);
+}
+
 extern "C" int g2v_cbow_fwdbwd(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
                                const int32_t *win, int64_t win_begin, int64_t n_win, float inv_n_total,
                                const float *W_ih, const float *W_ho, float *g_ih, float *g_ho,
                                double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce,
                                void *stream) {
-    G2V_REQUIRE(V > 0 && D > 0 && n_win >= 0 && win_begin >= 0, "g2v_cbow_fwdbwd: bad sizes (V=%d D=%d n_win=%lld)", V, D, (long long)n_win);
-    G2V_REQUIRE(rowptr && label && W_ih && W_ho && g_ih && g_ho, "g2v_cbow_fwdbwd: null pointer");
-    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "g2v_cbow_fwdbwd: unknown reduce %d", reduce);
-    if (n_win == 0) return 0;
-    return launch_rows<true>(rowptr, gene, label, win, win_begin, n_win, inv_n_total, W_ih, W_ho, g_ih, g_ho,
-                             loss_sum, n_correct, D, reduce, (cudaStream_t)stream);
+    return fwdbwd_impl<false>("g2v_cbow_fwdbwd", rowptr, gene, label, win, win_begin, n_win, inv_n_total, W_ih, W_ho,
+                              g_ih, g_ho, loss_sum, n_correct, V, D, reduce, float2{1.f, 1.f}, stream);
 }
 
-extern "C" int g2v_cbow_fwdbwd_csc(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
-                                   const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
-                                   const float *W_ho, const int32_t *cscptr, const int32_t *csc_pos, float *dO,
-                                   float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
-                                   int32_t D, int32_t reduce, void *stream) {
-    G2V_REQUIRE(V > 0 && D > 0 && n_win >= 0, "g2v_cbow_fwdbwd_csc: bad sizes (V=%d D=%d n_win=%lld)", V, D, (long long)n_win);
-    G2V_REQUIRE(rowptr && label && W_ih && W_ho && cscptr && dO && g_ih && g_ho, "g2v_cbow_fwdbwd_csc: null pointer");
-    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "g2v_cbow_fwdbwd_csc: unknown reduce %d", reduce);
+extern "C" int g2v_cbow_fwdbwd_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                  const int32_t *win, int64_t win_begin, int64_t n_win, float inv_n_total,
+                                  const float *W_ih, const float *W_ho, float *g_ih, float *g_ho,
+                                  double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce,
+                                  float w0, float w1, void *stream) {
+    G2V_CW_CHECK("g2v_cbow_fwdbwd_cw");
+    return fwdbwd_impl<true>("g2v_cbow_fwdbwd_cw", rowptr, gene, label, win, win_begin, n_win, inv_n_total, W_ih, W_ho,
+                             g_ih, g_ho, loss_sum, n_correct, V, D, reduce, float2{w0, w1}, stream);
+}
+
+template <bool CW>
+static int fwdbwd_csc_impl(const char *name, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                           const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
+                           const int32_t *cscptr, const int32_t *csc_pos, float *dO, float *g_ih, float *g_ho,
+                           double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce, float2 cw,
+                           void *stream) {
+    G2V_REQUIRE(V > 0 && D > 0 && n_win >= 0, "%s: bad sizes (V=%d D=%d n_win=%lld)", name, V, D, (long long)n_win);
+    G2V_REQUIRE(rowptr && label && W_ih && W_ho && cscptr && dO && g_ih && g_ho, "%s: null pointer", name);
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "%s: unknown reduce %d", name, reduce);
     if (n_win == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
     // with a tail pass pending (attached loop, ctl[6] set) the forward returns at once and the expansion reads its dO
-    int rc = launch_rows<true>(rowptr, gene, label, win, 0, n_win, inv_n_total, W_ih, W_ho, g_ih, g_ho, loss_sum,
-                               n_correct, D, reduce, st, dO, loop_carry_flag());
+    int rc = launch_rows<true, CW>(rowptr, gene, label, win, 0, n_win, inv_n_total, W_ih, W_ho, g_ih, g_ho, loss_sum,
+                                   n_correct, D, reduce, st, dO, loop_carry_flag(), cw);
     if (rc) return rc;
     int grid = 0;
     if ((rc = rows_grid((const void *)cbow_csc_expand_kernel, 0, V, &grid))) return rc;
@@ -1346,31 +1379,89 @@ extern "C" int g2v_cbow_fwdbwd_csc(const int32_t *rowptr, const int32_t *gene, c
     return 0;
 }
 
+extern "C" int g2v_cbow_fwdbwd_csc(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                   const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                                   const float *W_ho, const int32_t *cscptr, const int32_t *csc_pos, float *dO,
+                                   float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
+                                   int32_t D, int32_t reduce, void *stream) {
+    return fwdbwd_csc_impl<false>("g2v_cbow_fwdbwd_csc", rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho,
+                                  cscptr, csc_pos, dO, g_ih, g_ho, loss_sum, n_correct, V, D, reduce, float2{1.f, 1.f},
+                                  stream);
+}
+
+extern "C" int g2v_cbow_fwdbwd_csc_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                      const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                                      const float *W_ho, const int32_t *cscptr, const int32_t *csc_pos, float *dO,
+                                      float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
+                                      int32_t D, int32_t reduce, float w0, float w1, void *stream) {
+    G2V_CW_CHECK("g2v_cbow_fwdbwd_csc_cw");
+    return fwdbwd_csc_impl<true>("g2v_cbow_fwdbwd_csc_cw", rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho,
+                                 cscptr, csc_pos, dO, g_ih, g_ho, loss_sum, n_correct, V, D, reduce, float2{w0, w1},
+                                 stream);
+}
+
+template <bool CW>
+static int fwd_do_impl(const char *name, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                       const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
+                       float *dO, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V, int32_t D,
+                       int32_t reduce, float2 cw, void *stream) {
+    G2V_REQUIRE(V > 0 && D > 0 && n_win >= 0, "%s: bad sizes (V=%d D=%d n_win=%lld)", name, V, D, (long long)n_win);
+    G2V_REQUIRE(rowptr && label && W_ih && W_ho && dO && g_ho, "%s: null pointer", name);
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "%s: unknown reduce %d", name, reduce);
+    if (n_win == 0) return 0;
+    return launch_rows<true, CW>(rowptr, gene, label, win, 0, n_win, inv_n_total, W_ih, W_ho, nullptr, g_ho, loss_sum,
+                                 n_correct, D, reduce, (cudaStream_t)stream, dO, nullptr, cw);
+}
+
 extern "C" int g2v_cbow_fwd_do(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
                                int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho, float *dO,
                                float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce,
                                void *stream) {
-    G2V_REQUIRE(V > 0 && D > 0 && n_win >= 0, "g2v_cbow_fwd_do: bad sizes (V=%d D=%d n_win=%lld)", V, D, (long long)n_win);
-    G2V_REQUIRE(rowptr && label && W_ih && W_ho && dO && g_ho, "g2v_cbow_fwd_do: null pointer");
-    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "g2v_cbow_fwd_do: unknown reduce %d", reduce);
-    if (n_win == 0) return 0;
-    return launch_rows<true>(rowptr, gene, label, win, 0, n_win, inv_n_total, W_ih, W_ho, nullptr, g_ho, loss_sum,
-                             n_correct, D, reduce, (cudaStream_t)stream, dO);
+    return fwd_do_impl<false>("g2v_cbow_fwd_do", rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho,
+                              loss_sum, n_correct, V, D, reduce, float2{1.f, 1.f}, stream);
+}
+
+extern "C" int g2v_cbow_fwd_do_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                                  int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho, float *dO,
+                                  float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V, int32_t D,
+                                  int32_t reduce, float w0, float w1, void *stream) {
+    G2V_CW_CHECK("g2v_cbow_fwd_do_cw");
+    return fwd_do_impl<true>("g2v_cbow_fwd_do_cw", rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho,
+                             loss_sum, n_correct, V, D, reduce, float2{w0, w1}, stream);
+}
+
+template <bool CW>
+static int loop_tail_impl(const char *name, int64_t *ctl, const int32_t *rowptr, const int32_t *gene,
+                          const uint8_t *label, const int32_t *win, int64_t n_win, float inv_n_total,
+                          const float *W_ih, const float *W_ho, float *dO, float *g_ho, int64_t *acc, int32_t V,
+                          int32_t D, int32_t reduce, float2 cw, void *stream) {
+    G2V_REQUIRE(ctl && acc, "%s: null loop state", name);
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = fwd_do_impl<CW>(CW ? "g2v_cbow_fwd_do_cw" : "g2v_cbow_fwd_do", rowptr, gene, label, win, n_win,
+                             inv_n_total, W_ih, W_ho, dO, g_ho, reinterpret_cast<double *>(acc + 4), acc + 5, V, D,
+                             reduce, cw, st);
+    if (rc) return rc;
+    loop_carry_kernel<<<1, 1, 0, st>>>(reinterpret_cast<long long *>(ctl), reinterpret_cast<long long *>(acc));
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
 }
 
 extern "C" int g2v_cbow_loop_tail(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
                                   const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
                                   const float *W_ho, float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D,
                                   int32_t reduce, void *stream) {
-    G2V_REQUIRE(ctl && acc, "g2v_cbow_loop_tail: null loop state");
-    cudaStream_t st = (cudaStream_t)stream;
-    int rc = g2v_cbow_fwd_do(rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho,
-                             reinterpret_cast<double *>(acc + 4), acc + 5, V, D, reduce, st);
-    if (rc) return rc;
-    loop_carry_kernel<<<1, 1, 0, st>>>(reinterpret_cast<long long *>(ctl), reinterpret_cast<long long *>(acc));
-    G2V_CUDA_OK(cudaGetLastError());
-    count_launch();
-    return 0;
+    return loop_tail_impl<false>("g2v_cbow_loop_tail", ctl, rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho,
+                                 dO, g_ho, acc, V, D, reduce, float2{1.f, 1.f}, stream);
+}
+
+extern "C" int g2v_cbow_loop_tail_cw(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                     const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                                     const float *W_ho, float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D,
+                                     int32_t reduce, float w0, float w1, void *stream) {
+    G2V_CW_CHECK("g2v_cbow_loop_tail_cw");
+    return loop_tail_impl<true>("g2v_cbow_loop_tail_cw", ctl, rowptr, gene, label, win, n_win, inv_n_total, W_ih,
+                                W_ho, dO, g_ho, acc, V, D, reduce, float2{w0, w1}, stream);
 }
 
 extern "C" size_t g2v_cbow_det_workspace_bytes(int64_t n_win, int32_t D) {
@@ -1379,25 +1470,27 @@ extern "C" size_t g2v_cbow_det_workspace_bytes(int64_t n_win, int32_t D) {
     return det_ws_loss_bytes(n_tiles) + (size_t)n_tiles * (size_t)D * sizeof(float);
 }
 
+// name: the entry point's, a runtime string (errors)
 #define G2V_DET_CHECK(name)                                                                                            \
-    G2V_REQUIRE(V > 0 && D > 0 && n_win >= 0 && max_ctas >= 0, name ": bad sizes (V=%d D=%d n_win=%lld max_ctas=%d)", \
-                V, D, (long long)n_win, max_ctas);                                                                     \
+    G2V_REQUIRE(V > 0 && D > 0 && n_win >= 0 && max_ctas >= 0, "%s: bad sizes (V=%d D=%d n_win=%lld max_ctas=%d)",  \
+                name, V, D, (long long)n_win, max_ctas);                                                               \
     G2V_REQUIRE(n_win == 0 || (rowptr && gene && label && win && W_ih && W_ho && dO && g_ho && workspace),            \
-                name ": null pointer");                                                                                \
-    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, name ": unknown reduce %d", reduce)
+                "%s: null pointer", name);                                                                             \
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "%s: unknown reduce %d", name, reduce)
 
-extern "C" int g2v_cbow_fwdbwd_csc_det(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
-                                       const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
-                                       const float *W_ho, const int32_t *cscptr, const int32_t *csc_pos, float *dO,
-                                       float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
-                                       int32_t D, int32_t reduce, void *workspace, int32_t max_ctas, void *stream) {
-    G2V_DET_CHECK("g2v_cbow_fwdbwd_csc_det");
+template <bool CW>
+static int fwdbwd_csc_det_impl(const char *name, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                               const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                               const float *W_ho, const int32_t *cscptr, const int32_t *csc_pos, float *dO,
+                               float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V, int32_t D,
+                               int32_t reduce, void *workspace, int32_t max_ctas, float2 cw, void *stream) {
+    G2V_DET_CHECK(name);
     // csc_pos may be NULL: a list of empty windows has no incidences (every CSC segment is empty)
-    G2V_REQUIRE(n_win == 0 || (cscptr && g_ih), "g2v_cbow_fwdbwd_csc_det: null pointer");
+    G2V_REQUIRE(n_win == 0 || (cscptr && g_ih), "%s: null pointer", name);
     if (n_win == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
-    int rc = launch_rows_det(rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho, loss_sum, n_correct,
-                             D, reduce, workspace, max_ctas, st, loop_carry_flag());
+    int rc = launch_rows_det<CW>(rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho, loss_sum,
+                                 n_correct, D, reduce, workspace, max_ctas, st, loop_carry_flag(), cw);
     if (rc) return rc;
     int grid = 0;
     if ((rc = det_grid((const void *)cbow_csc_expand_kernel, 0, V, max_ctas, &grid))) return rc;
@@ -1407,31 +1500,96 @@ extern "C" int g2v_cbow_fwdbwd_csc_det(const int32_t *rowptr, const int32_t *gen
     return 0;
 }
 
+extern "C" int g2v_cbow_fwdbwd_csc_det(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                       const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                                       const float *W_ho, const int32_t *cscptr, const int32_t *csc_pos, float *dO,
+                                       float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
+                                       int32_t D, int32_t reduce, void *workspace, int32_t max_ctas, void *stream) {
+    return fwdbwd_csc_det_impl<false>("g2v_cbow_fwdbwd_csc_det", rowptr, gene, label, win, n_win, inv_n_total, W_ih,
+                                      W_ho, cscptr, csc_pos, dO, g_ih, g_ho, loss_sum, n_correct, V, D, reduce,
+                                      workspace, max_ctas, float2{1.f, 1.f}, stream);
+}
+
+extern "C" int g2v_cbow_fwdbwd_csc_det_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                          const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                                          const float *W_ho, const int32_t *cscptr, const int32_t *csc_pos, float *dO,
+                                          float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
+                                          int32_t D, int32_t reduce, void *workspace, int32_t max_ctas, float w0,
+                                          float w1, void *stream) {
+    G2V_CW_CHECK("g2v_cbow_fwdbwd_csc_det_cw");
+    return fwdbwd_csc_det_impl<true>("g2v_cbow_fwdbwd_csc_det_cw", rowptr, gene, label, win, n_win, inv_n_total, W_ih,
+                                     W_ho, cscptr, csc_pos, dO, g_ih, g_ho, loss_sum, n_correct, V, D, reduce,
+                                     workspace, max_ctas, float2{w0, w1}, stream);
+}
+
+template <bool CW>
+static int fwd_do_det_impl(const char *name, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                           const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
+                           float *dO, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V, int32_t D,
+                           int32_t reduce, void *workspace, int32_t max_ctas, float2 cw, void *stream) {
+    G2V_DET_CHECK(name);
+    if (n_win == 0) return 0;
+    return launch_rows_det<CW>(rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho, loss_sum, n_correct,
+                               D, reduce, workspace, max_ctas, (cudaStream_t)stream, nullptr, cw);
+}
+#undef G2V_DET_CHECK
+
 extern "C" int g2v_cbow_fwd_do_det(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
                                    const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
                                    const float *W_ho, float *dO, float *g_ho, double *loss_sum, int64_t *n_correct,
                                    int32_t V, int32_t D, int32_t reduce, void *workspace, int32_t max_ctas,
                                    void *stream) {
-    G2V_DET_CHECK("g2v_cbow_fwd_do_det");
-    if (n_win == 0) return 0;
-    return launch_rows_det(rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho, loss_sum, n_correct, D,
-                           reduce, workspace, max_ctas, (cudaStream_t)stream, nullptr);
+    return fwd_do_det_impl<false>("g2v_cbow_fwd_do_det", rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO,
+                                  g_ho, loss_sum, n_correct, V, D, reduce, workspace, max_ctas, float2{1.f, 1.f},
+                                  stream);
 }
-#undef G2V_DET_CHECK
 
-extern "C" int g2v_cbow_loop_tail_det(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+extern "C" int g2v_cbow_fwd_do_det_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
                                       const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
-                                      const float *W_ho, float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D,
-                                      int32_t reduce, void *workspace, int32_t max_ctas, void *stream) {
-    G2V_REQUIRE(ctl && acc, "g2v_cbow_loop_tail_det: null loop state");
+                                      const float *W_ho, float *dO, float *g_ho, double *loss_sum, int64_t *n_correct,
+                                      int32_t V, int32_t D, int32_t reduce, void *workspace, int32_t max_ctas,
+                                      float w0, float w1, void *stream) {
+    G2V_CW_CHECK("g2v_cbow_fwd_do_det_cw");
+    return fwd_do_det_impl<true>("g2v_cbow_fwd_do_det_cw", rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho,
+                                 dO, g_ho, loss_sum, n_correct, V, D, reduce, workspace, max_ctas, float2{w0, w1},
+                                 stream);
+}
+
+template <bool CW>
+static int loop_tail_det_impl(const char *name, int64_t *ctl, const int32_t *rowptr, const int32_t *gene,
+                              const uint8_t *label, const int32_t *win, int64_t n_win, float inv_n_total,
+                              const float *W_ih, const float *W_ho, float *dO, float *g_ho, int64_t *acc, int32_t V,
+                              int32_t D, int32_t reduce, void *workspace, int32_t max_ctas, float2 cw, void *stream) {
+    G2V_REQUIRE(ctl && acc, "%s: null loop state", name);
     cudaStream_t st = (cudaStream_t)stream;
-    int rc = g2v_cbow_fwd_do_det(rowptr, gene, label, win, n_win, inv_n_total, W_ih, W_ho, dO, g_ho,
-                                 reinterpret_cast<double *>(acc + 4), acc + 5, V, D, reduce, workspace, max_ctas, st);
+    int rc = fwd_do_det_impl<CW>(CW ? "g2v_cbow_fwd_do_det_cw" : "g2v_cbow_fwd_do_det", rowptr, gene, label, win,
+                                 n_win, inv_n_total, W_ih, W_ho, dO, g_ho, reinterpret_cast<double *>(acc + 4),
+                                 acc + 5, V, D, reduce, workspace, max_ctas, cw, st);
     if (rc) return rc;
     loop_carry_kernel<<<1, 1, 0, st>>>(reinterpret_cast<long long *>(ctl), reinterpret_cast<long long *>(acc));
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;
+}
+
+extern "C" int g2v_cbow_loop_tail_det(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                      const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                                      const float *W_ho, float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D,
+                                      int32_t reduce, void *workspace, int32_t max_ctas, void *stream) {
+    return loop_tail_det_impl<false>("g2v_cbow_loop_tail_det", ctl, rowptr, gene, label, win, n_win, inv_n_total,
+                                     W_ih, W_ho, dO, g_ho, acc, V, D, reduce, workspace, max_ctas, float2{1.f, 1.f},
+                                     stream);
+}
+
+extern "C" int g2v_cbow_loop_tail_det_cw(int64_t *ctl, const int32_t *rowptr, const int32_t *gene,
+                                         const uint8_t *label, const int32_t *win, int64_t n_win, float inv_n_total,
+                                         const float *W_ih, const float *W_ho, float *dO, float *g_ho, int64_t *acc,
+                                         int32_t V, int32_t D, int32_t reduce, void *workspace, int32_t max_ctas,
+                                         float w0, float w1, void *stream) {
+    G2V_CW_CHECK("g2v_cbow_loop_tail_det_cw");
+    return loop_tail_det_impl<true>("g2v_cbow_loop_tail_det_cw", ctl, rowptr, gene, label, win, n_win, inv_n_total,
+                                    W_ih, W_ho, dO, g_ho, acc, V, D, reduce, workspace, max_ctas, float2{w0, w1},
+                                    stream);
 }
 
 extern "C" int g2v_cbow_batch_expand(const int32_t *rows, const int32_t *segptr, const int32_t *pos, const float *dO,
@@ -1479,7 +1637,7 @@ extern "C" int g2v_cbow_eval_certified(const int32_t *rowptr, const int32_t *gen
         DeviceProps dp;
         if (device_props(&dp)) return 1;
         cudaFuncAttributes fa;
-        G2V_CUDA_OK(cudaFuncGetAttributes(&fa, cbow_rows_generic_kernel<false>));
+        G2V_CUDA_OK(cudaFuncGetAttributes(&fa, cbow_rows_generic_kernel<false, false>));
         G2V_REQUIRE((size_t)kCbowWarps * 2 * D * sizeof(float) + fa.sharedSizeBytes <= (size_t)dp.max_smem_optin,
                     "sizeHiddenlayer %d too large for the generic kernel", D);
         G2V_CUDA_OK(cudaFuncSetAttribute(cbow_eval_certified_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,

@@ -41,6 +41,19 @@ __device__ __forceinline__ void decay4(float4 &w, float wd) {
 // weight_decay as the *_wd entry points admit it: finite, 0 <= wd < 1 (NaN fails both comparisons)
 inline bool weight_decay_ok(float wd) { return wd >= 0.f && wd < 1.f; }
 
+// Class weights of the training loss (DESIGN.md §4.20): a window of label y counts with weight w_y, cw = {w0, w1}.
+// Applied to fl(fl(sigmoid(o) - y) * inv_n) and to the window's loss term, each product rounded on its own (never
+// one FMA), so cw = {1, 1} gives the unweighted bits.  CW = false is the unweighted kernel; cw is then unused.
+template <bool CW>
+__device__ __forceinline__ float class_weighted(float x, float y, float2 cw) {
+    return CW ? __fmul_rn(x, y != 0.f ? cw.y : cw.x) : x;
+}
+// a class weight as the *_cw entry points admit it: finite and > 0 (NaN fails both comparisons)
+inline bool class_weight_ok(float w) { return w > 0.f && w <= 0x1.fffffep127f; }
+#define G2V_CW_CHECK(name)                                                                                             \
+    G2V_REQUIRE(class_weight_ok(w0) && class_weight_ok(w1), name ": class weights must be finite and > 0 (w0=%g w1=%g)", \
+                (double)w0, (double)w1)
+
 // alpha of step t >= 1, with beta^t by repeated float32 multiplication, as TF1's beta1_power / beta2_power variables
 inline float adam_tf1_alpha(float lr, float beta1, float beta2, int32_t t) {
     float b1p = 1.f, b2p = 1.f;

@@ -71,13 +71,14 @@ r1_prepare_kernel(const float *__restrict__ W_ih, const float *__restrict__ W_ho
 // ---- per-window forward (+ backward into c) -------------------------------------------------------
 // MODE 0: accuracy only.  MODE 1: backward with c[gene] += dO (scalar red).  MODE 2: backward that only
 // stores dO[i] for list position i; c is then formed without atomics by r1_csc_reduce_kernel.
-template <int MODE>
+// CW (backward): the class-weighted dO and loss (class_weighted, DESIGN.md §4.20) with weights cw.
+template <int MODE, bool CW>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 r1_windows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
                   const uint8_t *__restrict__ label, const int32_t *__restrict__ win, int64_t win_begin,
                   int64_t n_win, float inv_n, const float *__restrict__ s, float *__restrict__ c,
                   double *__restrict__ loss_sum, unsigned long long *__restrict__ n_correct,
-                  int32_t reduce_mean, const int32_t *__restrict__ skip) {
+                  int32_t reduce_mean, const int32_t *__restrict__ skip, float2 cw) {
     G2V_SKIP_IF_STOPPED(skip);
     constexpr bool BACKWARD = MODE != 0;
     __shared__ CtaAcc sh;
@@ -109,8 +110,8 @@ r1_windows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict_
         if (active && sub == 0) {                        // one lane per window does the scalar math
             correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
             if (BACKWARD) {
-                loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
-                dO = (sigmoid_stable(o) - y) * inv_n * scale;
+                loss_acc += class_weighted<CW>(fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o))), y, cw);
+                dO = class_weighted<CW>((sigmoid_stable(o) - y) * inv_n, y, cw) * scale;
                 if (MODE == 2) c[i] = dO;                // c is the dO array here
             }
         }
@@ -302,28 +303,73 @@ extern "C" int g2v_cbow_r1_prepare(const float *W_ih, const float *W_ho, float *
     return launch_r1_prepare(W_ih, W_ho, s, V, D, false, (cudaStream_t)stream);
 }
 
-extern "C" int g2v_cbow_r1_windows(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
-                                   const int32_t *win, int64_t win_begin, int64_t n_win, float inv_n_total,
-                                   const float *s, float *c, double *loss_sum, int64_t *n_correct, int32_t V,
-                                   int32_t reduce, void *stream) {
-    G2V_REQUIRE(V > 0 && n_win >= 0 && win_begin >= 0, "g2v_cbow_r1_windows: bad sizes");
-    G2V_REQUIRE(rowptr && label && s, "g2v_cbow_r1_windows: null pointer");
-    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "g2v_cbow_r1_windows: unknown reduce %d", reduce);
+// One body for the plain and the class-weighted (_cw, DESIGN.md §4.20) forms; `name` is the entry point's, for errors.
+// c == NULL: the accuracy pass, which has no class weights.
+template <bool CW>
+static int r1_windows_impl(const char *name, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                           const int32_t *win, int64_t win_begin, int64_t n_win, float inv_n_total, const float *s,
+                           float *c, double *loss_sum, int64_t *n_correct, int32_t V, int32_t reduce, float2 cw,
+                           void *stream) {
+    G2V_REQUIRE(V > 0 && n_win >= 0 && win_begin >= 0, "%s: bad sizes", name);
+    G2V_REQUIRE(rowptr && label && s, "%s: null pointer", name);
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "%s: unknown reduce %d", name, reduce);
     if (n_win == 0) return 0;
     unsigned long long *nc = reinterpret_cast<unsigned long long *>(n_correct);
     int grid = 0, rc;
     cudaStream_t st = (cudaStream_t)stream;
     if (c) {
-        if ((rc = rows_grid((const void *)r1_windows_kernel<1>, 0, (n_win + 3) / 4, &grid))) return rc;
-        r1_windows_kernel<1><<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, win_begin, n_win,
-                                                              inv_n_total, s, c, loss_sum, nc, reduce, loop_skip_flag());
+        if ((rc = rows_grid((const void *)r1_windows_kernel<1, CW>, 0, (n_win + 3) / 4, &grid))) return rc;
+        r1_windows_kernel<1, CW><<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, win_begin, n_win,
+                                                                  inv_n_total, s, c, loss_sum, nc, reduce,
+                                                                  loop_skip_flag(), cw);
     } else {
-        if ((rc = rows_grid((const void *)r1_windows_kernel<0>, 0, (n_win + 3) / 4, &grid))) return rc;
-        r1_windows_kernel<0><<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, win_begin, n_win, 0.f,
-                                                              s, nullptr, nullptr, nc, reduce, loop_skip_flag());
+        if ((rc = rows_grid((const void *)r1_windows_kernel<0, false>, 0, (n_win + 3) / 4, &grid))) return rc;
+        r1_windows_kernel<0, false><<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, win_begin, n_win, 0.f,
+                                                                     s, nullptr, nullptr, nc, reduce, loop_skip_flag(),
+                                                                     cw);
     }
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_r1_windows(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                   const int32_t *win, int64_t win_begin, int64_t n_win, float inv_n_total,
+                                   const float *s, float *c, double *loss_sum, int64_t *n_correct, int32_t V,
+                                   int32_t reduce, void *stream) {
+    return r1_windows_impl<false>("g2v_cbow_r1_windows", rowptr, gene, label, win, win_begin, n_win, inv_n_total, s, c,
+                                  loss_sum, n_correct, V, reduce, float2{1.f, 1.f}, stream);
+}
+
+extern "C" int g2v_cbow_r1_windows_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                      const int32_t *win, int64_t win_begin, int64_t n_win, float inv_n_total,
+                                      const float *s, float *c, double *loss_sum, int64_t *n_correct, int32_t V,
+                                      int32_t reduce, float w0, float w1, void *stream) {
+    G2V_CW_CHECK("g2v_cbow_r1_windows_cw");
+    return r1_windows_impl<true>("g2v_cbow_r1_windows_cw", rowptr, gene, label, win, win_begin, n_win, inv_n_total, s,
+                                 c, loss_sum, n_correct, V, reduce, float2{w0, w1}, stream);
+}
+
+template <bool CW>
+static int r1_windows_csc_impl(const char *name, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                               const int32_t *win, int64_t n_win, float inv_n_total, const float *s,
+                               const int32_t *cscptr, const int32_t *csc_pos, float *dO, float *c, double *loss_sum,
+                               int64_t *n_correct, int32_t V, int32_t reduce, float2 cw, void *stream) {
+    G2V_REQUIRE(V > 0 && n_win >= 0, "%s: bad sizes", name);
+    G2V_REQUIRE(rowptr && label && s && cscptr && dO && c, "%s: null pointer", name);
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "%s: unknown reduce %d", name, reduce);
+    if (n_win == 0) return 0;
+    unsigned long long *nc = reinterpret_cast<unsigned long long *>(n_correct);
+    int grid = 0, rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = rows_grid((const void *)r1_windows_kernel<2, CW>, 0, (n_win + 3) / 4, &grid))) return rc;
+    r1_windows_kernel<2, CW><<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, 0, n_win, inv_n_total, s, dO,
+                                                              loss_sum, nc, reduce, loop_skip_flag(), cw);
+    G2V_CUDA_OK(cudaGetLastError());
+    if ((rc = rows_grid((const void *)r1_csc_reduce_kernel, 0, V, &grid))) return rc;
+    r1_csc_reduce_kernel<<<grid, kCbowWarps * 32, 0, st>>>(cscptr, csc_pos, dO, c, V, loop_skip_flag());
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch(2);
     return 0;
 }
 
@@ -332,22 +378,18 @@ extern "C" int g2v_cbow_r1_windows_csc(const int32_t *rowptr, const int32_t *gen
                                        const int32_t *cscptr, const int32_t *csc_pos, float *dO, float *c,
                                        double *loss_sum, int64_t *n_correct, int32_t V, int32_t reduce,
                                        void *stream) {
-    G2V_REQUIRE(V > 0 && n_win >= 0, "g2v_cbow_r1_windows_csc: bad sizes");
-    G2V_REQUIRE(rowptr && label && s && cscptr && dO && c, "g2v_cbow_r1_windows_csc: null pointer");
-    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "g2v_cbow_r1_windows_csc: unknown reduce %d", reduce);
-    if (n_win == 0) return 0;
-    unsigned long long *nc = reinterpret_cast<unsigned long long *>(n_correct);
-    int grid = 0, rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    if ((rc = rows_grid((const void *)r1_windows_kernel<2>, 0, (n_win + 3) / 4, &grid))) return rc;
-    r1_windows_kernel<2><<<grid, kCbowWarps * 32, 0, st>>>(rowptr, gene, label, win, 0, n_win, inv_n_total, s, dO,
-                                                          loss_sum, nc, reduce, loop_skip_flag());
-    G2V_CUDA_OK(cudaGetLastError());
-    if ((rc = rows_grid((const void *)r1_csc_reduce_kernel, 0, V, &grid))) return rc;
-    r1_csc_reduce_kernel<<<grid, kCbowWarps * 32, 0, st>>>(cscptr, csc_pos, dO, c, V, loop_skip_flag());
-    G2V_CUDA_OK(cudaGetLastError());
-    count_launch(2);
-    return 0;
+    return r1_windows_csc_impl<false>("g2v_cbow_r1_windows_csc", rowptr, gene, label, win, n_win, inv_n_total, s,
+                                      cscptr, csc_pos, dO, c, loss_sum, n_correct, V, reduce, float2{1.f, 1.f}, stream);
+}
+
+extern "C" int g2v_cbow_r1_windows_csc_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                          const int32_t *win, int64_t n_win, float inv_n_total, const float *s,
+                                          const int32_t *cscptr, const int32_t *csc_pos, float *dO, float *c,
+                                          double *loss_sum, int64_t *n_correct, int32_t V, int32_t reduce, float w0,
+                                          float w1, void *stream) {
+    G2V_CW_CHECK("g2v_cbow_r1_windows_csc_cw");
+    return r1_windows_csc_impl<true>("g2v_cbow_r1_windows_csc_cw", rowptr, gene, label, win, n_win, inv_n_total, s,
+                                     cscptr, csc_pos, dO, c, loss_sum, n_correct, V, reduce, float2{w0, w1}, stream);
 }
 
 constexpr int kR1MaxParts = 1024;   // upper bound on the update kernel's grid (scratch = kR1MaxParts * D floats)

@@ -57,7 +57,8 @@ slab_setup_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict_
 
 // MODE 0: training forward (hbuf carries the partial context sum; LAST computes dO and g_ho)
 // MODE 1: accuracy pass (obuf carries the partial logit; LAST counts correct predictions)
-template <int VEC, int MODE, bool FIRST, bool LAST>
+// CW (MODE 0, LAST): the class-weighted dO and loss (class_weighted, DESIGN.md §4.20) with weights cw.
+template <int VEC, int MODE, bool FIRST, bool LAST, bool CW>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 cbow_slab_fwd_kernel(const int32_t *__restrict__ gene, const uint8_t *__restrict__ label,
                      const int32_t *__restrict__ win, int64_t win_begin, int64_t n_win,
@@ -65,7 +66,7 @@ cbow_slab_fwd_kernel(const int32_t *__restrict__ gene, const uint8_t *__restrict
                      const float *__restrict__ W_ih, const float *__restrict__ W_ho, float *__restrict__ hbuf,
                      float *__restrict__ obuf, float *__restrict__ dOut, float *__restrict__ g_ho,
                      double *__restrict__ loss_sum, unsigned long long *__restrict__ n_correct, int32_t reduce_mean,
-                     const int32_t *__restrict__ skip) {
+                     const int32_t *__restrict__ skip, float2 cw) {
     G2V_SKIP_IF_STOPPED(skip);
     constexpr int D = 128 * VEC;
     constexpr int D4 = D / 4;
@@ -142,10 +143,10 @@ cbow_slab_fwd_kernel(const int32_t *__restrict__ gene, const uint8_t *__restrict
         const float y = (float)__ldg(label + n);
         if (lane == 0) {
             correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
-            if (TRAIN) loss_acc += fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o)));
+            if (TRAIN) loss_acc += class_weighted<CW>(fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o))), y, cw);
         }
         if (TRAIN) {
-            const float dO = (sigmoid_stable(o) - y) * inv_n;
+            const float dO = class_weighted<CW>((sigmoid_stable(o) - y) * inv_n, y, cw);
             const float hs = dO * scale;                          // d cost / d (sum of rows)
 #pragma unroll
             for (int v = 0; v < VEC; ++v) {
@@ -216,11 +217,13 @@ static int fwd_group() {       // forward slab group = this many backward slabs 
     return g >= 1 ? g : 1;
 }
 
-template <int VEC, int MODE>
+// CW: the last training pass is the class-weighted one, with weights cw (the passes before it form no dO).
+template <int VEC, int MODE, bool CW = false>
 static int launch_fwd_passes(const int32_t *gene, const uint8_t *label, const int32_t *win, int64_t win_begin,
                              int64_t n_win, const SlabLayout &l, int32_t S, float inv_n, const float *W_ih,
                              const float *W_ho, float *g_ho, double *loss_sum, unsigned long long *nc, int32_t reduce,
-                             cudaStream_t st) {
+                             cudaStream_t st, float2 cw = float2{1.f, 1.f}) {
+    static_assert(MODE == 0 || !CW, "the accuracy pass has no class weights");
     const int G = fwd_group();
     const int passes = (S + G - 1) / G;
     for (int j = 0; j < passes; ++j) {
@@ -229,10 +232,11 @@ static int launch_fwd_passes(const int32_t *gene, const uint8_t *label, const in
         int grid = 0, rc;
 #define G2V_SLAB_FWD(F, L)                                                                                 \
     {                                                                                                      \
-        auto kern = cbow_slab_fwd_kernel<VEC, MODE, F, L>;                                                 \
+        auto kern = cbow_slab_fwd_kernel<VEC, MODE, F, L, CW && L>;                                        \
         if ((rc = rows_grid((const void *)kern, 0, n_win, &grid))) return rc;                              \
         kern<<<grid, kCbowWarps * 32, 0, st>>>(gene, label, win, win_begin, n_win, l.slabptr, S + 1, lo, hi, inv_n, \
-                                               W_ih, W_ho, l.hbuf, l.obuf, l.dO, g_ho, loss_sum, nc, reduce, loop_skip_flag()); \
+                                               W_ih, W_ho, l.hbuf, l.obuf, l.dO, g_ho, loss_sum, nc, reduce, loop_skip_flag(), \
+                                               cw);                                                        \
     }
         if (first && last) G2V_SLAB_FWD(true, true)
         else if (first) G2V_SLAB_FWD(true, false)
@@ -323,14 +327,16 @@ extern "C" int g2v_cbow_slab_setup(const int32_t *rowptr, const int32_t *gene, c
     return 0;
 }
 
-extern "C" int g2v_cbow_fwdbwd_slabs(const int32_t *gene, const uint8_t *label, const int32_t *win, int64_t win_begin,
-                                     int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
-                                     float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
-                                     int32_t D, int32_t reduce, int32_t n_slabs, void *workspace, void *stream) {
-    G2V_REQUIRE(V > 0 && n_win >= 0 && n_slabs >= 1, "g2v_cbow_fwdbwd_slabs: bad sizes");
-    G2V_REQUIRE(D == 128 || D == 256 || D == 512, "g2v_cbow_fwdbwd_slabs: sizeHiddenlayer must be 128, 256 or 512 (got %d)", D);
-    G2V_REQUIRE(gene && label && W_ih && W_ho && g_ih && g_ho && workspace, "g2v_cbow_fwdbwd_slabs: null pointer");
-    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "g2v_cbow_fwdbwd_slabs: unknown reduce %d", reduce);
+// One body for the plain and the class-weighted (_cw, DESIGN.md §4.20) step; `name` is the entry point's, for errors.
+template <bool CW>
+static int fwdbwd_slabs_impl(const char *name, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                             int64_t win_begin, int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
+                             float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V, int32_t D,
+                             int32_t reduce, int32_t n_slabs, void *workspace, float2 cw, void *stream) {
+    G2V_REQUIRE(V > 0 && n_win >= 0 && n_slabs >= 1, "%s: bad sizes", name);
+    G2V_REQUIRE(D == 128 || D == 256 || D == 512, "%s: sizeHiddenlayer must be 128, 256 or 512 (got %d)", name, D);
+    G2V_REQUIRE(gene && label && W_ih && W_ho && g_ih && g_ho && workspace, "%s: null pointer", name);
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "%s: unknown reduce %d", name, reduce);
     if (n_win == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
     SlabLayout l = carve(workspace, n_win, n_slabs);
@@ -338,8 +344,8 @@ extern "C" int g2v_cbow_fwdbwd_slabs(const int32_t *gene, const uint8_t *label, 
     int rc;
 #define G2V_SLAB_STEP(VEC)                                                                                          \
     {                                                                                                               \
-        if ((rc = launch_fwd_passes<VEC, 0>(gene, label, win, win_begin, n_win, l, n_slabs, inv_n_total, W_ih, W_ho, \
-                                            g_ho, loss_sum, nc, reduce, st))) return rc;                             \
+        if ((rc = launch_fwd_passes<VEC, 0, CW>(gene, label, win, win_begin, n_win, l, n_slabs, inv_n_total, W_ih,  \
+                                                W_ho, g_ho, loss_sum, nc, reduce, st, cw))) return rc;              \
         if ((rc = launch_bwd_passes<VEC>(gene, n_win, l, n_slabs, W_ho, g_ih, st))) return rc;                       \
     }
     if (D == 128) G2V_SLAB_STEP(1)
@@ -347,6 +353,26 @@ extern "C" int g2v_cbow_fwdbwd_slabs(const int32_t *gene, const uint8_t *label, 
     else G2V_SLAB_STEP(4)
 #undef G2V_SLAB_STEP
     return 0;
+}
+
+extern "C" int g2v_cbow_fwdbwd_slabs(const int32_t *gene, const uint8_t *label, const int32_t *win, int64_t win_begin,
+                                     int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
+                                     float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V,
+                                     int32_t D, int32_t reduce, int32_t n_slabs, void *workspace, void *stream) {
+    return fwdbwd_slabs_impl<false>("g2v_cbow_fwdbwd_slabs", gene, label, win, win_begin, n_win, inv_n_total, W_ih,
+                                    W_ho, g_ih, g_ho, loss_sum, n_correct, V, D, reduce, n_slabs, workspace,
+                                    float2{1.f, 1.f}, stream);
+}
+
+extern "C" int g2v_cbow_fwdbwd_slabs_cw(const int32_t *gene, const uint8_t *label, const int32_t *win,
+                                        int64_t win_begin, int64_t n_win, float inv_n_total, const float *W_ih,
+                                        const float *W_ho, float *g_ih, float *g_ho, double *loss_sum,
+                                        int64_t *n_correct, int32_t V, int32_t D, int32_t reduce, int32_t n_slabs,
+                                        void *workspace, float w0, float w1, void *stream) {
+    G2V_CW_CHECK("g2v_cbow_fwdbwd_slabs_cw");
+    return fwdbwd_slabs_impl<true>("g2v_cbow_fwdbwd_slabs_cw", gene, label, win, win_begin, n_win, inv_n_total, W_ih,
+                                   W_ho, g_ih, g_ho, loss_sum, n_correct, V, D, reduce, n_slabs, workspace,
+                                   float2{w0, w1}, stream);
 }
 
 extern "C" int g2v_cbow_eval_slabs(const int32_t *gene, const uint8_t *label, const int32_t *win, int64_t win_begin,

@@ -238,6 +238,58 @@ int g2v_cbow_r1_update_wd(float *W_ih, float *W_ho, float *m_ih, float *v_ih, fl
                           float lr, float beta1, float beta2, float eps, float weight_decay, int32_t t,
                           const float *alpha_dev, void *stream);
 
+/* Class weights of the training loss (DESIGN.md §4.20; Keras fit(class_weight=...)): the *_cw entry points take the
+ * arguments of their counterparts plus the weights w0, w1 (labels 0 and 1) before the stream.  A window of label y
+ * forms
+ *     dO = fl(fl(fl(sigmoid(o) - y) * inv_n_total) * w_y)
+ * (then the counterpart's * scale and everything after it, unchanged) and adds fl(w_y * l) to *loss_sum instead of
+ * its BCE term l.  The correct count is not weighted.  With w0 = w1 = 1 both products are exact, so a *_cw call gives
+ * the bits of its counterpart (on the fixed-order routes; the atomic ones reorder as their counterparts do).  The
+ * weights must be finite and > 0, else the call fails with g2v_last_error() set and nothing launched.  The launches
+ * are the counterpart's, with the class-weighted instantiations of the kernels that form dO. */
+int g2v_cbow_fwdbwd_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                       int64_t win_begin, int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
+                       float *g_ih, float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V, int32_t D,
+                       int32_t reduce, float w0, float w1, void *stream);
+int g2v_cbow_fwdbwd_csc_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                           int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
+                           const int32_t *cscptr, const int32_t *csc_pos, float *dO, float *g_ih, float *g_ho,
+                           double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce, float w0,
+                           float w1, void *stream);
+int g2v_cbow_fwd_do_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                       int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho, float *dO, float *g_ho,
+                       double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce, float w0, float w1,
+                       void *stream);
+int g2v_cbow_fwdbwd_csc_det_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                               int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
+                               const int32_t *cscptr, const int32_t *csc_pos, float *dO, float *g_ih, float *g_ho,
+                               double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce,
+                               void *workspace, int32_t max_ctas, float w0, float w1, void *stream);
+int g2v_cbow_fwd_do_det_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                           int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho, float *dO,
+                           float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce,
+                           void *workspace, int32_t max_ctas, float w0, float w1, void *stream);
+int g2v_cbow_loop_tail_cw(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                          const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
+                          float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D, int32_t reduce, float w0,
+                          float w1, void *stream);
+int g2v_cbow_loop_tail_det_cw(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                              const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
+                              const float *W_ho, float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D,
+                              int32_t reduce, void *workspace, int32_t max_ctas, float w0, float w1, void *stream);
+int g2v_cbow_fwdbwd_slabs_cw(const int32_t *gene, const uint8_t *label, const int32_t *win, int64_t win_begin,
+                             int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho, float *g_ih,
+                             float *g_ho, double *loss_sum, int64_t *n_correct, int32_t V, int32_t D, int32_t reduce,
+                             int32_t n_slabs, void *workspace, float w0, float w1, void *stream);
+int g2v_cbow_r1_windows_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                           int64_t win_begin, int64_t n_win, float inv_n_total, const float *s, float *c,
+                           double *loss_sum, int64_t *n_correct, int32_t V, int32_t reduce, float w0, float w1,
+                           void *stream);
+int g2v_cbow_r1_windows_csc_cw(const int32_t *rowptr, const int32_t *gene, const uint8_t *label, const int32_t *win,
+                               int64_t n_win, float inv_n_total, const float *s, const int32_t *cscptr,
+                               const int32_t *csc_pos, float *dO, float *c, double *loss_sum, int64_t *n_correct,
+                               int32_t V, int32_t reduce, float w0, float w1, void *stream);
+
 /* Multi-GPU optimizer epilogue fused with the gradient exchange (one process per GPU, one node): replaces
  * ncclAllReduce(gradient) + g2v_cbow_update.  All buffers are flat [W_ih (V*D) | W_ho (D)] = n floats, the gradient
  * and the parameters in symmetric memory (same size on every rank, peer-mapped): g_ptrs_dev / w_ptrs_dev are DEVICE
