@@ -27,6 +27,12 @@ SIGNATURES = {
     "g2v_walk_launch_packed": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i64, _i32, _u64, _u32, _i64, _i64, _i64,
                                               _vp, _vp, _vp, _vp, _vp]),
     "g2v_walk_host": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i64, _i32, _u64, _u32, _i64, _i64, _i64, _vp, _vp]),
+    "g2v_walk_launch_biased": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i64, _i32, _u64, _u32, _i64, _i64, _i64,
+                                              _vp, _vp, _u32, _u32, _vp, _vp]),
+    "g2v_walk_launch_packed_biased": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i64, _i32, _u64, _u32, _i64, _i64, _i64,
+                                                     _vp, _vp, _vp, _u32, _u32, _vp, _vp]),
+    "g2v_walk_host_biased": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i64, _i32, _u64, _u32, _i64, _i64, _i64, _vp, _vp,
+                                            _u32, _u32]),
     "g2v_cbow_fwdbwd": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp,
                                        _i32, _i32, _i32, _vp]),
     "g2v_cbow_fwdbwd_csc": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,

@@ -69,6 +69,10 @@ def parse_arguments(argv=None):
     p.add_argument('-l', '--learningRate', type=float, default=0.005, help='')
     p.add_argument('-n', '--numBiomarker', type=int, default=50, help='')
     p.add_argument('--seed', type=int, default=0, help='seed of the walk sampler, the split and the init')
+    p.add_argument('--walk-q', type=float, default=1.0, metavar='Q',
+                   help="node2vec's in-out parameter of the random walks, in [1/256, 256]: Q > 1 keeps a walk near the "
+                        "previous gene's neighbours (BFS-like), Q < 1 moves it away (DFS-like); 1 (default) = the "
+                        "reference's first-order walk.  There is no return parameter: the walks never revisit a gene")
     p.add_argument('--algo', choices=['rows', 'rank1'], default='rows',
                    help="CBOW kernels: 'rows' = embedding-row gather/scatter (default), 'rank1' = collapsed, "
                         "bit-reproducible trainer; same results to fp32 rounding")
@@ -105,6 +109,8 @@ def parse_arguments(argv=None):
                    help="weights of the label-0 and label-1 windows in the training loss: 'balanced' = n / (2 n_y) "
                         "from the training windows, or two finite numbers > 0; default off")
     args = p.parse_args(argv)
+    if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
+        p.error("--walk-q must be a finite number in [1/256, 256]")
     if args.class_weight is not None:
         args.class_weight = _parse_class_weight(args.class_weight, p)
     if not 0.0 <= float(np.float32(args.weight_decay)) < 1.0:
@@ -301,6 +307,10 @@ def main(argv=None):
     print('>>> 3. Generate random paths from each group')
     print('    *** most time consuming step ***')
     from . import graph, paths, walks, cbow           # needs the GPU from here on
+    if args.walk_q != 1.0:
+        a_near, a_far = walks.walk_bias(args.walk_q)
+        print('    walk q  : %g\t(in-out multipliers %d near, %d far: effective q = %.6g)'
+              % (args.walk_q, a_near, a_far, walks.effective_q(args.walk_q)))
     idx = {g: i for i, g in enumerate(data['gene'])}
     src = np.fromiter((idx[e[0]] for e in network['edge']), dtype=np.int32, count=len(network['edge']))
     dst = np.fromiter((idx[e[1]] for e in network['edge']), dtype=np.int32, count=len(network['edge']))
@@ -318,13 +328,13 @@ def main(argv=None):
         if dist is None:
             # tuple(sorted(path)) is fused into the sampler: sorted rows + their 64-bit keys come back
             walks.generate_paths(wg, L, args.numRepetition, seed=args.seed, group=i, canonical=True,
-                                 out=(rows[sl], lens[sl], key[sl]))
+                                 out=(rows[sl], lens[sl], key[sl]), q=args.walk_q)
         else:
             # walkers rank, rank+world, ...: no collective during the walk (counter-based RNG); one all_gather after,
             # rows put back at their walker index so that every rank holds the 1-GPU arrays (same window order,
             # hence the same --seed split, whatever the number of GPUs)
             r_, l_, k_ = walks.generate_paths(wg, L, args.numRepetition, seed=args.seed, group=i, canonical=True,
-                                              walker_begin=rank, walker_stride=world)
+                                              walker_begin=rank, walker_stride=world, q=args.walk_q)
             rows[sl], lens[sl], key[sl] = paths.gather_walker_shards(dist, world, n_total, r_, l_, k_)
     group = torch.cat([torch.zeros(n_total, dtype=torch.uint8, device=dev), torch.ones(n_total, dtype=torch.uint8, device=dev)])
     w_rowptr, w_gene, w_label, code = paths.build_windows(rows, lens, key, group, n_genes)

@@ -37,6 +37,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <type_traits>
+
 #include "g2v_common.cuh"
 
 namespace g2v {
@@ -140,12 +142,72 @@ __device__ __forceinline__ void load_chunk(const WalkGraphPtrs &g, int32_t jb, i
 }
 
 // Inclusive warp scan of p; the first lane whose prefix exceeds `rem` holds the chosen neighbour.
-template <int EPL>
-__device__ __forceinline__ int32_t pick_in_chunk(uint32_t p, uint32_t q0, int32_t c0, int32_t c1, uint32_t incl,
-                                                 uint32_t rem) {
+template <int EPL, typename WT>
+__device__ __forceinline__ int32_t pick_in_chunk(WT p, WT q0, int32_t c0, int32_t c1, WT incl, WT rem) {
     const unsigned hit = __ballot_sync(0xffffffffu, incl > rem);
     const int32_t sel = (EPL == 2 && !(incl - p + q0 > rem)) ? c1 : c0;
     return __shfl_sync(0xffffffffu, sel, __ffs(hit) - 1);
+}
+
+// Chunk sums in the width the weights need: 32 bits for the unbiased walk (qw <= 2^24, 64 per chunk) and for biased
+// packed 16+16-bit edges (qw * a <= 2^24); 64 bits for biased plain CSR / {col, qw} pairs, where one weight reaches 2^32.
+__device__ __forceinline__ uint32_t warp_scan_w(uint32_t v, int lane) { return warp_inclusive_scan_u32(v, lane); }
+__device__ __forceinline__ unsigned long long warp_scan_w(unsigned long long v, int lane) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long t = __shfl_up_sync(0xffffffffu, v, o);
+        if (lane >= o) v += t;
+    }
+    return v;
+}
+__device__ __forceinline__ uint32_t warp_total_w(uint32_t v) { return __reduce_add_sync(0xffffffffu, v); }
+__device__ __forceinline__ unsigned long long warp_total_w(unsigned long long v) { return warp_sum_u64(v); }
+// r = floor(x*T / 2^64) for the 64-bit draw x = xhi:xlo.  T < 2^32: two 32x32 multiplies instead of a 64x64 high multiply
+__device__ __forceinline__ uint32_t draw_below(uint32_t xlo, uint32_t xhi, uint32_t T) {
+    const unsigned long long lo = (unsigned long long)xlo * T;
+    return (uint32_t)(((unsigned long long)xhi * T + (lo >> 32)) >> 32);
+}
+__device__ __forceinline__ unsigned long long draw_below(uint32_t xlo, uint32_t xhi, unsigned long long T) {
+    return __umul64hi(((unsigned long long)xhi << 32) | xlo, T);
+}
+
+// ---- node2vec's in-out bias (walk_bias_kernel) ----------------------------------------------------------------
+// A candidate x of the walker at v with previous node t weighs qw * a_near if x is in row(t) (distance 1 from t) and
+// qw * a_far otherwise.  Step 0 has no previous node: Bias{0, 0, 1, 1} (an empty row, multiplier 1) leaves the
+// weights unbiased.
+struct Bias {
+    int32_t pb, pe;       // the previous node's row [pb, pe) in the layout's edge array
+    uint32_t an, af;      // a_near, a_far
+};
+
+template <int LAYOUT>
+__device__ __forceinline__ int32_t col_at(const WalkGraphPtrs &g, int32_t j) {
+    if (LAYOUT == LAY_E4) return (int32_t)(__ldg(reinterpret_cast<const uint32_t *>(g.edges) + j) & 0xffffu);
+    if (LAYOUT == LAY_E8) return __ldg(reinterpret_cast<const int32_t *>(g.edges) + 2 * (size_t)j);
+    return __ldg(reinterpret_cast<const int32_t *>(g.edges) + j);
+}
+
+// x in the ascending row [pb, pe)?  Binary search bounded by the row's true end, so that the packed layouts' {0, 0}
+// pad pairs and sentinel words are never compared (0 is a real node id).
+template <int LAYOUT>
+__device__ __forceinline__ bool in_row(const WalkGraphPtrs &g, int32_t pb, int32_t pe, int32_t x) {
+    int32_t lo = pb, hi = pe;
+    while (lo < hi) {
+        const int32_t mid = (int32_t)(((uint32_t)lo + (uint32_t)hi) >> 1);
+        if (col_at<LAYOUT>(g, mid) < x) lo = mid + 1; else hi = mid;
+    }
+    return lo < pe && col_at<LAYOUT>(g, lo) == x;
+}
+
+// load_chunk, then the bias: masked (visited / outside the row) weights stay 0 and are not searched
+template <int LAYOUT, bool BITMAP, typename WT>
+__device__ __forceinline__ void load_chunk_w(const WalkGraphPtrs &g, const Bias &bz, int32_t jb, int32_t b, int32_t e,
+                                             int lane, int hs, uint32_t hmask, int hshift, uint32_t sent, int32_t &c0,
+                                             int32_t &c1, WT &q0, WT &q1) {
+    uint32_t u0, u1;
+    load_chunk<LAYOUT, BITMAP>(g, jb, b, e, lane, hs, hmask, hshift, sent, c0, c1, u0, u1);
+    q0 = u0 ? (WT)u0 * (WT)(in_row<LAYOUT>(g, bz.pb, bz.pe, c0) ? bz.an : bz.af) : (WT)0;
+    q1 = u1 ? (WT)u1 * (WT)(in_row<LAYOUT>(g, bz.pb, bz.pe, c1) ? bz.an : bz.af) : (WT)0;
 }
 
 template <bool BITMAP, int LAYOUT, bool CANON>
@@ -275,6 +337,216 @@ walk_kernel(const WalkGraphPtrs g, int32_t V, int32_t L, int32_t Lpad, int32_t H
                     }
                 }
             }
+            cur = nxt;
+        }
+
+        // ---------------------------------------------------------------- walk finished: n nodes in smem
+        G2V_WALK_STEP_SYNC();                            // (strict build: lane 0's path stores become visible)
+        int32_t *row = out_nodes + (size_t)t * (size_t)L;
+        if (!CANON) {
+            for (int i = lane; i < L; i += 32) row[i] = (i < n) ? smem[path + i] : -1;     // visit order
+        } else if (BITMAP) {
+            // tuple(sorted(path)) (G2Vec.py:345) read off the visited bitmap: the set bits in index order ARE the
+            // sorted path.  Lane l owns the words [l*B, (l+1)*B): count, one warp scan for its first output
+            // position, then emit its bits in order (and clear the words: the next walker starts from zero).
+            const int32_t lastn = smem[path + n - 1];            // the final node is appended but never inserted
+            G2V_WALK_ONE_WRITER smem[hs + (lastn >> 5)] |= (1 << (lastn & 31));
+            __syncwarp();
+            const int B = (H + 31) >> 5, w0 = lane * B, w1 = min(H, w0 + B);
+            uint32_t cnt = 0;
+            for (int wi = w0; wi < w1; ++wi) cnt += __popc((uint32_t)smem[hs + wi] & ~(uint32_t)((SENT && wi == sw) ? sbit : 0));
+            uint32_t pos = warp_inclusive_scan_u32(cnt, lane) - cnt;
+            uint64_t h = 0;
+            for (int wi = w0; wi < w1; ++wi) {
+                const int32_t keepbit = (SENT && wi == sw) ? sbit : 0;
+                uint32_t bits = (uint32_t)smem[hs + wi] & ~(uint32_t)keepbit;
+                if (bits) smem[hs + wi] = keepbit;
+                while (bits) {
+                    const int32_t v = wi * 32 + (__ffs(bits) - 1);
+                    bits &= bits - 1;
+                    row[pos] = v;
+                    h += path_key_term(v, (int)pos);
+                    ++pos;
+                }
+            }
+            for (int i = n + lane; i < L; i += 32) row[i] = kPathPad;
+            h = warp_sum_u64(h);
+            if (lane == 0) out_key[t] = path_key_finish(h);
+            dirty = false;                                       // already cleared
+        } else {
+            // tuple(sorted(path)) (G2Vec.py:345): bitonic network over the next power of two, INT32_MAX padding
+            int P2 = 1;
+            while (P2 < n) P2 <<= 1;
+            if (n > 1) {
+                for (int i = n + lane; i < P2; i += 32) smem[path + i] = kPathPad;
+                __syncwarp();
+                for (int k = 2; k <= P2; k <<= 1)
+                    for (int j = k >> 1; j > 0; j >>= 1) {
+                        for (int x = lane; x < (P2 >> 1); x += 32) {
+                            const int i = ((x / j) * 2 * j) + (x % j), l = i + j;
+                            const bool up = (i & k) == 0;
+                            const int32_t a = smem[path + i], c = smem[path + l];
+                            if ((a > c) == up) { smem[path + i] = c; smem[path + l] = a; }
+                        }
+                        __syncwarp();
+                    }
+            }
+            uint64_t h = 0;
+            for (int i = lane; i < L; i += 32) {
+                const int32_t v = (i < n) ? smem[path + i] : kPathPad;
+                row[i] = v;
+                if (i < n) h += path_key_term(v, i);
+            }
+            h = warp_sum_u64(h);
+            if (lane == 0) out_key[t] = path_key_finish(h);
+        }
+        if (lane == 0) out_len[t] = n;
+        if (dirty) {
+            if (BITMAP) {                                // every lane resets the words it owns (one writer per word)
+                __syncwarp();
+                const int B = (H + 31) >> 5, w0 = lane * B, w1 = min(H, w0 + B);
+                for (int wi = w0; wi < w1; ++wi)
+                    if (smem[hs + wi] != 0) smem[hs + wi] = (SENT && wi == sw) ? sbit : 0;
+            } else {
+                for (int i = lane; i < H; i += 32) smem[hs + i] = -1;
+            }
+        }
+        __syncwarp();
+    }
+}
+
+// walk_kernel's walk with node2vec's in-out multipliers (a_near, a_far) on every step after the first.  Its own copy of
+// the step loop (walk_kernel's code stays exactly as it was); same launch bounds, so it is compiled under the same
+// register caps.
+template <bool BITMAP, int LAYOUT, bool CANON>
+__global__ void __launch_bounds__(kWalkWarps * 32, BITMAP ? G2V_WALK_MINB_BITMAP : G2V_WALK_MINB_HASH)
+walk_bias_kernel(const WalkGraphPtrs g, int32_t V, int32_t L, int32_t Lpad, int32_t H, int32_t hshift, uint64_t seed,
+                 uint32_t group, int64_t walker_begin, int64_t n_walkers, int64_t walker_stride,
+                 int32_t *__restrict__ out_nodes, int32_t *__restrict__ out_len,
+                 unsigned long long *__restrict__ out_key, unsigned long long *__restrict__ ticket, uint32_t a_near,
+                 uint32_t a_far) {
+    using WT = typename std::conditional<LAYOUT == LAY_E4, uint32_t, unsigned long long>::type;
+    int32_t *const smem = g2v_walk_smem;
+    constexpr int EPL = LAYOUT == LAY_CSR ? 1 : 2;      // neighbours per lane per chunk
+    constexpr int CH = 32 * EPL;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int path = warp * (Lpad + H);                  // offsets into smem (ints), not pointers
+    const int hs = path + Lpad;
+    const uint32_t hmask = (uint32_t)H - 1u;
+
+    constexpr bool SENT = BITMAP && LAYOUT == LAY_E4;   // bit V of the bitmap = a node that is always "visited"
+    const uint32_t sent = (uint32_t)V;                   // sentinel edge word: col = V, weight field 0
+    const int sw = V >> 5;
+    const int32_t sbit = SENT ? (int32_t)(1u << (V & 31)) : 0;
+    for (int i = lane; i < H; i += 32) smem[hs + i] = BITMAP ? ((SENT && i == sw) ? sbit : 0) : -1;
+    __syncwarp();
+
+    while (true) {
+        // ------------------------------------------------------------------ take the next walker
+        unsigned long long t = 0;
+        if (lane == 0) t = atomicAdd(ticket, 1ull);
+        t = __shfl_sync(0xffffffffu, t, 0);
+        if ((int64_t)t >= n_walkers) break;
+        const int64_t w = walker_begin + (int64_t)t * walker_stride;
+        const uint64_t subseq = ((uint64_t)group << 40) + (uint64_t)w;
+        int32_t cur = (int32_t)(w % V);
+        int32_t n = 0;                                   // nodes appended = step index + 1
+        uint32_t dlo = 0, dhi = 0;                       // lane holds the draw of step (s & ~31) + lane
+        bool dirty = false;
+        Bias bz{0, 0, 1u, 1u};                           // step 0: no previous node, unbiased weights
+
+        while (true) {
+            G2V_WALK_ONE_WRITER smem[path + n] = cur;    // read back only after the walk (epilogue)
+            const int32_t s = n++;
+            if (s == L - 1) break;                       // the L-th node is appended, never expanded
+            int32_t b, e;
+            if (LAYOUT == LAY_CSR) {
+                b = __ldg(g.rows + cur); e = __ldg(g.rows + cur + 1);
+            } else {
+                const int2 be = __ldg(reinterpret_cast<const int2 *>(g.rows) + cur);
+                b = be.x; e = be.y;
+            }
+            if (b == e) break;                           // no out-edges: dead end
+            if (BITMAP) {                                // visited.insert(cur)
+                G2V_WALK_ONE_WRITER smem[hs + (cur >> 5)] |= (1 << (cur & 31));
+            } else {
+                uint32_t i = hash_slot(cur, hshift);
+                while (smem[hs + i] >= 0) i = (i + 1) & hmask;
+                __syncwarp();                            // every lane has found the free slot before it is filled
+                G2V_WALK_ONE_WRITER smem[hs + i] = cur;
+            }
+            G2V_WALK_STEP_SYNC();
+            dirty = true;
+            if ((s & 31) == 0) {                         // 32 steps of 64-bit Philox draws at once, one per lane
+                const uint64_t d = draw64(seed, subseq, (uint32_t)(s + lane));
+                dlo = (uint32_t)d; dhi = (uint32_t)(d >> 32);
+            }
+            const uint32_t xlo = __shfl_sync(0xffffffffu, dlo, s & 31), xhi = __shfl_sync(0xffffffffu, dhi, s & 31);
+
+            const int32_t jb0 = b;                       // (packed rows start at even indices)
+            int32_t nxt;
+            if (e - jb0 <= CH) {
+                // ---- short row: one chunk.  One scan gives the total (lane 31) and the prefix sums.
+                int32_t c0, c1; WT q0, q1;
+                load_chunk_w<LAYOUT, BITMAP, WT>(g, bz, jb0, b, e, lane, hs, hmask, hshift, sent, c0, c1, q0, q1);
+                const WT p = q0 + q1;
+                const WT incl = warp_scan_w(p, lane);
+                const WT T = __shfl_sync(0xffffffffu, incl, 31);                  // 32 bits: <= 64 * 2^24 < 2^32
+                if (T == 0) break;                       // every neighbour already visited
+                const WT rem = draw_below(xlo, xhi, T);
+                nxt = pick_in_chunk<EPL>(p, q0, c0, c1, incl, rem);
+            } else {
+                // ---- long row: pass 1 = per-chunk totals (first kKC chunks stay in registers), pass 2 = select
+                WT P[kKC], Q0[kKC], tot[kKC];
+                int32_t C0[kKC], C1[kKC];
+                unsigned long long T = 0;
+#pragma unroll
+                for (int k = 0; k < kKC; ++k) {
+                    P[k] = 0; Q0[k] = 0; tot[k] = 0; C0[k] = 0; C1[k] = 0;
+                    if (jb0 + k * CH < e) {              // warp-uniform
+                        WT q1;
+                        load_chunk_w<LAYOUT, BITMAP, WT>(g, bz, jb0 + k * CH, b, e, lane, hs, hmask, hshift, sent, C0[k], C1[k], Q0[k], q1);
+                        P[k] = Q0[k] + q1;
+                        tot[k] = warp_total_w(P[k]);
+                        T += tot[k];
+                    }
+                }
+                for (int32_t jb = jb0 + kKC * CH; jb < e; jb += CH) {
+                    int32_t c0, c1; WT q0, q1;
+                    load_chunk_w<LAYOUT, BITMAP, WT>(g, bz, jb, b, e, lane, hs, hmask, hshift, sent, c0, c1, q0, q1);
+                    T += warp_total_w(q0 + q1);
+                }
+                if (T == 0) break;
+                unsigned long long rem = __umul64hi(((unsigned long long)xhi << 32) | xlo, T);
+                nxt = -1;
+                bool found = false;
+#pragma unroll
+                for (int k = 0; k < kKC; ++k) {
+                    if (!found && jb0 + k * CH < e) {
+                        if (rem < (unsigned long long)tot[k]) {
+                            const WT incl = warp_scan_w(P[k], lane);
+                            nxt = pick_in_chunk<EPL>(P[k], Q0[k], C0[k], C1[k], incl, (WT)rem);
+                            found = true;
+                        } else {
+                            rem -= tot[k];
+                        }
+                    }
+                }
+                for (int32_t jb = jb0 + kKC * CH; !found && jb < e; jb += CH) {
+                    int32_t c0, c1; WT q0, q1;
+                    load_chunk_w<LAYOUT, BITMAP, WT>(g, bz, jb, b, e, lane, hs, hmask, hshift, sent, c0, c1, q0, q1);
+                    const WT p = q0 + q1;
+                    const WT ct = warp_total_w(p);
+                    if (rem < (unsigned long long)ct) {
+                        const WT incl = warp_scan_w(p, lane);
+                        nxt = pick_in_chunk<EPL>(p, q0, c0, c1, incl, (WT)rem);
+                        found = true;
+                    } else {
+                        rem -= ct;
+                    }
+                }
+            }
+            bz = Bias{b, e, a_near, a_far};              // cur becomes the previous node
             cur = nxt;
         }
 
@@ -624,11 +896,19 @@ __global__ void test_draws_kernel(uint64_t seed, uint64_t subseq, int32_t n, uin
 typedef void (*walk_kern_t)(const WalkGraphPtrs, int32_t, int32_t, int32_t, int32_t, int32_t, uint64_t, uint32_t,
                             int64_t, int64_t, int64_t, int32_t *, int32_t *, unsigned long long *,
                             unsigned long long *);
+typedef void (*walk_bias_kern_t)(const WalkGraphPtrs, int32_t, int32_t, int32_t, int32_t, int32_t, uint64_t, uint32_t,
+                                 int64_t, int64_t, int64_t, int32_t *, int32_t *, unsigned long long *,
+                                 unsigned long long *, uint32_t, uint32_t);
 
+// a_near = a_far = 0: a plain entry point (first-order walk).  Otherwise the in-out multipliers in [1, 256]; equal
+// multipliers scale every weight alike, which picks the same neighbours, so they take the unbiased kernels too unless
+// G2V_WALK_BIAS=kernel forces the biased one.
 static int launch_walk(const WalkGraphPtrs &g, int layout, int32_t V, int64_t E, int32_t L, uint64_t seed,
                        uint32_t group, int64_t walker_begin, int64_t walker_end, int64_t walker_stride,
-                       int32_t *out_nodes, int32_t *out_len, int64_t *out_key, void *workspace, cudaStream_t st,
-                       const char *who) {
+                       int32_t *out_nodes, int32_t *out_len, int64_t *out_key, uint32_t a_near, uint32_t a_far,
+                       void *workspace, cudaStream_t st, const char *who) {
+    G2V_REQUIRE((a_near == 0 && a_far == 0) || (a_near >= 1 && a_near <= 256 && a_far >= 1 && a_far <= 256),
+                "%s: the in-out multipliers must be in [1, 256] (got %u, %u)", who, a_near, a_far);
     G2V_REQUIRE(V > 0 && E >= 0, "%s: V must be > 0 and E >= 0 (V=%d E=%lld)", who, V, (long long)E);
     G2V_REQUIRE(L >= 1 && L <= 4096, "%s: lenPath must be in [1, 4096] (got %d)", who, L);
     G2V_REQUIRE(walker_stride >= 1 && walker_begin >= 0, "%s: bad walker range", who);
@@ -667,6 +947,15 @@ static int launch_walk(const WalkGraphPtrs &g, int layout, int32_t V, int64_t E,
         {{walk_kernel<true, LAY_CSR, false>, walk_kernel<true, LAY_CSR, true>},
          {walk_kernel<true, LAY_E8, false>, walk_kernel<true, LAY_E8, true>},
          {walk_kernel<true, LAY_E4, false>, walk_kernel<true, LAY_E4, true>}}};
+    static const walk_bias_kern_t bias_table[2][3][2] = {
+        {{walk_bias_kernel<false, LAY_CSR, false>, walk_bias_kernel<false, LAY_CSR, true>},
+         {walk_bias_kernel<false, LAY_E8, false>, walk_bias_kernel<false, LAY_E8, true>},
+         {walk_bias_kernel<false, LAY_E4, false>, walk_bias_kernel<false, LAY_E4, true>}},
+        {{walk_bias_kernel<true, LAY_CSR, false>, walk_bias_kernel<true, LAY_CSR, true>},
+         {walk_bias_kernel<true, LAY_E8, false>, walk_bias_kernel<true, LAY_E8, true>},
+         {walk_bias_kernel<true, LAY_E4, false>, walk_bias_kernel<true, LAY_E4, true>}}};
+    const char *fb = getenv("G2V_WALK_BIAS");                    // test / A-B hook: "kernel" = biased kernel at (a, a)
+    const bool bias = a_near != 0 && (a_near != a_far || (fb && fb[0] == 'k'));
     // two walkers per warp (walk_pair_kernel): packed edges + bitmap, and both tiles' bitmaps within the 56 KB budget
     const char *ft = getenv("G2V_WALK_TILE");                    // test / A-B hook: "32" / "16" force one / two walkers per warp
     const size_t pair_smem = 2 * per_warp * (size_t)(Lpad + bm_words);
@@ -678,7 +967,8 @@ static int launch_walk(const WalkGraphPtrs &g, int layout, int32_t V, int64_t E,
 #else
     const bool short_rows = (double)E <= 56.0 * (double)V && (double)E >= 8.0 * (double)V;
 #endif
-    if (layout == LAY_E4 && bitmap && pair_smem <= 56 * 1024 && (ft ? atoi(ft) == 16 : short_rows)) {
+    // (the biased walk has no two-walker form: it takes the one-walker kernel of its layout)
+    if (!bias && layout == LAY_E4 && bitmap && pair_smem <= 56 * 1024 && (ft ? atoi(ft) == 16 : short_rows)) {
         auto pk = canon ? walk_pair_kernel<true> : walk_pair_kernel<false>;
         G2V_CUDA_OK(cudaFuncSetAttribute(pk, cudaFuncAttributeMaxDynamicSharedMemorySize, dp.max_smem_optin));
         G2V_CUDA_OK(cudaFuncSetAttribute(pk, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
@@ -698,20 +988,28 @@ static int launch_walk(const WalkGraphPtrs &g, int layout, int32_t V, int64_t E,
         return 0;
     }
     walk_kern_t kern = table[bitmap][layout][canon];
+    walk_bias_kern_t bkern = bias_table[bitmap][layout][canon];
+    const void *fn = bias ? (const void *)bkern : (const void *)kern;
     // per-device function attributes (set on every call: the process may have switched device)
-    G2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dp.max_smem_optin));
-    G2V_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    G2V_CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, dp.max_smem_optin));
+    G2V_CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     int per_sm = 0;
-    G2V_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kWalkWarps * 32, smem));
+    G2V_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kWalkWarps * 32, smem));
     G2V_REQUIRE(per_sm > 0, "%s: kernel does not fit on an SM", who);
     int64_t grid = (int64_t)dp.sm_count * per_sm;                 // persistent: whole chip resident
     const int64_t need = (n_walkers + kWalkWarps - 1) / kWalkWarps;
     if (grid > need) grid = need;
     G2V_CUDA_OK(cudaMemsetAsync(workspace, 0, sizeof(unsigned long long), st));
-    kern<<<(unsigned)grid, kWalkWarps * 32, smem, st>>>(g, V, L, Lpad, H, hshift, seed, group, walker_begin, n_walkers,
-                                                        walker_stride, out_nodes, out_len,
-                                                        reinterpret_cast<unsigned long long *>(out_key),
-                                                        (unsigned long long *)workspace);
+    if (bias)
+        bkern<<<(unsigned)grid, kWalkWarps * 32, smem, st>>>(g, V, L, Lpad, H, hshift, seed, group, walker_begin,
+                                                             n_walkers, walker_stride, out_nodes, out_len,
+                                                             reinterpret_cast<unsigned long long *>(out_key),
+                                                             (unsigned long long *)workspace, a_near, a_far);
+    else
+        kern<<<(unsigned)grid, kWalkWarps * 32, smem, st>>>(g, V, L, Lpad, H, hshift, seed, group, walker_begin,
+                                                            n_walkers, walker_stride, out_nodes, out_len,
+                                                            reinterpret_cast<unsigned long long *>(out_key),
+                                                            (unsigned long long *)workspace);
     G2V_CUDA_OK(cudaGetLastError());
     count_launch();
     return 0;
@@ -723,14 +1021,37 @@ using namespace g2v;
 
 extern "C" size_t g2v_walk_workspace_bytes(void) { return 256; }
 
+// the biased entry points' multipliers: [1, 256] each (0 is the plain entry points' "no bias")
+#define G2V_REQUIRE_BIAS(who, an, af)                                                                          \
+    G2V_REQUIRE((an) >= 1 && (an) <= 256 && (af) >= 1 && (af) <= 256,                                       \
+                "%s: a_near and a_far must be in [1, 256] (got %u, %u)", who, (unsigned)(an), (unsigned)(af))
+
+static int walk_launch_csr(const int32_t *rowptr, const int32_t *col, const uint32_t *qw, int32_t V, int64_t E,
+                           int32_t L, uint64_t seed, uint32_t group, int64_t walker_begin, int64_t walker_end,
+                           int64_t walker_stride, int32_t *out_nodes, int32_t *out_len, uint32_t a_near,
+                           uint32_t a_far, void *workspace, void *stream, const char *who) {
+    WalkGraphPtrs g{rowptr, col, qw};
+    return launch_walk(g, LAY_CSR, V, E, L, seed, group, walker_begin, walker_end, walker_stride, out_nodes, out_len,
+                       nullptr, a_near, a_far, workspace, (cudaStream_t)stream, who);
+}
+
 extern "C" int g2v_walk_launch(const int32_t *rowptr, const int32_t *col, const uint32_t *qw,
                                int32_t V, int64_t E, int32_t L, uint64_t seed, uint32_t group,
                                int64_t walker_begin, int64_t walker_end, int64_t walker_stride,
                                int32_t *out_nodes, int32_t *out_len, void *workspace,
                                void *stream) {
-    WalkGraphPtrs g{rowptr, col, qw};
-    return launch_walk(g, LAY_CSR, V, E, L, seed, group, walker_begin, walker_end, walker_stride, out_nodes, out_len,
-                       nullptr, workspace, (cudaStream_t)stream, "g2v_walk_launch");
+    return walk_launch_csr(rowptr, col, qw, V, E, L, seed, group, walker_begin, walker_end, walker_stride, out_nodes,
+                           out_len, 0u, 0u, workspace, stream, "g2v_walk_launch");
+}
+
+extern "C" int g2v_walk_launch_biased(const int32_t *rowptr, const int32_t *col, const uint32_t *qw,
+                                      int32_t V, int64_t E, int32_t L, uint64_t seed, uint32_t group,
+                                      int64_t walker_begin, int64_t walker_end, int64_t walker_stride,
+                                      int32_t *out_nodes, int32_t *out_len, uint32_t a_near, uint32_t a_far,
+                                      void *workspace, void *stream) {
+    G2V_REQUIRE_BIAS("g2v_walk_launch_biased", a_near, a_far);
+    return walk_launch_csr(rowptr, col, qw, V, E, L, seed, group, walker_begin, walker_end, walker_stride, out_nodes,
+                           out_len, a_near, a_far, workspace, stream, "g2v_walk_launch_biased");
 }
 
 // 8-byte pairs need 8*(E + one pad pair per odd row); packed 4-byte words 4*(E + up to 3 sentinels per row + overhang)
@@ -788,20 +1109,38 @@ extern "C" int g2v_walk_prepare(const int32_t *rowptr, const int32_t *col, const
     return 0;
 }
 
+static int walk_launch_packed(const void *rows, const void *edges, int32_t layout, int32_t V, int64_t E, int32_t L,
+                              uint64_t seed, uint32_t group, int64_t walker_begin, int64_t walker_end,
+                              int64_t walker_stride, int32_t *out_nodes, int32_t *out_len, int64_t *out_key,
+                              uint32_t a_near, uint32_t a_far, void *workspace, void *stream, const char *who) {
+    G2V_REQUIRE(layout == LAY_E8 || layout == LAY_E4, "%s: layout must come from g2v_walk_prepare", who);
+    WalkGraphPtrs g{reinterpret_cast<const int32_t *>(rows), edges, nullptr};
+    return launch_walk(g, layout, V, E, L, seed, group, walker_begin, walker_end, walker_stride, out_nodes, out_len,
+                       out_key, a_near, a_far, workspace, (cudaStream_t)stream, who);
+}
+
 extern "C" int g2v_walk_launch_packed(const void *rows, const void *edges, int32_t layout, int32_t V, int64_t E,
                                       int32_t L, uint64_t seed, uint32_t group, int64_t walker_begin,
                                       int64_t walker_end, int64_t walker_stride, int32_t *out_nodes, int32_t *out_len,
                                       int64_t *out_key, void *workspace, void *stream) {
-    G2V_REQUIRE(layout == LAY_E8 || layout == LAY_E4, "g2v_walk_launch_packed: layout must come from g2v_walk_prepare");
-    WalkGraphPtrs g{reinterpret_cast<const int32_t *>(rows), edges, nullptr};
-    return launch_walk(g, layout, V, E, L, seed, group, walker_begin, walker_end, walker_stride, out_nodes, out_len,
-                       out_key, workspace, (cudaStream_t)stream, "g2v_walk_launch_packed");
+    return walk_launch_packed(rows, edges, layout, V, E, L, seed, group, walker_begin, walker_end, walker_stride,
+                              out_nodes, out_len, out_key, 0u, 0u, workspace, stream, "g2v_walk_launch_packed");
 }
 
-extern "C" int g2v_walk_host(const int32_t *rowptr, const int32_t *col, const uint32_t *qw,
-                             int32_t V, int64_t E, int32_t L, uint64_t seed, uint32_t group,
-                             int64_t walker_begin, int64_t walker_end, int64_t walker_stride,
-                             int32_t *out_nodes, int32_t *out_len) {
+extern "C" int g2v_walk_launch_packed_biased(const void *rows, const void *edges, int32_t layout, int32_t V,
+                                             int64_t E, int32_t L, uint64_t seed, uint32_t group,
+                                             int64_t walker_begin, int64_t walker_end, int64_t walker_stride,
+                                             int32_t *out_nodes, int32_t *out_len, int64_t *out_key, uint32_t a_near,
+                                             uint32_t a_far, void *workspace, void *stream) {
+    G2V_REQUIRE_BIAS("g2v_walk_launch_packed_biased", a_near, a_far);
+    return walk_launch_packed(rows, edges, layout, V, E, L, seed, group, walker_begin, walker_end, walker_stride,
+                              out_nodes, out_len, out_key, a_near, a_far, workspace, stream,
+                              "g2v_walk_launch_packed_biased");
+}
+
+static int walk_host(const int32_t *rowptr, const int32_t *col, const uint32_t *qw, int32_t V, int64_t E, int32_t L,
+                     uint64_t seed, uint32_t group, int64_t walker_begin, int64_t walker_end, int64_t walker_stride,
+                     int32_t *out_nodes, int32_t *out_len, uint32_t a_near, uint32_t a_far) {
     G2V_REQUIRE(V > 0 && E >= 0 && L >= 1 && walker_stride >= 1, "g2v_walk_host: bad arguments");
     const int64_t n = walker_end > walker_begin ? (walker_end - walker_begin + walker_stride - 1) / walker_stride : 0;
     if (n == 0) return 0;
@@ -828,8 +1167,9 @@ extern "C" int g2v_walk_host(const int32_t *rowptr, const int32_t *col, const ui
         rc = g2v_walk_prepare((int32_t *)(d + o_rp), (int32_t *)(d + o_col), (uint32_t *)(d + o_qw), V, E, d + o_rows,
                               d + o_edges, &layout, d + o_ws, st);
         if (rc) break;
-        rc = g2v_walk_launch_packed(d + o_rows, d + o_edges, layout, V, E, L, seed, group, walker_begin, walker_end,
-                                    walker_stride, (int32_t *)(d + o_nodes), (int32_t *)(d + o_len), nullptr, d + o_ws, st);
+        rc = walk_launch_packed(d + o_rows, d + o_edges, layout, V, E, L, seed, group, walker_begin, walker_end,
+                                walker_stride, (int32_t *)(d + o_nodes), (int32_t *)(d + o_len), nullptr, a_near, a_far,
+                                d + o_ws, st, a_near ? "g2v_walk_host_biased" : "g2v_walk_launch_packed");
         if (rc) break;
         rc = 1;
         if (cudaMemcpyAsync(out_nodes, d + o_nodes, sizeof(int32_t) * (size_t)n * (size_t)L, cudaMemcpyDeviceToHost, st) != cudaSuccess) break;
@@ -844,6 +1184,23 @@ extern "C" int g2v_walk_host(const int32_t *rowptr, const int32_t *col, const ui
     cudaFree(d);
     if (st) cudaStreamDestroy(st);
     return rc;
+}
+
+extern "C" int g2v_walk_host(const int32_t *rowptr, const int32_t *col, const uint32_t *qw,
+                             int32_t V, int64_t E, int32_t L, uint64_t seed, uint32_t group,
+                             int64_t walker_begin, int64_t walker_end, int64_t walker_stride,
+                             int32_t *out_nodes, int32_t *out_len) {
+    return walk_host(rowptr, col, qw, V, E, L, seed, group, walker_begin, walker_end, walker_stride, out_nodes, out_len,
+                     0u, 0u);
+}
+
+extern "C" int g2v_walk_host_biased(const int32_t *rowptr, const int32_t *col, const uint32_t *qw,
+                                    int32_t V, int64_t E, int32_t L, uint64_t seed, uint32_t group,
+                                    int64_t walker_begin, int64_t walker_end, int64_t walker_stride,
+                                    int32_t *out_nodes, int32_t *out_len, uint32_t a_near, uint32_t a_far) {
+    G2V_REQUIRE_BIAS("g2v_walk_host_biased", a_near, a_far);
+    return walk_host(rowptr, col, qw, V, E, L, seed, group, walker_begin, walker_end, walker_stride, out_nodes, out_len,
+                     a_near, a_far);
 }
 
 extern "C" int g2v_test_draws(uint64_t seed, uint64_t subsequence, int32_t n, uint64_t *out_dev,

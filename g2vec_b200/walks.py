@@ -3,6 +3,8 @@
 324-352).  The work is done by ``g2v_walk_launch`` (csrc/g2v_walk.cu) on the current CUDA
 device; this module only owns buffers (torch tensors) and the walker-range bookkeeping.
 """
+import math
+
 import numpy as np
 import torch
 
@@ -80,13 +82,42 @@ class WalkGraph:
         return 4 * (self.V + 1) + 8 * self.E
 
 
+Q_MIN, Q_MAX = 1.0 / 256.0, 256.0          # node2vec in-out parameter q: the multipliers are integers in [1, 256]
+
+
+def walk_bias(q):
+    """node2vec's in-out parameter ``q`` (Grover & Leskovec 2016) -> the integer multipliers ``(a_near, a_far)``.
+
+    A candidate that is also an out-neighbour of the previous node (distance 1) weighs ``qw * a_near``, any other
+    candidate ``qw * a_far``: ``(256, rint(256 / q))`` for q >= 1 (BFS-like, stay near), ``(rint(256 q), 256)``
+    below (DFS-like, move away).  Powers of two are exact; otherwise a_near / a_far is within 0.5 / min(a) of 1/q
+    in relative terms.  There is no return parameter p: the walks are self-avoiding, so the move back to the
+    previous node always has weight 0 and p could not change anything.  Raises ValueError unless q is finite
+    and in [1/256, 256]."""
+    try:
+        qf = float(q)
+    except (TypeError, ValueError):
+        raise ValueError("q must be a number in [1/256, 256] (got %r)" % (q,))
+    if not (math.isfinite(qf) and Q_MIN <= qf <= Q_MAX):
+        raise ValueError("q must be finite and in [1/256, 256] (got %r)" % (q,))
+    if qf >= 1.0:
+        return 256, int(np.rint(256.0 / qf))
+    return int(np.rint(256.0 * qf)), 256
+
+
+def effective_q(q):
+    """the q the integer multipliers realise: a_near / a_far"""
+    a_near, a_far = walk_bias(q)
+    return a_near / a_far
+
+
 def num_walkers(V, reps, begin=0, end=None, stride=1):
     end = V * reps if end is None else end
     return max(0, (end - begin + stride - 1) // stride)
 
 
 def generate_paths(g, len_path, reps, seed=0, group=0, walker_begin=0, walker_end=None, walker_stride=1,
-                   out=None, canonical=False, plain_csr=False):
+                   out=None, canonical=False, plain_csr=False, q=1.0):
     """Run walkers w = walker_begin + i*walker_stride < walker_end (w = rep*V + src) of graph ``g``.
 
     Returns (nodes int32 [n, len_path] in VISIT order padded with -1, lens int32 [n]) as device
@@ -95,7 +126,10 @@ def generate_paths(g, len_path, reps, seed=0, group=0, walker_begin=0, walker_en
     ``canonical=True`` fuses ``path = tuple(sorted(path))`` (G2Vec.py:345) into the sampler: the rows come back
     sorted ascending and padded with INT32_MAX, and a third tensor holds their 64-bit keys (what
     ``paths.canonical_rows`` would otherwise compute from the visit-order rows in a second kernel).
-    ``plain_csr=True`` runs the kernel on the unpacked CSR arrays through ``g2v_walk_launch``."""
+    ``plain_csr=True`` runs the kernel on the unpacked CSR arrays through ``g2v_walk_launch``.
+    ``q`` is node2vec's in-out parameter (see ``walk_bias``); ``q == 1`` is the first-order walk and makes exactly
+    the launches of the plain entry points, any other q calls the ``_biased`` ones."""
+    bias = None if float(q) == 1.0 else walk_bias(q)
     lib = _capi.load()
     end = g.V * reps if walker_end is None else walker_end
     n = num_walkers(g.V, reps, walker_begin, end, walker_stride)
@@ -112,14 +146,21 @@ def generate_paths(g, len_path, reps, seed=0, group=0, walker_begin=0, walker_en
         if plain_csr:
             if canonical:
                 raise ValueError("canonical rows need the packed graph")
-            rc = lib.g2v_walk_launch(g.rowptr.data_ptr(), g.col.data_ptr(), g.qw.data_ptr(), g.V, g.E, int(len_path),
-                                     int(seed) & (2**64 - 1), int(group), int(walker_begin), int(end),
-                                     int(walker_stride), nodes.data_ptr(), lens.data_ptr(), g._ws.data_ptr(), st)
+            args = (g.rowptr.data_ptr(), g.col.data_ptr(), g.qw.data_ptr(), g.V, g.E, int(len_path),
+                    int(seed) & (2**64 - 1), int(group), int(walker_begin), int(end), int(walker_stride),
+                    nodes.data_ptr(), lens.data_ptr())
+            if bias is None:
+                rc = lib.g2v_walk_launch(*args, g._ws.data_ptr(), st)
+            else:
+                rc = lib.g2v_walk_launch_biased(*args, *bias, g._ws.data_ptr(), st)
         else:
-            rc = lib.g2v_walk_launch_packed(g.rows.data_ptr(), g.edges.data_ptr(), g.layout, g.V, g.E, int(len_path),
-                                            int(seed) & (2**64 - 1), int(group), int(walker_begin), int(end),
-                                            int(walker_stride), nodes.data_ptr(), lens.data_ptr(),
-                                            0 if key is None else key.data_ptr(), g._ws.data_ptr(), st)
+            args = (g.rows.data_ptr(), g.edges.data_ptr(), g.layout, g.V, g.E, int(len_path), int(seed) & (2**64 - 1),
+                    int(group), int(walker_begin), int(end), int(walker_stride), nodes.data_ptr(), lens.data_ptr(),
+                    0 if key is None else key.data_ptr())
+            if bias is None:
+                rc = lib.g2v_walk_launch_packed(*args, g._ws.data_ptr(), st)
+            else:
+                rc = lib.g2v_walk_launch_packed_biased(*args, *bias, g._ws.data_ptr(), st)
     _capi.check(rc, "g2v_walk_launch")
     if canonical:
         return nodes, lens, key
@@ -127,8 +168,10 @@ def generate_paths(g, len_path, reps, seed=0, group=0, walker_begin=0, walker_en
 
 
 def generate_paths_host(rowptr, col, qw, len_path, reps, seed=0, group=0, walker_begin=0, walker_end=None,
-                        walker_stride=1):
-    """Same through ``g2v_walk_host``: NumPy arrays in, NumPy arrays out (the C ABI does the copies)."""
+                        walker_stride=1, q=1.0):
+    """Same through ``g2v_walk_host`` (``g2v_walk_host_biased`` for q != 1): NumPy arrays in, NumPy arrays out (the
+    C ABI does the copies)."""
+    bias = None if float(q) == 1.0 else walk_bias(q)
     lib = _capi.load()
     rowptr = np.ascontiguousarray(rowptr, dtype=np.int32); col = np.ascontiguousarray(col, dtype=np.int32)
     qw = np.ascontiguousarray(qw, dtype=np.uint32)
@@ -138,17 +181,19 @@ def generate_paths_host(rowptr, col, qw, len_path, reps, seed=0, group=0, walker
     # page-locked result buffers: the device->host copy of the rows then runs at PCIe speed
     nodes = torch.empty((n, len_path), dtype=torch.int32, pin_memory=True).numpy()
     lens = torch.empty((n,), dtype=torch.int32, pin_memory=True).numpy()
-    rc = lib.g2v_walk_host(rowptr.ctypes.data, col.ctypes.data, qw.ctypes.data, V, col.shape[0], int(len_path),
-                           int(seed) & (2**64 - 1), int(group), int(walker_begin), int(end), int(walker_stride),
-                           nodes.ctypes.data, lens.ctypes.data)
+    args = (rowptr.ctypes.data, col.ctypes.data, qw.ctypes.data, V, col.shape[0], int(len_path),
+            int(seed) & (2**64 - 1), int(group), int(walker_begin), int(end), int(walker_stride),
+            nodes.ctypes.data, lens.ctypes.data)
+    rc = lib.g2v_walk_host(*args) if bias is None else lib.g2v_walk_host_biased(*args, *bias)
     _capi.check(rc, "g2v_walk_host")
     return nodes, lens
 
 
-def generate_pathSet(adjMat, maximumLength, iterations, seed=0, group=0):
+def generate_pathSet(adjMat, maximumLength, iterations, seed=0, group=0, q=1.0):
     """Drop-in for the reference's ``generate_pathSet(adjMat, maximumLength, iterations)``
-    (G2Vec.py:324): dense adjacency (or a WalkGraph) in, ``set`` of sorted int tuples out."""
+    (G2Vec.py:324): dense adjacency (or a WalkGraph) in, ``set`` of sorted int tuples out.  ``q``: node2vec's
+    in-out parameter (``walk_bias``)."""
     g = adjMat if isinstance(adjMat, WalkGraph) else WalkGraph.from_dense(adjMat)
-    nodes, lens = generate_paths(g, maximumLength, iterations, seed=seed, group=group)
+    nodes, lens = generate_paths(g, maximumLength, iterations, seed=seed, group=group, q=q)
     nodes = nodes.cpu().numpy(); lens = lens.cpu().numpy()
     return {tuple(sorted(int(x) for x in row[:n])) for row, n in zip(nodes, lens)}

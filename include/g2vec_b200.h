@@ -97,6 +97,25 @@ int g2v_walk_host(const int32_t *rowptr, const int32_t *col, const uint32_t *qw,
                   int64_t walker_end, int64_t walker_stride, int32_t *out_nodes,
                   int32_t *out_len);
 
+/* node2vec's in-out bias (Grover & Leskovec 2016, parameter q).  A walker at v whose previous node is t weighs an
+ * unvisited out-neighbour x of quantised weight qw as  qw * a_near  if the edge t -> x exists (x in t's CSR row)
+ * and  qw * a_far  otherwise; step 0 has no previous node and uses qw.  The draw is unchanged: T = sum of the
+ * effective weights (uint64), r = floor(x * T / 2^64), first neighbour in ascending order whose inclusive prefix
+ * exceeds r.  1 <= a_near, a_far <= 256, else the call fails.  Equal multipliers scale every weight alike and give
+ * the bits of the plain entry point (they run its kernels).  Arguments otherwise as their plain counterparts. */
+int g2v_walk_launch_biased(const int32_t *rowptr, const int32_t *col, const uint32_t *qw, int32_t V,
+                           int64_t E, int32_t L, uint64_t seed, uint32_t group, int64_t walker_begin,
+                           int64_t walker_end, int64_t walker_stride, int32_t *out_nodes,
+                           int32_t *out_len, uint32_t a_near, uint32_t a_far, void *workspace, void *stream);
+int g2v_walk_launch_packed_biased(const void *rows, const void *edges, int32_t layout, int32_t V, int64_t E,
+                                  int32_t L, uint64_t seed, uint32_t group, int64_t walker_begin,
+                                  int64_t walker_end, int64_t walker_stride, int32_t *out_nodes, int32_t *out_len,
+                                  int64_t *out_key, uint32_t a_near, uint32_t a_far, void *workspace, void *stream);
+int g2v_walk_host_biased(const int32_t *rowptr, const int32_t *col, const uint32_t *qw, int32_t V,
+                         int64_t E, int32_t L, uint64_t seed, uint32_t group, int64_t walker_begin,
+                         int64_t walker_end, int64_t walker_stride, int32_t *out_nodes,
+                         int32_t *out_len, uint32_t a_near, uint32_t a_far);
+
 /* ---------------------------------------------------------------------------------------
  * HOT PATH 2 -- modified CBOW.  Replaces the TF1 graph of compute_genetovec,
  * G2Vec.py:231-251, one optimizer step at a time; the epoch loop and the early stop
