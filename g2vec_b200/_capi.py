@@ -122,6 +122,7 @@ SIGNATURES = {
                                          _f32, _f32, _i32, _vp, _vp]),
     "g2v_pcc_zscore": (ctypes.c_int, [_vp, _i32, _i32, _vp, _vp]),
     "g2v_pcc_edge_weights": (ctypes.c_int, [_vp, _i32, _i32, _vp, _vp, _i64, _vp, _vp]),
+    "g2v_corr_transform": (ctypes.c_int, [_vp, _i32, _i32, _i32, _vp, _vp]),
     "g2v_paths_canonicalise": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
     "g2v_paths_mark": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "g2v_paths_set_workspace_bytes": (ctypes.c_size_t, [_i64]),

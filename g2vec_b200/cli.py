@@ -37,6 +37,14 @@ fall between the groups; a training split with one label only is an error.  The 
 run prints a ``class weights:`` line after ``Start training``; the accuracies, ``LOSS[val]``, ``--patience`` and
 ``--lr-patience`` keep their meanings, and the logged training loss is the weighted one.
 
+``--correlation {pearson,spearman,bicor}`` (default ``pearson``, the reference's) chooses the coefficient of step 3's
+edge weights, and ``--min-corr T`` (default 0.5, finite, 0 <= T < 1) the cutoff: an edge is kept in a group's graph iff
+its |coefficient| over that group's samples is > T (DESIGN.md §4.22).  ``spearman`` is Pearson's coefficient of the
+average ranks (ties share the mean of their positions); ``bicor`` is the biweight midcorrelation of WGCNA
+(Langfelder & Horvath 2012), falling back to Pearson for a gene whose median absolute deviation is 0.  Both need
+finite expression values and at most 32768 samples per group.  A run with either option off its default prints a
+``correlation:`` line under the step-3 banner.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle`` or ``--class-weight``, at every table size (DESIGN.md §4.13); ``--class-weight 1,1`` writes the
@@ -73,6 +81,13 @@ def parse_arguments(argv=None):
                    help="node2vec's in-out parameter of the random walks, in [1/256, 256]: Q > 1 keeps a walk near the "
                         "previous gene's neighbours (BFS-like), Q < 1 moves it away (DFS-like); 1 (default) = the "
                         "reference's first-order walk.  There is no return parameter: the walks never revisit a gene")
+    p.add_argument('--correlation', choices=['pearson', 'spearman', 'bicor'], default='pearson',
+                   help="coefficient of the edge weights: 'pearson' (default, the reference's), 'spearman' (Pearson "
+                        "on average ranks) or 'bicor' (biweight midcorrelation); spearman and bicor take at most "
+                        "32768 samples per group and finite expression values")
+    p.add_argument('--min-corr', type=float, default=0.5, metavar='T',
+                   help="an edge is kept iff its |coefficient| over the group's samples is > T, 0 <= T < 1 "
+                        "(default 0.5, the reference's cutoff)")
     p.add_argument('--algo', choices=['rows', 'rank1'], default='rows',
                    help="CBOW kernels: 'rows' = embedding-row gather/scatter (default), 'rank1' = collapsed, "
                         "bit-reproducible trainer; same results to fp32 rounding")
@@ -111,6 +126,8 @@ def parse_arguments(argv=None):
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
+    if not (np.isfinite(args.min_corr) and 0.0 <= args.min_corr < 1.0):
+        p.error("--min-corr must be a finite number with 0 <= T < 1")
     if args.class_weight is not None:
         args.class_weight = _parse_class_weight(args.class_weight, p)
     if not 0.0 <= float(np.float32(args.weight_decay)) < 1.0:
@@ -311,6 +328,8 @@ def main(argv=None):
         a_near, a_far = walks.walk_bias(args.walk_q)
         print('    walk q  : %g\t(in-out multipliers %d near, %d far: effective q = %.6g)'
               % (args.walk_q, a_near, a_far, walks.effective_q(args.walk_q)))
+    if args.correlation != 'pearson' or args.min_corr != 0.5:
+        print('    correlation: %s (|r| > %g)' % (args.correlation, args.min_corr))
     idx = {g: i for i, g in enumerate(data['gene'])}
     src = np.fromiter((idx[e[0]] for e in network['edge']), dtype=np.int32, count=len(network['edge']))
     dst = np.fromiter((idx[e[1]] for e in network['edge']), dtype=np.int32, count=len(network['edge']))
@@ -322,7 +341,8 @@ def main(argv=None):
     lens = torch.empty(2 * n_total, dtype=torch.int32, device=dev)
     key = torch.empty(2 * n_total, dtype=torch.int64, device=dev)
     for i, _group in enumerate(['g', 'p']):
-        rp, col, w = graph.group_csr_gpu(data['expr'], data['label'], i, src, dst)
+        rp, col, w = graph.group_csr_gpu(data['expr'], data['label'], i, src, dst, threshold=args.min_corr,
+                                         method=args.correlation)
         wg = walks.WalkGraph(rp, col, weights=w)
         sl = slice(i * n_total, (i + 1) * n_total)
         if dist is None:

@@ -11,33 +11,35 @@
 // bit; agreement is ~1e-7, tests compare at 2e-6 and the kept-edge set away from the 0.5 threshold).
 // Thresholding and CSR assembly stay with the host (torch sort as plumbing, g2vec_b200/graph.py).
 #include "g2v_common.cuh"
+#include "g2v_pcc.cuh"
 
 namespace g2v {
 
 __global__ void __launch_bounds__(256)
 pcc_zscore_kernel(const float *__restrict__ expr, int32_t S, int32_t V, float *__restrict__ z) {
     // block = 32 genes x 8 sample-lanes; expr is sample-major [S][V] (the reference's data['expr'] rows)
-    __shared__ double sh[8][33];
+    // (the arithmetic is g2v_pcc.cuh's, which the bicor transform's Pearson fallback shares)
+    __shared__ double sh[kZscoreLanes][33];
     const int gx = threadIdx.x & 31, sy = threadIdx.x >> 5;
     const int g = blockIdx.x * 32 + gx;
+    const auto x = [&](int s) { return expr[(size_t)s * V + g]; };
     double sum = 0.0;
-    if (g < V) for (int s = sy; s < S; s += 8) sum += (double)expr[(size_t)s * V + g];
+    if (g < V) sum = zscore_lane_sum(x, sy, S);
     sh[sy][gx] = sum;
     __syncthreads();
     double mu = 0.0;
-    for (int k = 0; k < 8; ++k) mu += sh[k][gx];
+    for (int k = 0; k < kZscoreLanes; ++k) mu += sh[k][gx];
     mu /= (double)S;
     __syncthreads();
     double ss = 0.0;
-    if (g < V) for (int s = sy; s < S; s += 8) { const double d = (double)expr[(size_t)s * V + g] - mu; ss += d * d; }
+    if (g < V) ss = zscore_lane_ss(x, sy, S, mu);
     sh[sy][gx] = ss;
     __syncthreads();
     double var = 0.0;
-    for (int k = 0; k < 8; ++k) var += sh[k][gx];
+    for (int k = 0; k < kZscoreLanes; ++k) var += sh[k][gx];
     const double sd = sqrt(var / (double)S);
     if (g < V)
-        for (int s = sy; s < S; s += 8)
-            z[(size_t)g * S + s] = sd > 0.0 ? (float)(((double)expr[(size_t)s * V + g] - mu) / sd) : 0.f;
+        for (int s = sy; s < S; s += kZscoreLanes) z[(size_t)g * S + s] = zscore_value(x(s), mu, sd);
 }
 
 __global__ void __launch_bounds__(256)

@@ -539,6 +539,21 @@ int g2v_pcc_zscore(const float *expr, int32_t S, int32_t V, float *z, void *stre
 int g2v_pcc_edge_weights(const float *z, int32_t S, int32_t V, const int32_t *src, const int32_t *dst,
                          int64_t E, float *w, void *stream);
 
+/* Spearman and biweight-midcorrelation edge weights (DESIGN.md §4.22).  g2v_corr_transform writes, like
+ * g2v_pcc_zscore, a gene-major z [V*S] from the sample-major expr [S*V] (z must not overlap expr), with
+ * mean_s z[a][s] * z[b][s] = the coefficient, so g2v_pcc_edge_weights turns z into the weights unchanged:
+ *   G2V_CORR_SPEARMAN  z = the Pearson z-score (population std; 0 for a constant gene) of the average ranks
+ *                      r_i = (#{x < x_i} + #{x <= x_i} + 1) / 2, -0.0 tying with +0.0;
+ *   G2V_CORR_BICOR     med = median(x) (mean of the two middle values for even S), mad = median(|x - med|); if
+ *                      mad > 0: u = (x - med) / (9 mad), t = (x - med)(1 - u^2)^2 for |u| < 1 else 0,
+ *                      z = t sqrt(S) / ||t||; if mad = 0: the bits g2v_pcc_zscore gives the gene.
+ * Double arithmetic, float32 z; the bits do not depend on the run or on the launch.  1 <= S <= G2V_CORR_MAX_SAMPLES
+ * and V >= 1, else the call fails with nothing launched.  Two launches, never synchronises. */
+#define G2V_CORR_SPEARMAN 1
+#define G2V_CORR_BICOR 2
+#define G2V_CORR_MAX_SAMPLES 32768
+int g2v_corr_transform(const float *expr, int32_t S, int32_t V, int32_t method, float *z, void *stream);
+
 /* ---------------------------------------------------------------------------------------
  * Between the two hot paths (SURVEY.md 8f-2): `tuple(sorted(path))` into a set (G2Vec.py:345,351) and
  * the removal of paths common to both groups (G2Vec.py:313).
