@@ -61,10 +61,10 @@ ROUTES = ["fwdbwd", "fwdbwd_csc", "fwd_do", "fwdbwd_csc_det", "fwd_do_det", "loo
 FIXED_ORDER = {"fwdbwd_csc_det", "fwd_do_det", "loop_tail_det", "r1_windows_csc"}
 
 
-def run(env, P, route, cw, lo=0, n=None):
+def run(env, P, route, cw, lo=0, n=None, max_ctas=0):
     """One call of g2v_cbow_<route> (cw None) or its _cw form over list positions [lo, lo + n) of P.win; returns its
     outputs as NumPy: dO (per position, times the scale where the entry point stores it so), c, g_ih, g_ho, loss,
-    correct count."""
+    correct count, and the whole counter buffer acc.  max_ctas: the grid cap of the fixed-order routes."""
     import torch
     lib, d = env["lib"], P.d
     n = P.n - lo if n is None else n
@@ -87,16 +87,16 @@ def run(env, P, route, cw, lo=0, n=None):
     elif route in ("fwdbwd_csc", "fwdbwd_csc_det"):
         args = (*common, win_ptr, n, inv_n, W, Wo, d["cscptr"].data_ptr(), d["pos"].data_ptr(), out["dO"].data_ptr(),
                 out["g_ih"].data_ptr(), out["g_ho"].data_ptr(), acc, acc + 8, V, D, red)
-        rc = fn(*args, *((ws.data_ptr(), 0) if route.endswith("det") else ()), *extra, stream())
+        rc = fn(*args, *((ws.data_ptr(), max_ctas) if route.endswith("det") else ()), *extra, stream())
     elif route in ("fwd_do", "fwd_do_det"):
         args = (*common, win_ptr, n, inv_n, W, Wo, out["dO"].data_ptr(), out["g_ho"].data_ptr(), acc, acc + 8, V, D, red)
-        rc = fn(*args, *((ws.data_ptr(), 0) if route.endswith("det") else ()), *extra, stream())
+        rc = fn(*args, *((ws.data_ptr(), max_ctas) if route.endswith("det") else ()), *extra, stream())
     elif route in ("loop_tail", "loop_tail_det"):
         ctl = z(8, dtype=torch.int64)
         env["capi"].check(lib.g2v_cbow_loop_init(ctl.data_ptr(), 10, 1, stream()), "g2v_cbow_loop_init")
         args = (ctl.data_ptr(), *common, win_ptr, n, inv_n, W, Wo, out["dO"].data_ptr(), out["g_ho"].data_ptr(), acc,
                 V, D, red)
-        rc = fn(*args, *((ws.data_ptr(), 0) if route.endswith("det") else ()), *extra, stream())
+        rc = fn(*args, *((ws.data_ptr(), max_ctas) if route.endswith("det") else ()), *extra, stream())
         out["ctl"] = ctl
     elif route == "fwdbwd_slabs":
         S = 3
@@ -123,6 +123,7 @@ def run(env, P, route, cw, lo=0, n=None):
     res["dO"] = res["dO"][:n]
     res["loss"] = float(a[slot:slot + 1].view(np.float64)[0])
     res["correct"] = int(a[slot + 1])
+    res["acc"] = a
     if route.startswith("loop_tail"):
         assert int(out["ctl"].cpu()[6]) == 1                      # the carry is pending
     return res
