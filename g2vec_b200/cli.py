@@ -45,6 +45,16 @@ average ranks (ties share the mean of their positions); ``bicor`` is the biweigh
 finite expression values and at most 32768 samples per group.  A run with either option off its default prints a
 ``correlation:`` line under the step-3 banner.
 
+``--permutations B`` (default 0: off) adds a label-permutation test of every gene's t statistic (DESIGN.md §4.24):
+B permutations of the good / poor labels (Fisher-Yates, seeded by ``--seed``; the observed labelling is not among
+them) give each gene a raw p-value P = (1 + #{|t_b| >= |t|}) / (B + 1), Westfall & Young's step-down maxT adjusted
+p-value P_maxT (Ge, Dudoit & Speed 2003, as multtest's mt.maxT) and the Benjamini-Hochberg q-value Q of P.  The
+family is every gene of the analysis.  The inputs are checked before step 3 (labels 0 and 1 both present, 3 to 32768
+samples with label 0 or 1, finite expression values, 1 <= B <= 2^24), the test runs on the GPU after step 6 (on rank 0
+only under torchrun) and prints a ``permutation test:`` line, and step 7 also writes RESULT_NAME_pvalues.txt: per gene,
+in the order of _lgroups.txt, its L-group, T (the observed |t|, ``inf`` at perfect separation, where step 6's t-score
+is 0), P, P_maxT, Q and whether it is a biomarker.  P, P_maxT and Q do not depend on training.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle`` or ``--class-weight``, at every table size (DESIGN.md §4.13); ``--class-weight 1,1`` writes the
@@ -123,6 +133,10 @@ def parse_arguments(argv=None):
     p.add_argument('--class-weight', type=str, default=None, metavar='{balanced | W0,W1}',
                    help="weights of the label-0 and label-1 windows in the training loss: 'balanced' = n / (2 n_y) "
                         "from the training windows, or two finite numbers > 0; default off")
+    p.add_argument('--permutations', type=int, default=0, metavar='B',
+                   help="label-permutation test of every gene's t statistic with B permutations (1 <= B <= 2^24): "
+                        "raw, step-down maxT and Benjamini-Hochberg p-values in RESULT_NAME_pvalues.txt; 0 (default) "
+                        "= off")
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
@@ -132,6 +146,8 @@ def parse_arguments(argv=None):
         args.class_weight = _parse_class_weight(args.class_weight, p)
     if not 0.0 <= float(np.float32(args.weight_decay)) < 1.0:
         p.error("--weight-decay must be a finite number with 0 <= weight-decay < 1")
+    if not 0 <= args.permutations <= 1 << 24:
+        p.error("--permutations must be an integer in [0, 2^24]")
     if args.patience < 1:
         p.error("--patience must be an integer >= 1")
     if args.lr_patience < 0:
@@ -276,6 +292,15 @@ def write_lgroups(prefix, lgroup, genes):
         f.writelines('%s\t%d\n' % (g, k) for g, k in zip(genes, lgroup))
 
 
+def write_pvalues(prefix, genes, lgroup, res, biomarkers):
+    """One row per gene in the order of _lgroups.txt: L-group, T, P, P_maxT, Q of a perm.PermResult, biomarker 0/1."""
+    bm = set(biomarkers)
+    with open(prefix + "_pvalues.txt", 'w') as f:
+        f.write('GeneSymbol\tLgroup(0:good,1:poor,2:other)\tT\tP\tP_maxT\tQ\tBiomarker\n')
+        f.writelines('%s\t%d\t%.6f\t%.6g\t%.6g\t%.6g\t%d\n' % (g, k, t, pv, pm, qv, g in bm)
+                     for g, k, t, pv, pm, qv in zip(genes, lgroup, res.T, res.P, res.P_maxT, res.Q))
+
+
 def write_vectors(prefix, genes, mat):
     with open(prefix + "_vectors.txt", 'w') as f:
         f.write('GeneSymbol' + ''.join('\tV%d' % i for i in range(mat.shape[1])) + '\n')
@@ -320,6 +345,13 @@ def main(argv=None):
     print('    n_samples: %d' % n_samples)
     print('    n_genes  : %d\t(common genes in both EXPRESSION and NETWORK)' % n_genes)
     print('    n_edges  : %d\t(edges with the common genes)' % len(network['edge']))
+    if args.permutations:
+        from . import perm
+        try:                                           # fail now rather than after training
+            perm.check_inputs(data['expr'], data['label'], args.permutations)
+        except ValueError as e:
+            print('ERROR: %s' % e)
+            sys.exit(1)
 
     print('>>> 3. Generate random paths from each group')
     print('    *** most time consuming step ***')
@@ -389,6 +421,11 @@ def main(argv=None):
         ranked = sorted(zip(genes[sel], score), key=lambda gs: gs[1], reverse=True)
         biomarkers += sorted(g for g, _ in ranked[:args.numBiomarker])
     biomarkers = sorted(biomarkers)
+    if args.permutations:
+        res = perm.perm_test(data['expr'], data['label'], args.permutations, seed=args.seed)
+        sig = res.P_maxT <= 0.05
+        print('    permutation test: %d label permutations: %d genes with P_maxT <= 0.05 (%d of the biomarkers)'
+              % (args.permutations, int(sig.sum()), len(set(genes[sig]) & set(biomarkers))))
 
     print(">>> 7. Save results")
     write_biomarkers(args.RESULT_NAME, biomarkers)
@@ -397,6 +434,9 @@ def main(argv=None):
     print('    %s_lgroups.txt' % args.RESULT_NAME)
     write_vectors(args.RESULT_NAME, genes, mat)
     print('    %s_vectors.txt' % args.RESULT_NAME)
+    if args.permutations:
+        write_pvalues(args.RESULT_NAME, genes, lgroup, res, biomarkers)
+        print('    %s_pvalues.txt' % args.RESULT_NAME)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

@@ -555,6 +555,30 @@ int g2v_pcc_edge_weights(const float *z, int32_t S, int32_t V, const int32_t *sr
 int g2v_corr_transform(const float *expr, int32_t S, int32_t V, int32_t method, float *z, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Label-permutation test of the gene t statistics (DESIGN.md §4.24; g2vec_b200/perm.py does the host side).
+ * n samples (3 <= n <= G2V_PERM_MAX_SAMPLES), S_pad = a multiple of 32 with n <= S_pad <= G2V_PERM_MAX_SAMPLES;
+ * padding bytes are 0.  Permutations are numbered b = 1 .. B, B <= G2V_PERM_MAX_PERMUTATIONS.
+ * g2v_perm_labels: M [n_b * S_pad] u8, row r = permutation b = b_begin + 1 + r of the indicator obs [n] (0/1):
+ *   Fisher-Yates from obs, for i = n-1 down to 1: j = hi64(draw64(seed, 2^63 + b, n-1-i) * (i+1)), swap i and j
+ *   (draw64 = the walk sampler's Philox4x32-10 stream).  A row depends only on (obs, seed, b): chunks of one
+ *   sequence of calls give the rows of one big call.
+ * g2v_perm_sums: A [n_b * G] int64 = M . q, exact.  q [G][S_pad] reaches the device as three byte planes,
+ *   planes = {h [G*S_pad] s8, m [G*S_pad] u8, l [G*S_pad] u8} back to back, q = 2^16 h + 2^8 m + l, each gene's
+ *   samples contiguous; |q| <= 2^22.  INT8 tensor cores (mma.sync m16n8k32), int64 only in the epilogue.
+ * g2v_perm_tally: per row of A, N_j = n A_j - k Q_j and rho_j = N_j^2 / W_j (float64, 0 when W_j = 0);
+ *   count[j] += |N_j| >= absN_obs[j];  count_maxt[j] += (max over j' >= j of rho_j') >= rho_obs[j].
+ *   Integer atomics only; the counts do not depend on the grid or on how the rows are chunked.
+ * Out-of-range sizes fail with nothing launched.  One launch each, never synchronises. */
+#define G2V_PERM_MAX_SAMPLES 32768
+#define G2V_PERM_MAX_PERMUTATIONS (1 << 24)
+int g2v_perm_labels(const uint8_t *obs, int32_t n, int32_t S_pad, uint64_t seed, int64_t b_begin, int64_t n_b,
+                    uint8_t *M, void *stream);
+int g2v_perm_sums(const uint8_t *M, const uint8_t *planes, int64_t n_b, int32_t S_pad, int32_t G, int64_t *A,
+                  void *stream);
+int g2v_perm_tally(const int64_t *A, int64_t n_b, int32_t G, int32_t n, int32_t k, const int64_t *Q, const double *W,
+                   const int64_t *absN_obs, const double *rho_obs, int64_t *count, int64_t *count_maxt, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Between the two hot paths (SURVEY.md 8f-2): `tuple(sorted(path))` into a set (G2Vec.py:345,351) and
  * the removal of paths common to both groups (G2Vec.py:313).
  * g2v_paths_canonicalise: row i of nodes [n*L] (-1 or INT32_MAX padded) -> sorted [n*L] ascending with
