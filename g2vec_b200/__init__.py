@@ -6,6 +6,7 @@ behind the reference's call sites and CLI.  Hand-written sm_90a CUDA reached thr
 from .walks import WalkGraph, generate_paths, generate_paths_host, generate_pathSet, walk_bias  # noqa: F401
 from .cbow import train_cbow, compute_genetovec, cbow_step_host, CbowModel, WindowFeeder  # noqa: F401
 from .perm import perm_test  # noqa: F401
+from .neighbors import nearest_genes  # noqa: F401
 from . import graph, paths  # noqa: F401
 
 __version__ = "0.1.0"

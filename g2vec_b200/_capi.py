@@ -126,6 +126,10 @@ SIGNATURES = {
     "g2v_perm_labels": (ctypes.c_int, [_vp, _i32, _i32, _u64, _i64, _i64, _vp, _vp]),
     "g2v_perm_sums": (ctypes.c_int, [_vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     "g2v_perm_tally": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "g2v_nbr_splits": (_i32, [_i64]),
+    "g2v_nbr_norms": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp]),
+    "g2v_nbr_partial": (ctypes.c_int, [_vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp]),
+    "g2v_nbr_merge": (ctypes.c_int, [_vp, _vp, _i32, _i64, _i32, _vp, _vp, _vp]),
     "g2v_paths_canonicalise": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
     "g2v_paths_mark": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "g2v_paths_set_workspace_bytes": (ctypes.c_size_t, [_i64]),

@@ -55,6 +55,14 @@ only under torchrun) and prints a ``permutation test:`` line, and step 7 also wr
 in the order of _lgroups.txt, its L-group, T (the observed |t|, ``inf`` at perfect separation, where step 6's t-score
 is 0), P, P_maxT, Q and whether it is a biomarker.  P, P_maxT and Q do not depend on training.
 
+``--neighbors K`` (default 0: off; 0 <= K <= 64) adds the K nearest genes of every gene in the learned embedding, by
+exact cosine on the GPU (DESIGN.md §4.25).  The searched genes are those in at least one good or poor random path (the
+``n_genes`` count of step 3): the others keep their random initial vectors.  A run whose paths hold K genes or fewer
+stops with an ``ERROR`` after step 3, before training.  After step 6 (on rank 0 only under torchrun) the run prints a
+``neighbors:`` line with the share of (gene, neighbour) pairs in the same L-group, and step 7 also writes
+RESULT_NAME_neighbors.txt: per searched gene, in the order of _lgroups.txt, K rows of its L-group, the rank 1..K, the
+neighbour, its L-group and the cosine, nearest first (equal cosines by the neighbour's position in _lgroups.txt).
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle`` or ``--class-weight``, at every table size (DESIGN.md §4.13); ``--class-weight 1,1`` writes the
@@ -137,6 +145,9 @@ def parse_arguments(argv=None):
                    help="label-permutation test of every gene's t statistic with B permutations (1 <= B <= 2^24): "
                         "raw, step-down maxT and Benjamini-Hochberg p-values in RESULT_NAME_pvalues.txt; 0 (default) "
                         "= off")
+    p.add_argument('--neighbors', type=int, default=0, metavar='K',
+                   help="the K nearest genes (0 <= K <= 64) of every gene in the random paths by cosine of the "
+                        "learned vectors, in RESULT_NAME_neighbors.txt; 0 (default) = off")
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
@@ -148,6 +159,8 @@ def parse_arguments(argv=None):
         p.error("--weight-decay must be a finite number with 0 <= weight-decay < 1")
     if not 0 <= args.permutations <= 1 << 24:
         p.error("--permutations must be an integer in [0, 2^24]")
+    if not 0 <= args.neighbors <= 64:
+        p.error("--neighbors must be an integer in [0, 64]")
     if args.patience < 1:
         p.error("--patience must be an integer >= 1")
     if args.lr_patience < 0:
@@ -301,6 +314,16 @@ def write_pvalues(prefix, genes, lgroup, res, biomarkers):
                      for g, k, t, pv, pm, qv in zip(genes, lgroup, res.T, res.P, res.P_maxT, res.Q))
 
 
+def write_neighbors(prefix, genes, lgroup, sub, idx, sim):
+    """K rows per searched gene (sub: their indices in genes, ascending): L-group, rank 1..K, the neighbour (idx holds
+    positions in sub), its L-group and the cosine."""
+    with open(prefix + "_neighbors.txt", 'w') as f:
+        f.write('GeneSymbol\tLgroup(0:good,1:poor,2:other)\tRank\tNeighbor\tNeighborLgroup\tCosine\n')
+        for g, row, srow in zip(sub, idx, sim):
+            f.writelines('%s\t%d\t%d\t%s\t%d\t%.6f\n' % (genes[g], lgroup[g], r + 1, genes[sub[j]], lgroup[sub[j]], s)
+                         for r, (j, s) in enumerate(zip(row, srow)))
+
+
 def write_vectors(prefix, genes, mat):
     with open(prefix + "_vectors.txt", 'w') as f:
         f.write('GeneSymbol' + ''.join('\tV%d' % i for i in range(mat.shape[1])) + '\n')
@@ -394,6 +417,13 @@ def main(argv=None):
     geneFreq = paths.gene_freq_dict(code, data['gene'])
     print("    n_paths : %d" % int(w_label.shape[0]))
     print("    n_genes : %d\t(genes in good or poor random paths)" % len(geneFreq))
+    if args.neighbors:
+        from . import neighbors
+        in_paths = neighbors.genes_in_paths(code)     # the same on every rank: each holds the 1-GPU windows
+        if args.neighbors >= len(in_paths):
+            print('ERROR: --neighbors %d needs more than %d genes in the random paths, found %d'
+                  % (args.neighbors, args.neighbors, len(in_paths)))
+            sys.exit(1)
 
     print(">>> 4. Compute distributed representations using modified CBOW")
     mat = cbow.train_cbow(w_rowptr, w_gene, w_label, n_genes, args.sizeHiddenlayer, args.learningRate,
@@ -426,6 +456,11 @@ def main(argv=None):
         sig = res.P_maxT <= 0.05
         print('    permutation test: %d label permutations: %d genes with P_maxT <= 0.05 (%d of the biomarkers)'
               % (args.permutations, int(sig.sum()), len(set(genes[sig]) & set(biomarkers))))
+    if args.neighbors:
+        nbr_idx, nbr_sim = neighbors.nearest_genes(mat[in_paths], args.neighbors)
+        print("    neighbors: %d nearest genes by cosine for each of %d genes in paths; %.1f %% of the pairs share the "
+              "gene's L-group" % (args.neighbors, len(in_paths),
+                                  100.0 * neighbors.same_lgroup_share(lgroup[in_paths], nbr_idx)))
 
     print(">>> 7. Save results")
     write_biomarkers(args.RESULT_NAME, biomarkers)
@@ -437,6 +472,9 @@ def main(argv=None):
     if args.permutations:
         write_pvalues(args.RESULT_NAME, genes, lgroup, res, biomarkers)
         print('    %s_pvalues.txt' % args.RESULT_NAME)
+    if args.neighbors:
+        write_neighbors(args.RESULT_NAME, genes, lgroup, in_paths, nbr_idx, nbr_sim)
+        print('    %s_neighbors.txt' % args.RESULT_NAME)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

@@ -579,6 +579,32 @@ int g2v_perm_tally(const int64_t *A, int64_t n_b, int32_t G, int32_t n, int32_t 
                    const int64_t *absN_obs, const double *rho_obs, int64_t *count, int64_t *count_maxt, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Exact cosine K nearest genes of every gene (DESIGN.md §4.25; g2vec_b200/neighbors.py does the host side).
+ * W [m][D] float32 row-major, 2 <= m <= G2V_NBR_MAX_GENES, D >= 1, every value finite; 1 <= K <= min(G2V_NBR_MAX_K,
+ * m - 1).  Everything in IEEE float64:
+ *   dot_ij = ((0 + W_i0 W_j0) + W_i1 W_j1) + ... + W_i(D-1) W_j(D-1)   (a chain of fma in ascending d, from +0);
+ *   n_i = dot_ii;  inv_i = 1 / sqrt(n_i) (correctly rounded), 0 when n_i = 0;
+ *   s_ij = (dot_ij * inv_i) * inv_j, +0 when either norm is 0.
+ * The neighbours of i are the K genes j != i with the largest s_ij, ordered by s_ij descending, equal values by j
+ * ascending: idx [m][K] int32 and sim [m][K] float64, the same bits whatever the grid or the split.
+ * g2v_nbr_splits: the number of column splits of g2v_nbr_partial for m genes on the current device (a function of m
+ *   and the SM count only); 0 on error.  The partial lists take splits * m * K entries of each type.
+ * g2v_nbr_norms: inv [m].
+ * g2v_nbr_partial: per split y and row i, the list of row i over split y's column range at [(y * m + i) * K], padded
+ *   with j = -1, s = -inf when the range holds fewer than K genes.  With one split the lists are the result: pass idx
+ *   and sim as part_idx and part_sim.
+ * g2v_nbr_merge: splits > 1 (must equal g2v_nbr_splits(m)) partial lists -> idx, sim.
+ * Out-of-range sizes fail with nothing launched.  One launch each, never synchronises. */
+#define G2V_NBR_MAX_K 64
+#define G2V_NBR_MAX_GENES (1 << 30)
+int32_t g2v_nbr_splits(int64_t m);
+int g2v_nbr_norms(const float *W, int64_t m, int32_t D, double *inv, void *stream);
+int g2v_nbr_partial(const float *W, const double *inv, int64_t m, int32_t D, int32_t K, int32_t *part_idx,
+                    double *part_sim, void *stream);
+int g2v_nbr_merge(const int32_t *part_idx, const double *part_sim, int32_t splits, int64_t m, int32_t K, int32_t *idx,
+                  double *sim, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Between the two hot paths (SURVEY.md 8f-2): `tuple(sorted(path))` into a set (G2Vec.py:345,351) and
  * the removal of paths common to both groups (G2Vec.py:313).
  * g2v_paths_canonicalise: row i of nodes [n*L] (-1 or INT32_MAX padded) -> sorted [n*L] ascending with
