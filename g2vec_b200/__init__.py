@@ -7,6 +7,7 @@ from .walks import WalkGraph, generate_paths, generate_paths_host, generate_path
 from .cbow import train_cbow, compute_genetovec, cbow_step_host, CbowModel, WindowFeeder  # noqa: F401
 from .perm import perm_test  # noqa: F401
 from .neighbors import nearest_genes  # noqa: F401
+from .kmeans import kmeans_lgroups  # noqa: F401
 from . import graph, paths  # noqa: F401
 
 __version__ = "0.1.0"

@@ -130,6 +130,13 @@ SIGNATURES = {
     "g2v_nbr_norms": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp]),
     "g2v_nbr_partial": (ctypes.c_int, [_vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp]),
     "g2v_nbr_merge": (ctypes.c_int, [_vp, _vp, _i32, _i64, _i32, _vp, _vp, _vp]),
+    "g2v_km_assign": (ctypes.c_int, [_vp, _i64, _i32, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp]),
+    "g2v_km_seed": (ctypes.c_int, [_vp, _i64, _i32, _vp, _u64, _i64, _i32, _i32, _vp, _vp, _vp]),
+    "g2v_km_blocks": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i32, _vp, _i32, _vp, _vp, _vp, _vp]),
+    "g2v_km_update": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp,
+                                     _vp, _vp]),
+    "g2v_km_contingency": (ctypes.c_int, [_vp, _vp, _i64, _i32, _vp, _vp]),
+    "g2v_km_agree": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "g2v_paths_canonicalise": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
     "g2v_paths_mark": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "g2v_paths_set_workspace_bytes": (ctypes.c_size_t, [_i64]),

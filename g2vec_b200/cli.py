@@ -2,8 +2,8 @@
 
 Same positionals, options, progress banners and output files as /root/reference/G2Vec.py
 (parse_arguments :505-518, main :11-119, writers :127-131,159-165,203-215).  Steps 1, 2, 5, 6, 7 are
-plain Python/NumPy/scikit-learn as in the reference; step 3 runs g2vec_b200.walks on the GPU and
-step 4 g2vec_b200.cbow.  Two documented differences: ``--epoch`` is honoured as the cap on optimizer
+plain Python/NumPy/scikit-learn as in the reference (step 5 runs on the GPU with ``--kmeans-restarts``);
+step 3 runs g2vec_b200.walks on the GPU and step 4 g2vec_b200.cbow.  Two documented differences: ``--epoch`` is honoured as the cap on optimizer
 steps (the reference parses it, :515, and then loops ``range(500)``, :262 -- the default 500 is the
 reference behaviour), and ``--seed`` (default 0) seeds the walk sampler, the path glue, the split and the
 initial vectors (the reference is unseeded).
@@ -62,6 +62,15 @@ stops with an ``ERROR`` after step 3, before training.  After step 6 (on rank 0 
 ``neighbors:`` line with the share of (gene, neighbour) pairs in the same L-group, and step 7 also writes
 RESULT_NAME_neighbors.txt: per searched gene, in the order of _lgroups.txt, K rows of its L-group, the rank 1..K, the
 neighbour, its L-group and the cosine, nearest first (equal cosines by the neighbour's position in _lgroups.txt).
+
+``--kmeans-restarts R`` (default 0: off, step 5 is scikit-learn's ``KMeans(3, random_state=0)`` as in the reference;
+0 <= R <= 1024) finds the L-groups on the GPU with the best of R k-means++ restarts instead (DESIGN.md §4.26): restart r
+is seeded by ``--seed`` and r, every restart runs Lloyd's iterations (at most 300) in exact float64, and the one of
+lowest inertia names the L-groups by the same rule.  Each gene's agreement is the share of restarts that put it in the
+best restart's cluster, after matching every restart's cluster labels to the best one's.  A run with fewer than 3
+common genes stops with an ``ERROR`` before step 3.  Step 5 (on rank 0 only under torchrun) prints a ``k-means:`` line,
+and step 7 also writes RESULT_NAME_kmeans.txt: per gene, in the order of _lgroups.txt, its L-group and agreement,
+followed by the same line.  Steps 6 and 7, ``--permutations`` and ``--neighbors`` use these L-groups.
 
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
@@ -148,6 +157,10 @@ def parse_arguments(argv=None):
     p.add_argument('--neighbors', type=int, default=0, metavar='K',
                    help="the K nearest genes (0 <= K <= 64) of every gene in the random paths by cosine of the "
                         "learned vectors, in RESULT_NAME_neighbors.txt; 0 (default) = off")
+    p.add_argument('--kmeans-restarts', type=int, default=0, metavar='R',
+                   help="find the L-groups with the best of R k-means++ restarts on the GPU (0 <= R <= 1024, seeded "
+                        "by --seed) and write each gene's agreement across them to RESULT_NAME_kmeans.txt; 0 (default) "
+                        "= scikit-learn's KMeans(3, random_state=0)")
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
@@ -161,6 +174,8 @@ def parse_arguments(argv=None):
         p.error("--permutations must be an integer in [0, 2^24]")
     if not 0 <= args.neighbors <= 64:
         p.error("--neighbors must be an integer in [0, 64]")
+    if not 0 <= args.kmeans_restarts <= 1024:
+        p.error("--kmeans-restarts must be an integer in [0, 1024]")
     if args.patience < 1:
         p.error("--patience must be an integer >= 1")
     if args.lr_patience < 0:
@@ -247,25 +262,14 @@ def restrict(data, network):
 
 # ------------------------------------------------------------------------------ step 5: L-groups
 def find_lgroups(mat, gene_names, geneFreq):
-    """KMeans(3, random_state=0) on the vectors; largest cluster -> 2 (other); of the remaining two
-    clusters the reference compares good/poor gene-frequency votes (G2Vec.py:167-200).  In the reference
+    """KMeans(3, random_state=0) on the vectors, named by kmeans.name_lgroups: largest cluster -> 2 (other); of the
+    remaining two clusters the reference compares good/poor gene-frequency votes (G2Vec.py:167-200).  In the reference
     ``freqIdx`` is a Python list, so ``freqIdx==0`` is the scalar False and both votes are always 0
     (:172,186-187): the outcome is therefore always good = second remaining cluster, poor = first.  That
     behaviour is reproduced here so the output files match."""
     from sklearn.cluster import KMeans
-    km = KMeans(n_clusters=3, random_state=0).fit(mat).labels_
-    sizes = [int(np.count_nonzero(km == k)) for k in range(3)]
-    largest = 0
-    for k in (1, 2):
-        if sizes[k] > sizes[largest]:
-            largest = k
-    rest = [k for k in (0, 1, 2) if k != largest]
-    poor_c, good_c = rest[0], rest[1]
-    out = np.zeros(mat.shape[0], dtype=np.int32)
-    out[km == good_c] = 0
-    out[km == poor_c] = 1
-    out[km == largest] = 2
-    return out
+    from .kmeans import name_lgroups
+    return name_lgroups(KMeans(n_clusters=3, random_state=0).fit(mat).labels_)
 
 
 # ------------------------------------------------------------------------------- step 6: scoring
@@ -324,6 +328,16 @@ def write_neighbors(prefix, genes, lgroup, sub, idx, sim):
                          for r, (j, s) in enumerate(zip(row, srow)))
 
 
+def write_kmeans(prefix, genes, res):
+    """One row per gene in the order of _lgroups.txt: its L-group and agreement (a kmeans.KMeansResult), then the
+    k-means line."""
+    from .kmeans import summary
+    with open(prefix + "_kmeans.txt", 'w') as f:
+        f.write('GeneSymbol\tLgroup(0:good,1:poor,2:other)\tAgreement\n')
+        f.writelines('%s\t%d\t%.6f\n' % (g, k, a) for g, k, a in zip(genes, res.lgroups, res.agreement))
+        f.write(summary(res) + '\n')
+
+
 def write_vectors(prefix, genes, mat):
     with open(prefix + "_vectors.txt", 'w') as f:
         f.write('GeneSymbol' + ''.join('\tV%d' % i for i in range(mat.shape[1])) + '\n')
@@ -375,6 +389,9 @@ def main(argv=None):
         except ValueError as e:
             print('ERROR: %s' % e)
             sys.exit(1)
+    if args.kmeans_restarts and n_genes < 3:
+        print('ERROR: --kmeans-restarts needs at least 3 common genes, found %d' % n_genes)
+        sys.exit(1)
 
     print('>>> 3. Generate random paths from each group')
     print('    *** most time consuming step ***')
@@ -439,7 +456,13 @@ def main(argv=None):
         return
 
     print('>>> 5. Find L-groups')
-    lgroup = find_lgroups(mat, genes, geneFreq)
+    if args.kmeans_restarts:
+        from . import kmeans
+        km = kmeans.kmeans_lgroups(mat, args.kmeans_restarts, seed=args.seed)
+        lgroup = km.lgroups
+        print('    ' + kmeans.summary(km))
+    else:
+        lgroup = find_lgroups(mat, genes, geneFreq)
 
     print(">>> 6. Select biomarkers with gene scores")
     biomarkers = []
@@ -475,6 +498,9 @@ def main(argv=None):
     if args.neighbors:
         write_neighbors(args.RESULT_NAME, genes, lgroup, in_paths, nbr_idx, nbr_sim)
         print('    %s_neighbors.txt' % args.RESULT_NAME)
+    if args.kmeans_restarts:
+        write_kmeans(args.RESULT_NAME, genes, km)
+        print('    %s_kmeans.txt' % args.RESULT_NAME)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

@@ -605,6 +605,46 @@ int g2v_nbr_merge(const int32_t *part_idx, const double *part_sim, int32_t split
                   double *sim, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Best-of-R k-means (k = 3) restarts of the L-groups (DESIGN.md §4.26; g2vec_b200/kmeans.py does the host side).
+ * W [n][D] float32 row-major, 3 <= n <= G2V_KM_MAX_GENES, D >= 1, every value finite; x_i = (double) W_i.
+ * dist(i, c) = the float64 chain acc = acc + t * t, t = x_id - c_d, d ascending from +0, every operation rounded
+ * separately (no fma).  A chunk holds R' <= G2V_KM_MAX_RESTARTS restarts in slots 0 .. R'-1; slot s is restart
+ * r_begin + s, whose seeding draws come from draw64(seed, 2^62 + r_begin + s, t).  Per slot: centres [3][D] double at
+ * [s * 3 * D], labels [n] int8 and mind [n] double at [s * n], flags (bit c: cluster c holds a row, bit 3: a label
+ * changed), state (0 running, 1 done).  `active` lists the n_active slots a launch works on.  Sums run in blocks of
+ * G2V_KM_BLOCK consecutive rows (nb = ceil(n / G2V_KM_BLOCK)): psum [R'][nb][3][D] double, pcnt [R'][nb][3] int32,
+ * pin [R'][nb] double.
+ * g2v_km_assign: kc in [1, 3] centres; mind_i = min over c < kc of dist(i, c).  With kc = 3 also labels_i = the argmin
+ *   (ties: the lower c) and the flags (integer atomics; the caller zeroes them once, g2v_km_update resets them).
+ * g2v_km_seed: k-means++ pick t in [0, 2] of every slot 0 .. R'-1 (t > 0 reads mind of the first t centres): writes
+ *   seeds [s * 3 + t] (a row) and centre t = x of that row.
+ * g2v_km_blocks: per active slot and block, the chain of x over the block's rows of each cluster, the counts and the
+ *   chain of mind.
+ * g2v_km_update: per active slot, one Lloyd decision at iteration it (1-based) of max_iter: stop (state = 1, inertia,
+ *   n_iter = it) when it == max_iter or (it > 1, no label changed and no cluster empty); otherwise the new centres
+ *   (block chains / count) with each empty cluster, in ascending c, moved to a distinct row of largest mind (ties:
+ *   the lowest row).  Resets the slot's flags.
+ * g2v_km_contingency: table [R'][3][3] int64 += #{i : labels_si = a, best_i = b} (the caller zeroes it).
+ * g2v_km_agree: count [n] int32 += #{s < R' : perm[s][labels_si] = best_i}, perm [R'][3] int8.
+ * Out-of-range sizes fail with nothing launched.  One launch each, never synchronises; no floating-point atomics. */
+#define G2V_KM_MAX_GENES (1 << 30)
+#define G2V_KM_MAX_RESTARTS 1024
+#define G2V_KM_BLOCK 256
+int g2v_km_assign(const float *W, int64_t n, int32_t D, const double *centres, int32_t kc, const int32_t *active,
+                  int32_t n_active, int8_t *labels, double *mind, int32_t *flags, void *stream);
+int g2v_km_seed(const float *W, int64_t n, int32_t D, const double *mind, uint64_t seed, int64_t r_begin, int32_t t,
+                int32_t n_slots, double *centres, int32_t *seeds, void *stream);
+int g2v_km_blocks(const float *W, const int8_t *labels, const double *mind, int64_t n, int32_t D,
+                  const int32_t *active, int32_t n_active, double *psum, int32_t *pcnt, double *pin, void *stream);
+int g2v_km_update(const float *W, const double *mind, const double *psum, const int32_t *pcnt, const double *pin,
+                  int64_t n, int32_t D, const int32_t *active, int32_t n_active, int32_t it, int32_t max_iter,
+                  int32_t *flags, double *centres, int32_t *state, double *inertia, int32_t *n_iter, void *stream);
+int g2v_km_contingency(const int8_t *labels, const int8_t *best, int64_t n, int32_t n_slots, int64_t *table,
+                       void *stream);
+int g2v_km_agree(const int8_t *labels, const int8_t *best, const int8_t *perm, int64_t n, int32_t n_slots,
+                 int32_t *count, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Between the two hot paths (SURVEY.md 8f-2): `tuple(sorted(path))` into a set (G2Vec.py:345,351) and
  * the removal of paths common to both groups (G2Vec.py:313).
  * g2v_paths_canonicalise: row i of nodes [n*L] (-1 or INT32_MAX padded) -> sorted [n*L] ascending with
