@@ -137,6 +137,13 @@ SIGNATURES = {
                                      _vp, _vp]),
     "g2v_km_contingency": (ctypes.c_int, [_vp, _vp, _i64, _i32, _vp, _vp]),
     "g2v_km_agree": (ctypes.c_int, [_vp, _vp, _vp, _i64, _i32, _vp, _vp]),
+    "g2v_tsne_workspace_bytes": (ctypes.c_size_t, [_i64]),
+    "g2v_tsne_dist": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp]),
+    "g2v_tsne_affinity": (ctypes.c_int, [_vp, _i64, ctypes.c_double, _vp, _vp, _vp]),
+    "g2v_tsne_symmetrize": (ctypes.c_int, [_vp, _i64, _vp]),
+    "g2v_tsne_grad": (ctypes.c_int, [_vp, _vp, _i64, _vp, _vp]),
+    "g2v_tsne_update": (ctypes.c_int, [_vp, _i64, _i32, ctypes.c_double, _vp, _vp, _vp, _vp]),
+    "g2v_tsne_kl": (ctypes.c_int, [_vp, _vp, _i64, _vp, _vp, _vp]),
     "g2v_paths_canonicalise": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
     "g2v_paths_mark": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "g2v_paths_set_workspace_bytes": (ctypes.c_size_t, [_i64]),

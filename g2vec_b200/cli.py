@@ -72,6 +72,14 @@ common genes stops with an ``ERROR`` before step 3.  Step 5 (on rank 0 only unde
 and step 7 also writes RESULT_NAME_kmeans.txt: per gene, in the order of _lgroups.txt, its L-group and agreement,
 followed by the same line.  Steps 6 and 7, ``--permutations`` and ``--neighbors`` use these L-groups.
 
+``--tsne P`` (default 0: off; otherwise a finite perplexity, 1 <= P <= 1000) adds an exact 2-D t-SNE map of the genes in
+paths (the same genes as ``--neighbors``) from their learned vectors, on the GPU in float64 (DESIGN.md §4.27):
+scikit-learn's exact method with its defaults (early exaggeration 12 for 250 iterations, learning rate
+max(n / 48, 50), PCA initialisation), always 1000 iterations, the same bits for the same vectors.  A run whose paths hold
+P genes or fewer, or more than 32768, stops with an ``ERROR`` after step 3, before training.  After step 6 (on rank 0
+only under torchrun) the run prints a ``t-SNE:`` line with the final KL divergence, and step 7 also writes
+RESULT_NAME_tsne.txt: per gene in paths, in the order of _lgroups.txt, its L-group and its X and Y in the map.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle`` or ``--class-weight``, at every table size (DESIGN.md §4.13); ``--class-weight 1,1`` writes the
@@ -161,6 +169,9 @@ def parse_arguments(argv=None):
                    help="find the L-groups with the best of R k-means++ restarts on the GPU (0 <= R <= 1024, seeded "
                         "by --seed) and write each gene's agreement across them to RESULT_NAME_kmeans.txt; 0 (default) "
                         "= scikit-learn's KMeans(3, random_state=0)")
+    p.add_argument('--tsne', type=float, default=0.0, metavar='P',
+                   help="an exact 2-D t-SNE map on the GPU of the genes in the random paths with perplexity P "
+                        "(1 <= P <= 1000), in RESULT_NAME_tsne.txt; 0 (default) = off")
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
@@ -176,6 +187,8 @@ def parse_arguments(argv=None):
         p.error("--neighbors must be an integer in [0, 64]")
     if not 0 <= args.kmeans_restarts <= 1024:
         p.error("--kmeans-restarts must be an integer in [0, 1024]")
+    if not (args.tsne == 0 or (np.isfinite(args.tsne) and 1.0 <= args.tsne <= 1000.0)):
+        p.error("--tsne must be 0 (off) or a finite perplexity in [1, 1000]")
     if args.patience < 1:
         p.error("--patience must be an integer >= 1")
     if args.lr_patience < 0:
@@ -338,6 +351,13 @@ def write_kmeans(prefix, genes, res):
         f.write(summary(res) + '\n')
 
 
+def write_tsne(prefix, genes, lgroup, sub, Y):
+    """One row per gene in paths (sub: their indices in genes, ascending): its L-group and its map coordinates."""
+    with open(prefix + "_tsne.txt", 'w') as f:
+        f.write('GeneSymbol\tLgroup(0:good,1:poor,2:other)\tX\tY\n')
+        f.writelines('%s\t%d\t%.6f\t%.6f\n' % (genes[g], lgroup[g], x, y) for g, (x, y) in zip(sub, Y))
+
+
 def write_vectors(prefix, genes, mat):
     with open(prefix + "_vectors.txt", 'w') as f:
         f.write('GeneSymbol' + ''.join('\tV%d' % i for i in range(mat.shape[1])) + '\n')
@@ -434,12 +454,19 @@ def main(argv=None):
     geneFreq = paths.gene_freq_dict(code, data['gene'])
     print("    n_paths : %d" % int(w_label.shape[0]))
     print("    n_genes : %d\t(genes in good or poor random paths)" % len(geneFreq))
-    if args.neighbors:
+    if args.neighbors or args.tsne:
         from . import neighbors
         in_paths = neighbors.genes_in_paths(code)     # the same on every rank: each holds the 1-GPU windows
+    if args.neighbors:
         if args.neighbors >= len(in_paths):
             print('ERROR: --neighbors %d needs more than %d genes in the random paths, found %d'
                   % (args.neighbors, args.neighbors, len(in_paths)))
+            sys.exit(1)
+    if args.tsne:
+        from . import tsne
+        if not args.tsne < len(in_paths) <= tsne.MAX_GENES:
+            print('ERROR: --tsne %g needs more than %g and at most %d genes in the random paths, found %d'
+                  % (args.tsne, args.tsne, tsne.MAX_GENES, len(in_paths)))
             sys.exit(1)
 
     print(">>> 4. Compute distributed representations using modified CBOW")
@@ -484,6 +511,9 @@ def main(argv=None):
         print("    neighbors: %d nearest genes by cosine for each of %d genes in paths; %.1f %% of the pairs share the "
               "gene's L-group" % (args.neighbors, len(in_paths),
                                   100.0 * neighbors.same_lgroup_share(lgroup[in_paths], nbr_idx)))
+    if args.tsne:
+        tsne_res = tsne.tsne_map(mat[in_paths], args.tsne, n_iter=tsne.N_ITER, seed=args.seed)
+        print('    ' + tsne.summary(len(in_paths), args.tsne, tsne.N_ITER, tsne_res.kl))
 
     print(">>> 7. Save results")
     write_biomarkers(args.RESULT_NAME, biomarkers)
@@ -501,6 +531,9 @@ def main(argv=None):
     if args.kmeans_restarts:
         write_kmeans(args.RESULT_NAME, genes, km)
         print('    %s_kmeans.txt' % args.RESULT_NAME)
+    if args.tsne:
+        write_tsne(args.RESULT_NAME, genes, lgroup, in_paths, tsne_res.Y)
+        print('    %s_tsne.txt' % args.RESULT_NAME)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

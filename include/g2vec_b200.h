@@ -645,6 +645,38 @@ int g2v_km_agree(const int8_t *labels, const int8_t *best, const int8_t *perm, i
                  int32_t *count, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Exact 2-D t-SNE of the gene vectors (DESIGN.md §4.27; g2vec_b200/tsne.py does the host side).
+ * W [m][D] float32 row-major, 2 <= m <= G2V_TSNE_MAX_GENES, D >= 1, every value finite; x_i = (double) W_i.
+ * P [m][m] double: first d, then the conditional affinities c, then the joint P.  Y, u, gains [m][2] double.
+ * nb = ceil(m / G2V_TSNE_BLOCK); ws: g2v_tsne_workspace_bytes(m) bytes (0 for an m out of range), laid out as the
+ * block partials [nb][5][m], the row chains [5][m] and the row-block chains of Z [nb].
+ * g2v_tsne_dist: d_ij = the float64 chain acc = acc + t * t, t = x_id - x_jd, d ascending from +0, every operation
+ *   rounded separately (no fma); d_ji has the bits of d_ij and d_ii = +0.
+ * g2v_tsne_affinity: per row i, scikit-learn's perplexity bisection on the row of d (1 <= perplexity < m, at most 100
+ *   evaluations, tolerance float32(1e-5) on |H - log perplexity|, a row sum of 0 taken as float32(1e-8), j = i left
+ *   out); writes beta [m] double (the beta the row was computed from), steps [m] int32 (the 0-based evaluation that
+ *   met the tolerance, 100 if none did) and overwrites the row with c_ij = exp(-d_ij beta_i) / S_i, c_ii = 0.
+ * g2v_tsne_symmetrize: in place P_ij = (c_ij + c_ji) / (2m); P is symmetric bit for bit and P_ii = 0.
+ * g2v_tsne_grad: per row i and column block b, the chains over the block's j != i (ascending) of w = 1 / (1 + d),
+ *   p_ij w t_c and w^2 t_c, t_c = y_ic - y_jc, d = t_0 t_0 + t_1 t_1, into the block partials of ws.
+ * g2v_tsne_update: iteration it >= 0 from the partials of g2v_tsne_grad at the current Y: per row the chains of the
+ *   block partials, Z = the chain of Z_i in blocks of 256 rows, g = 4 ((alpha A) - (R / Z)), then scikit-learn's gains
+ *   (+0.2 / *0.8, at least 0.01), momentum and step with learning rate eta > 0 (alpha = 12, momentum 0.5 for it < 250,
+ *   else 1 and 0.8; u and the gains start over at 0 and 1 at it = 0 and it = 250).
+ * g2v_tsne_kl: kl [1] double = sum over i != j of p_ij log(max(p_ij, eps) / max(w_ij / Z, eps)) at Y, in a fixed
+ *   order (overwrites ws).
+ * Out-of-range sizes fail with nothing launched.  Never synchronises; no atomics, no tensor cores. */
+#define G2V_TSNE_MAX_GENES 32768
+#define G2V_TSNE_BLOCK 256
+size_t g2v_tsne_workspace_bytes(int64_t m);
+int g2v_tsne_dist(const float *W, int64_t m, int32_t D, double *P, void *stream);
+int g2v_tsne_affinity(double *P, int64_t m, double perplexity, double *beta, int32_t *steps, void *stream);
+int g2v_tsne_symmetrize(double *P, int64_t m, void *stream);
+int g2v_tsne_grad(const double *P, const double *Y, int64_t m, double *ws, void *stream);
+int g2v_tsne_update(double *ws, int64_t m, int32_t it, double eta, double *Y, double *u, double *gains, void *stream);
+int g2v_tsne_kl(const double *P, const double *Y, int64_t m, double *ws, double *kl, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Between the two hot paths (SURVEY.md 8f-2): `tuple(sorted(path))` into a set (G2Vec.py:345,351) and
  * the removal of paths common to both groups (G2Vec.py:313).
  * g2v_paths_canonicalise: row i of nodes [n*L] (-1 or INT32_MAX padded) -> sorted [n*L] ascending with
