@@ -144,7 +144,12 @@ SIGNATURES = {
     "g2v_tsne_grad": (ctypes.c_int, [_vp, _vp, _i64, _vp, _vp]),
     "g2v_tsne_update": (ctypes.c_int, [_vp, _i64, _i32, ctypes.c_double, _vp, _vp, _vp, _vp]),
     "g2v_tsne_kl": (ctypes.c_int, [_vp, _vp, _i64, _vp, _vp, _vp]),
-    "g2v_paths_canonicalise": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
+    "g2v_gsea_keys": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "g2v_gsea_rank_workspace_bytes": (ctypes.c_size_t, [_i64, _i32]),
+    "g2v_gsea_rank": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, ctypes.c_size_t, _vp]),
+    "g2v_gsea_es": (ctypes.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _i32, _i32, _vp, _vp]),
+    "g2v_gsea_norm": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "g2v_paths_canonicalise":(ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
     "g2v_paths_mark": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "g2v_paths_set_workspace_bytes": (ctypes.c_size_t, [_i64]),
     "g2v_paths_set_select": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp]),

@@ -80,6 +80,18 @@ P genes or fewer, or more than 32768, stops with an ``ERROR`` after step 3, befo
 only under torchrun) the run prints a ``t-SNE:`` line with the final KL divergence, and step 7 also writes
 RESULT_NAME_tsne.txt: per gene in paths, in the order of _lgroups.txt, its L-group and its X and Y in the map.
 
+``--gene-sets FILE`` (default off) adds gene-set enrichment of the good / poor contrast, phenotype-permutation GSEA
+(Subramanian et al. 2005) on the GPU (DESIGN.md §4.28), for the sets of the GMT file FILE (one set per line: name,
+description, genes, tab-separated).  The ranking metric is each gene's point-biserial correlation with the poor label
+(label 1), the weight its absolute value; ``--gene-set-permutations B`` (default 1000, 1 <= B <= 2^20) label
+permutations, seeded by ``--seed`` and the same as ``--permutations`` makes for the same B, give each set its ES, NES,
+nominal P, FDR q and FWER p.  ``--gene-set-size MIN,MAX`` (default 15,500; 1 <= MIN <= MAX <= 4096) keeps the sets
+with MIN to MAX genes in the analysis (the common genes of step 2).  The file and the inputs are checked after step 2,
+where the run prints a ``gene sets:`` line or stops with an ``ERROR``; after step 6 (on rank 0 only under torchrun) it
+prints a ``gene-set test:`` line, and step 7 also writes RESULT_NAME_gsea.txt: per kept set, in the file's order, its
+size, ES, NES, P, FDR_Q, FWER_P (``nan`` when the needed side of the null is empty), how many of its genes are
+biomarkers, and its leading-edge genes in rank order.  None of these depend on training.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle`` or ``--class-weight``, at every table size (DESIGN.md §4.13); ``--class-weight 1,1`` writes the
@@ -172,6 +184,14 @@ def parse_arguments(argv=None):
     p.add_argument('--tsne', type=float, default=0.0, metavar='P',
                    help="an exact 2-D t-SNE map on the GPU of the genes in the random paths with perplexity P "
                         "(1 <= P <= 1000), in RESULT_NAME_tsne.txt; 0 (default) = off")
+    p.add_argument('--gene-sets', type=str, default=None, metavar='FILE',
+                   help="gene-set enrichment (phenotype-permutation GSEA) of the good / poor contrast for the sets "
+                        "of the GMT file FILE, in RESULT_NAME_gsea.txt; default off")
+    p.add_argument('--gene-set-permutations', type=int, default=1000, metavar='B',
+                   help="with --gene-sets: label permutations of the gene-set test, 1 <= B <= 2^20 (default 1000)")
+    p.add_argument('--gene-set-size', type=str, default='15,500', metavar='MIN,MAX',
+                   help="with --gene-sets: keep the sets with MIN to MAX genes in the analysis, 1 <= MIN <= MAX <= "
+                        "4096 (default 15,500)")
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
@@ -183,6 +203,9 @@ def parse_arguments(argv=None):
         p.error("--weight-decay must be a finite number with 0 <= weight-decay < 1")
     if not 0 <= args.permutations <= 1 << 24:
         p.error("--permutations must be an integer in [0, 2^24]")
+    if not 1 <= args.gene_set_permutations <= 1 << 20:
+        p.error("--gene-set-permutations must be an integer in [1, 2^20]")
+    args.gene_set_size = _parse_gene_set_size(args.gene_set_size, p)
     if not 0 <= args.neighbors <= 64:
         p.error("--neighbors must be an integer in [0, 64]")
     if not 0 <= args.kmeans_restarts <= 1024:
@@ -221,6 +244,17 @@ def _parse_class_weight(text, p):
     if w is None or not all(np.isfinite(x) and x > 0 for x in w):
         p.error("--class-weight must be 'balanced' or W0,W1: two numbers that are finite and > 0 in float32")
     return tuple(float(x) for x in w)
+
+
+def _parse_gene_set_size(text, p):
+    """'MIN,MAX' -> (MIN, MAX), two integers with 1 <= MIN <= MAX <= 4096; anything else is p.error."""
+    try:
+        lo, hi = (int(x) for x in text.split(','))
+    except ValueError:
+        lo = hi = 0
+    if not 1 <= lo <= hi <= 4096:
+        p.error("--gene-set-size must be MIN,MAX: two integers with 1 <= MIN <= MAX <= 4096")
+    return lo, hi
 
 
 # ----------------------------------------------------------------------------------- step 1: I/O
@@ -358,6 +392,18 @@ def write_tsne(prefix, genes, lgroup, sub, Y):
         f.writelines('%s\t%d\t%.6f\t%.6f\n' % (genes[g], lgroup[g], x, y) for g, (x, y) in zip(sub, Y))
 
 
+def write_gsea(prefix, genes, res, biomarkers):
+    """One row per kept gene set (a gsea.GseaResult): size, ES, NES, P, FDR_Q, FWER_P, how many of its genes are
+    biomarkers, and its leading-edge genes in rank order, comma-separated."""
+    bm = set(biomarkers)
+    with open(prefix + "_gsea.txt", 'w') as f:
+        f.write('GeneSet\tSize\tES\tNES\tP\tFDR_Q\tFWER_P\tBiomarkers\tLeadingEdge\n')
+        for i, name in enumerate(res.name):
+            f.write('%s\t%d\t%.6f\t%.6f\t%.6g\t%.6g\t%.6g\t%d\t%s\n'
+                    % (name, res.size[i], res.ES[i], res.NES[i], res.P[i], res.FDR[i], res.FWER[i],
+                       sum(genes[g] in bm for g in res.members[i]), ','.join(genes[g] for g in res.leading_edge[i])))
+
+
 def write_vectors(prefix, genes, mat):
     with open(prefix + "_vectors.txt", 'w') as f:
         f.write('GeneSymbol' + ''.join('\tV%d' % i for i in range(mat.shape[1])) + '\n')
@@ -409,6 +455,17 @@ def main(argv=None):
         except ValueError as e:
             print('ERROR: %s' % e)
             sys.exit(1)
+    if args.gene_sets is not None:
+        from .gsea import check_inputs as gsea_check, read_gmt, restrict_sets
+        try:                                           # fail now rather than after training
+            gmt = read_gmt(args.gene_sets)
+            set_ptr, _, set_names = restrict_sets(gmt, data['gene'], *args.gene_set_size)
+            gsea_check(data['expr'], data['label'], args.gene_set_permutations, len(set_names), *args.gene_set_size)
+        except (OSError, ValueError) as e:
+            print('ERROR: --gene-sets: %s' % e)
+            sys.exit(1)
+        print('    gene sets: %d of %d in %s with %d..%d genes in the analysis'
+              % (len(set_names), len(gmt), args.gene_sets, args.gene_set_size[0], args.gene_set_size[1]))
     if args.kmeans_restarts and n_genes < 3:
         print('ERROR: --kmeans-restarts needs at least 3 common genes, found %d' % n_genes)
         sys.exit(1)
@@ -515,6 +572,12 @@ def main(argv=None):
         tsne_res = tsne.tsne_map(mat[in_paths], args.tsne, n_iter=tsne.N_ITER, seed=args.seed)
         print('    ' + tsne.summary(len(in_paths), args.tsne, tsne.N_ITER, tsne_res.kl))
 
+    if args.gene_sets is not None:
+        from .gsea import gsea as gsea_test, summary as gsea_summary
+        gsea_res = gsea_test(data['expr'], data['label'], gmt, args.gene_set_permutations, seed=args.seed,
+                             min_size=args.gene_set_size[0], max_size=args.gene_set_size[1], genes=genes)
+        print('    ' + gsea_summary(gsea_res))
+
     print(">>> 7. Save results")
     write_biomarkers(args.RESULT_NAME, biomarkers)
     print('    %s_biomarkers.txt' % args.RESULT_NAME)
@@ -534,6 +597,9 @@ def main(argv=None):
     if args.tsne:
         write_tsne(args.RESULT_NAME, genes, lgroup, in_paths, tsne_res.Y)
         print('    %s_tsne.txt' % args.RESULT_NAME)
+    if args.gene_sets is not None:
+        write_gsea(args.RESULT_NAME, genes, gsea_res, biomarkers)
+        print('    %s_gsea.txt' % args.RESULT_NAME)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

@@ -677,6 +677,46 @@ int g2v_tsne_update(double *ws, int64_t m, int32_t it, double eta, double *Y, do
 int g2v_tsne_kl(const double *P, const double *Y, int64_t m, double *ws, double *kl, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Phenotype-permutation gene-set enrichment (GSEA) of the good / poor contrast (DESIGN.md §4.28; g2vec_b200/gsea.py
+ * does the host side).  A row is one labelling (the observed one, or a permutation from g2v_perm_labels) with its
+ * exact sums A [n_b][G] from g2v_perm_sums over the genes in their input order; n, k, Q, W as for g2v_perm_tally, and
+ * s = +1 when the selected group is label 1, -1 when it is label 0.  2 <= G <= G2V_GSEA_MAX_GENES, 1 <= n_b <=
+ * G2V_GSEA_MAX_ROWS with n_b * G < 2^31.
+ * g2v_gsea_keys: per row and gene N = n A - k Q, r = (double)(s N) / sqrt(W) (+0 when W = 0), rq = rint(r 2^32);
+ *   u [n_b][G] = |rq| and key [n_b][G] = ((2^32 - rq) << 20) | g: ascending keys order a row by rq descending, ties
+ *   by gene ascending.
+ * g2v_gsea_rank: pos [n_b][G] int32 = the 0-based rank of each gene in its row's key order.  workspace:
+ *   g2v_gsea_rank_workspace_bytes(n_b, G) bytes of device scratch (0 for sizes out of range).
+ * g2v_gsea_es: es [n_b][n_sets] = the enrichment score of every set in every row.  The sets are CSR over the genes:
+ *   set_ptr [n_sets + 1], set_gene [set_ptr[n_sets]] (distinct genes per set); max_k >= the largest set, 1 <= max_k
+ *   <= min(G2V_GSEA_MAX_SET_SIZE, G - 1).  With the members' ranks sorted, p_1 < ... < p_k, their weights u_j,
+ *   S_j = u_1 + ... + u_j (exact), N_R = S_k and m_j = p_j - (j - 1):
+ *     D+ = max(0, max_j (S_j / N_R - m_j / (G - k))),  D- = min(0, min_j (S_(j-1) / N_R - m_j / (G - k))),
+ *   each term three correctly rounded float64 operations; ES = D+ if D+ >= -D-, else D-; +0 when N_R = 0.
+ * g2v_gsea_norm: es [B][n_sets] of the permutations and es_obs [n_sets] of the observed labelling -> per set
+ *   mean_pos = the mean of the es >= 0 and mean_neg = the mean of |es| over es < 0 (float64 sums in b order; NaN when
+ *   empty), nes_obs = es_obs / mean_pos (es_obs >= 0) or es_obs / mean_neg, NaN when that side is empty; nes [B][n_sets]
+ *   = each es over the mean of its own side, or NaN for the whole column of a set whose nes_obs is NaN; counts
+ *   [3][n_sets] int64 = #{b: es >= 0}, #{b: es < 0} and #{b: es >= es_obs} (es_obs >= 0) or #{b: es <= es_obs}.
+ *   B * n_sets <= G2V_GSEA_MAX_ES.
+ * Out-of-range sizes fail with nothing launched.  Never synchronises; no floating-point atomics. */
+#define G2V_GSEA_MAX_GENES (1 << 20)
+#define G2V_GSEA_MAX_ROWS 65535
+#define G2V_GSEA_MAX_SETS (1 << 28)
+#define G2V_GSEA_MAX_SET_SIZE 4096
+#define G2V_GSEA_MAX_PERMUTATIONS (1 << 20)
+#define G2V_GSEA_MAX_ES (1 << 28)
+int g2v_gsea_keys(const int64_t *A, int64_t n_b, int32_t G, int32_t n, int32_t k, int32_t s, const int64_t *Q,
+                  const double *W, uint64_t *key, uint64_t *u, void *stream);
+size_t g2v_gsea_rank_workspace_bytes(int64_t n_b, int32_t G);
+int g2v_gsea_rank(const uint64_t *key, int64_t n_b, int32_t G, int32_t *pos, void *workspace, size_t workspace_bytes,
+                  void *stream);
+int g2v_gsea_es(const int32_t *pos, const uint64_t *u, int64_t n_b, int32_t G, const int32_t *set_ptr,
+                const int32_t *set_gene, int32_t n_sets, int32_t max_k, double *es, void *stream);
+int g2v_gsea_norm(const double *es, int64_t B, int32_t n_sets, const double *es_obs, double *nes, double *mean_pos,
+                  double *mean_neg, double *nes_obs, int64_t *counts, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Between the two hot paths (SURVEY.md 8f-2): `tuple(sorted(path))` into a set (G2Vec.py:345,351) and
  * the removal of paths common to both groups (G2Vec.py:313).
  * g2v_paths_canonicalise: row i of nodes [n*L] (-1 or INT32_MAX padded) -> sorted [n*L] ascending with
