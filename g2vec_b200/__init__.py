@@ -10,6 +10,7 @@ from .neighbors import nearest_genes  # noqa: F401
 from .kmeans import kmeans_lgroups  # noqa: F401
 from .tsne import tsne_map  # noqa: F401
 from .gsea import gsea, read_gmt  # noqa: F401
+from .signature import signature_cv  # noqa: F401
 from . import graph, paths  # noqa: F401
 
 __version__ = "0.1.0"

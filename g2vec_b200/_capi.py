@@ -149,6 +149,12 @@ SIGNATURES = {
     "g2v_gsea_rank": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, ctypes.c_size_t, _vp]),
     "g2v_gsea_es": (ctypes.c_int, [_vp, _vp, _i64, _i32, _vp, _vp, _i32, _i32, _vp, _vp]),
     "g2v_gsea_norm": (ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "g2v_sig_folds": (ctypes.c_int, [_vp, _i32, _i32, _i32, _u64, _vp, _vp]),
+    "g2v_sig_draw": (ctypes.c_int, [_i32, _i32, _u64, _i64, _i64, _vp, _vp]),
+    "g2v_sig_fit_smem_bytes": (ctypes.c_size_t, [_i32]),
+    "g2v_sig_fit": (ctypes.c_int, [_vp, _i32, _i32, _i64, _vp, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp,
+                                   _i32, _vp]),
+    "g2v_sig_auc": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "g2v_paths_canonicalise":(ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
     "g2v_paths_mark": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "g2v_paths_set_workspace_bytes": (ctypes.c_size_t, [_i64]),

@@ -92,6 +92,21 @@ prints a ``gene-set test:`` line, and step 7 also writes RESULT_NAME_gsea.txt: p
 size, ES, NES, P, FDR_Q, FWER_P (``nan`` when the needed side of the null is empty), how many of its genes are
 biomarkers, and its leading-edge genes in rank order.  None of these depend on training.
 
+``--signature-cv R`` (default 0: off; 0 <= R <= 65536) adds a cross-validated test of whether the biomarkers predict
+the good / poor label, on the GPU (DESIGN.md §4.29): ridge logistic regression (scikit-learn's
+``LogisticRegression(C=1.0)`` objective, features standardised on each training fold) over ``--signature-repeats K``
+(default 10, 1 <= K <= 100) repeats of stratified ``--signature-folds F``-fold splits (default 5, 2 <= F <= 100, and F
+at most the number of samples of either label), the same splits for every signature.  The biomarkers are compared with
+the same number of genes of largest |t| (``top_t``) and with R random signatures of that size (Floyd's sampling, seeded
+by ``--seed``).  The biomarkers and ``top_t`` were both chosen with every sample's label, so their AUCs are optimistic
+and comparable with each other; the random signatures are not selected, and P_random = (1 + #{random AUC >= AUC}) /
+(R + 1) says how often one does at least as well.  Nested re-selection (the walks and the training rerun inside every
+fold) is not done.  It needs ``-n`` <= 64 (at most 128 biomarkers).  The inputs are checked after step 2, where the run
+stops with an ``ERROR`` if they are refused; after step 6 (on rank 0 only under torchrun) it prints a ``signature CV:``
+line, and step 7 also writes RESULT_NAME_signature.txt: per signature (biomarkers, top_t, random_1 .. random_R) its
+size, mean AUC over the K F fits, the SD of the K per-repeat AUCs, mean accuracy, P_random (``nan`` on random rows)
+and how many of its genes are biomarkers.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle`` or ``--class-weight``, at every table size (DESIGN.md §4.13); ``--class-weight 1,1`` writes the
@@ -192,6 +207,13 @@ def parse_arguments(argv=None):
     p.add_argument('--gene-set-size', type=str, default='15,500', metavar='MIN,MAX',
                    help="with --gene-sets: keep the sets with MIN to MAX genes in the analysis, 1 <= MIN <= MAX <= "
                         "4096 (default 15,500)")
+    p.add_argument('--signature-cv', type=int, default=0, metavar='R',
+                   help="cross-validated AUC of the biomarkers against the top-|t| genes and R random signatures of "
+                        "the same size (0 <= R <= 65536), in RESULT_NAME_signature.txt; 0 (default) = off")
+    p.add_argument('--signature-folds', type=int, default=5, metavar='F',
+                   help="with --signature-cv: stratified folds per repeat, 2 <= F <= 100 (default 5)")
+    p.add_argument('--signature-repeats', type=int, default=10, metavar='K',
+                   help="with --signature-cv: repeats of the fold split, 1 <= K <= 100 (default 10)")
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
@@ -206,6 +228,14 @@ def parse_arguments(argv=None):
     if not 1 <= args.gene_set_permutations <= 1 << 20:
         p.error("--gene-set-permutations must be an integer in [1, 2^20]")
     args.gene_set_size = _parse_gene_set_size(args.gene_set_size, p)
+    if not 0 <= args.signature_cv <= 1 << 16:
+        p.error("--signature-cv must be an integer in [0, 65536]")
+    if not 2 <= args.signature_folds <= 100:
+        p.error("--signature-folds must be an integer in [2, 100]")
+    if not 1 <= args.signature_repeats <= 100:
+        p.error("--signature-repeats must be an integer in [1, 100]")
+    if args.signature_cv and args.numBiomarker > 64:
+        p.error("--signature-cv needs -n <= 64: a signature has at most 128 genes")
     if not 0 <= args.neighbors <= 64:
         p.error("--neighbors must be an integer in [0, 64]")
     if not 0 <= args.kmeans_restarts <= 1024:
@@ -404,6 +434,19 @@ def write_gsea(prefix, genes, res, biomarkers):
                        sum(genes[g] in bm for g in res.members[i]), ','.join(genes[g] for g in res.leading_edge[i])))
 
 
+def write_signature(prefix, genes, res, biomarkers):
+    """One row per signature of a signature.SignatureResult: size, AUC, AUC_SD, accuracy, P_random (nan on the random
+    rows) and how many of its genes are biomarkers."""
+    bm = set(biomarkers)
+    p_random = list(res.p_random) + [float("nan")] * (len(res.names) - 2)
+    with open(prefix + "_signature.txt", 'w') as f:
+        f.write('Signature\tSize\tAUC\tAUC_SD\tAccuracy\tP_random\tBiomarkers\n')
+        for i, name in enumerate(res.names):
+            f.write('%s\t%d\t%.6f\t%.6f\t%.6f\t%.6g\t%d\n'
+                    % (name, res.genes.shape[1], res.auc_mean[i], res.auc_sd[i], res.acc_mean[i], p_random[i],
+                       sum(genes[g] in bm for g in res.genes[i])))
+
+
 def write_vectors(prefix, genes, mat):
     with open(prefix + "_vectors.txt", 'w') as f:
         f.write('GeneSymbol' + ''.join('\tV%d' % i for i in range(mat.shape[1])) + '\n')
@@ -466,6 +509,14 @@ def main(argv=None):
             sys.exit(1)
         print('    gene sets: %d of %d in %s with %d..%d genes in the analysis'
               % (len(set_names), len(gmt), args.gene_sets, args.gene_set_size[0], args.gene_set_size[1]))
+    if args.signature_cv:
+        from . import signature
+        try:                                           # fail now rather than after training
+            signature.check_inputs(data['expr'], data['label'], min(2 * args.numBiomarker, n_genes), args.signature_cv,
+                                   args.signature_folds, args.signature_repeats)
+        except ValueError as e:
+            print('ERROR: --signature-cv: %s' % e)
+            sys.exit(1)
     if args.kmeans_restarts and n_genes < 3:
         print('ERROR: --kmeans-restarts needs at least 3 common genes, found %d' % n_genes)
         sys.exit(1)
@@ -578,6 +629,13 @@ def main(argv=None):
                              min_size=args.gene_set_size[0], max_size=args.gene_set_size[1], genes=genes)
         print('    ' + gsea_summary(gsea_res))
 
+    if args.signature_cv:
+        pos = {g: i for i, g in enumerate(genes)}
+        sig_res = signature.signature_cv(data['expr'], data['label'], np.array([pos[g] for g in biomarkers]),
+                                         args.signature_cv, folds=args.signature_folds,
+                                         repeats=args.signature_repeats, seed=args.seed)
+        print('    ' + signature.summary(sig_res))
+
     print(">>> 7. Save results")
     write_biomarkers(args.RESULT_NAME, biomarkers)
     print('    %s_biomarkers.txt' % args.RESULT_NAME)
@@ -600,6 +658,9 @@ def main(argv=None):
     if args.gene_sets is not None:
         write_gsea(args.RESULT_NAME, genes, gsea_res, biomarkers)
         print('    %s_gsea.txt' % args.RESULT_NAME)
+    if args.signature_cv:
+        write_signature(args.RESULT_NAME, genes, sig_res, biomarkers)
+        print('    %s_signature.txt' % args.RESULT_NAME)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

@@ -717,6 +717,45 @@ int g2v_gsea_norm(const double *es, int64_t B, int32_t n_sets, const double *es_
                   double *mean_neg, double *nes_obs, int64_t *counts, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Cross-validated prediction of the good / poor label from a gene signature (DESIGN.md §4.29; g2vec_b200/signature.py
+ * does the host side).  n samples (3 <= n <= G2V_SIG_MAX_SAMPLES) with y [n] in {0, 1}; K repeats (1 <= K <=
+ * G2V_SIG_MAX_REPEATS) of stratified F-fold splits (2 <= F <= G2V_SIG_MAX_FOLDS); signatures of p sorted distinct gene
+ * indices (1 <= p <= min(G2V_SIG_MAX_SIZE, G)).  A fit is (signature s, repeat k, fold f), numbered (s K + k) F + f.
+ * g2v_sig_folds: fold [K][n] int8.  For repeat k and class c the class's samples in ascending order are Fisher-Yates
+ *   shuffled (draw s swaps position m-1-s with umulhi(draw64(seed, 2^61 + 2k + c, s), m - s)); the sample at shuffled
+ *   position t goes to fold t mod F.  F <= n / 2 (the caller keeps F <= min(n0, n1)).
+ * g2v_sig_draw: genes [count][p] int32 for random signatures r = r_begin .. r_begin + count - 1 (1 <= r <=
+ *   G2V_SIG_MAX_RANDOM): Floyd's sampling with u_t = draw64(seed, 2^61 + 2^40 + r, t), j = G - p + t,
+ *   v = umulhi(u_t, j + 1), v if new else j; sorted ascending.
+ * g2v_sig_fit: one fit per CTA.  X [G][n_pad] float64 (gene-major, n_pad >= n); genes [n_sig][p].  Per fit, on the
+ *   samples outside fold f: each feature standardised by the training mean and population SD (mu = the value, SD = 1
+ *   for a feature whose training values are all equal), then the ridge logistic loss sum log(1 + e^eta) - y eta +
+ *   |beta|^2 / 2 (intercept unpenalised) minimised by damped Newton from 0: Cholesky solve of H d = g, Armijo halving
+ *   (at most 40) with constant 1e-4, stop after the step with max |t d| <= 1e-10, at most 100 iterations.
+ *   scores [n_sig][K][n] = the out-of-fold logit of every sample; n_iter and converged [n_sig * K * F]; beta
+ *   [beta_rows][K][F][p + 1] (intercept first) for the first beta_rows signatures (beta may be NULL when 0).
+ *   g2v_sig_fit_smem_bytes(p): the fit kernel's dynamic shared memory (0 for p out of range).
+ * g2v_sig_auc: per fit over its test fold, auc = (2 #{pos > neg} + #{pos == neg}) / (2 n_pos n_neg) and acc =
+ *   #{(score > 0) == y} / n_test, from exact integer counts.  cap >= the largest test fold (shared memory of cap
+ *   doubles); a fold larger than cap gets NaN.
+ * n_sig K F <= G2V_SIG_MAX_FITS.  Out-of-range sizes fail with nothing launched.  Never synchronises; no floating-point
+ * atomics. */
+#define G2V_SIG_MAX_SAMPLES 32768
+#define G2V_SIG_MAX_SIZE 128
+#define G2V_SIG_MAX_FOLDS 100
+#define G2V_SIG_MAX_REPEATS 100
+#define G2V_SIG_MAX_RANDOM 65536
+#define G2V_SIG_MAX_FITS (1 << 24)
+int g2v_sig_folds(const uint8_t *y, int32_t n, int32_t K, int32_t F, uint64_t seed, int8_t *fold, void *stream);
+int g2v_sig_draw(int32_t G, int32_t p, uint64_t seed, int64_t r_begin, int64_t count, int32_t *genes, void *stream);
+size_t g2v_sig_fit_smem_bytes(int32_t p);
+int g2v_sig_fit(const double *X, int32_t G, int32_t n, int64_t n_pad, const uint8_t *y, const int8_t *fold, int32_t K,
+                int32_t F, const int32_t *genes, int32_t n_sig, int32_t p, double *scores, int32_t *n_iter,
+                uint8_t *converged, double *beta, int32_t beta_rows, void *stream);
+int g2v_sig_auc(const double *scores, const uint8_t *y, const int8_t *fold, int32_t n, int32_t K, int32_t F,
+                int32_t n_sig, int32_t cap, double *auc, double *acc, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Between the two hot paths (SURVEY.md 8f-2): `tuple(sorted(path))` into a set (G2Vec.py:345,351) and
  * the removal of paths common to both groups (G2Vec.py:313).
  * g2v_paths_canonicalise: row i of nodes [n*L] (-1 or INT32_MAX padded) -> sorted [n*L] ascending with
