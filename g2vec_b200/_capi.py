@@ -155,6 +155,9 @@ SIGNATURES = {
     "g2v_sig_fit": (ctypes.c_int, [_vp, _i32, _i32, _i64, _vp, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp,
                                    _i32, _vp]),
     "g2v_sig_auc": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "g2v_dcx_sums": (ctypes.c_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
+                                    _vp, _vp, _vp]),
+    "g2v_dcx_tally": (ctypes.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp]),
     "g2v_paths_canonicalise":(ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
     "g2v_paths_mark": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "g2v_paths_set_workspace_bytes": (ctypes.c_size_t, [_i64]),

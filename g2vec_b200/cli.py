@@ -107,6 +107,19 @@ line, and step 7 also writes RESULT_NAME_signature.txt: per signature (biomarker
 size, mean AUC over the K F fits, the SD of the K per-repeat AUCs, mean accuracy, P_random (``nan`` on random rows)
 and how many of its genes are biomarkers.
 
+``--diff-coexpression B`` (default 0: off; 1 <= B <= 2^20) adds a label-permutation test of differential co-expression
+for every pair of genes joined in the network, on the GPU (DESIGN.md §4.30): the pairs are the distinct unordered
+gene pairs of step 2's edges (self-loops dropped, direction and duplicates collapsed), and each pair's Pearson
+correlations over the good and the poor samples are compared by Fisher's z.  The test is always Pearson, whatever
+``--correlation`` chose for step 3's graphs.  B label permutations, seeded by ``--seed`` and the same as
+``--permutations`` makes for the same B, give each pair a raw P, Westfall & Young's step-down maxT P_maxT over the
+pairs and the Benjamini-Hochberg Q.  The inputs are checked after step 2 (at least 4 samples of each label, at most
+32768 in all, finite expression values, 1 to 2^26 pairs), where the run stops with an ``ERROR`` if they are refused;
+after step 6 (on rank 0 only under torchrun) it prints a ``differential co-expression:`` line (the last two counts are
+over the pairs with Q <= 0.05), and step 7 also writes RESULT_NAME_diffcoex.txt: per pair, ordered by the two genes'
+positions in _lgroups.txt, R_good, R_poor, Z, P, P_maxT, Q, whether step 3 kept the pair in the good and in the poor
+graph (either direction), and how many of its two genes are biomarkers.  None of these depend on training.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle`` or ``--class-weight``, at every table size (DESIGN.md §4.13); ``--class-weight 1,1`` writes the
@@ -214,6 +227,10 @@ def parse_arguments(argv=None):
                    help="with --signature-cv: stratified folds per repeat, 2 <= F <= 100 (default 5)")
     p.add_argument('--signature-repeats', type=int, default=10, metavar='K',
                    help="with --signature-cv: repeats of the fold split, 1 <= K <= 100 (default 10)")
+    p.add_argument('--diff-coexpression', type=int, default=0, metavar='B',
+                   help="label-permutation test of differential co-expression (Pearson, Fisher's z) of every gene pair "
+                        "of the network with B permutations (1 <= B <= 2^20): raw, step-down maxT and "
+                        "Benjamini-Hochberg p-values in RESULT_NAME_diffcoex.txt; 0 (default) = off")
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
@@ -228,6 +245,8 @@ def parse_arguments(argv=None):
     if not 1 <= args.gene_set_permutations <= 1 << 20:
         p.error("--gene-set-permutations must be an integer in [1, 2^20]")
     args.gene_set_size = _parse_gene_set_size(args.gene_set_size, p)
+    if not 0 <= args.diff_coexpression <= 1 << 20:
+        p.error("--diff-coexpression must be an integer in [0, 2^20]")
     if not 0 <= args.signature_cv <= 1 << 16:
         p.error("--signature-cv must be an integer in [0, 65536]")
     if not 2 <= args.signature_folds <= 100:
@@ -447,6 +466,18 @@ def write_signature(prefix, genes, res, biomarkers):
                        sum(genes[g] in bm for g in res.genes[i])))
 
 
+def write_diffcoex(prefix, genes, res, in_good, in_poor, biomarkers):
+    """One row per pair of a diffcoex.DiffCoexResult in pair order: R_good, R_poor, Z, P, P_maxT, Q, whether the pair is
+    in step 3's good and poor graphs (0/1), and how many of its genes are biomarkers (0..2)."""
+    with open(prefix + "_diffcoex.txt", 'w') as f:
+        f.write('Gene1\tGene2\tR_good\tR_poor\tZ\tP\tP_maxT\tQ\tInGood\tInPoor\tBiomarkers\n')
+        f.writelines('%s\t%s\t%.6f\t%.6f\t%.6f\t%.6g\t%.6g\t%.6g\t%d\t%d\t%d\n'
+                     % (genes[i], genes[j], rg, rp, z, pv, pm, qv, a, b, c)
+                     for (i, j), rg, rp, z, pv, pm, qv, a, b, c
+                     in zip(res.pairs, res.R_good, res.R_poor, res.Z, res.P, res.P_maxT, res.Q, in_good, in_poor,
+                            biomarkers))
+
+
 def write_vectors(prefix, genes, mat):
     with open(prefix + "_vectors.txt", 'w') as f:
         f.write('GeneSymbol' + ''.join('\tV%d' % i for i in range(mat.shape[1])) + '\n')
@@ -517,6 +548,17 @@ def main(argv=None):
         except ValueError as e:
             print('ERROR: --signature-cv: %s' % e)
             sys.exit(1)
+    if args.diff_coexpression:
+        from . import diffcoex
+        try:                                           # fail now rather than after training
+            gi = {g: i for i, g in enumerate(data['gene'])}
+            dcx_pairs = diffcoex.pairs_from_edges([gi[e[0]] for e in network['edge']],
+                                                  [gi[e[1]] for e in network['edge']])
+            diffcoex.check_inputs(data['expr'], data['label'], dcx_pairs, args.diff_coexpression)
+        except ValueError as e:
+            print('ERROR: --diff-coexpression: %s' % e)
+            sys.exit(1)
+        dcx_in_graph = []
     if args.kmeans_restarts and n_genes < 3:
         print('ERROR: --kmeans-restarts needs at least 3 common genes, found %d' % n_genes)
         sys.exit(1)
@@ -543,6 +585,8 @@ def main(argv=None):
     for i, _group in enumerate(['g', 'p']):
         rp, col, w = graph.group_csr_gpu(data['expr'], data['label'], i, src, dst, threshold=args.min_corr,
                                          method=args.correlation)
+        if args.diff_coexpression:                     # which pairs this group's graph kept, either direction
+            dcx_in_graph.append(diffcoex.graph_pairs(dcx_pairs, n_genes, rp.cpu().numpy(), col.cpu().numpy()))
         wg = walks.WalkGraph(rp, col, weights=w)
         sl = slice(i * n_total, (i + 1) * n_total)
         if dist is None:
@@ -636,6 +680,13 @@ def main(argv=None):
                                          repeats=args.signature_repeats, seed=args.seed)
         print('    ' + signature.summary(sig_res))
 
+    if args.diff_coexpression:
+        dcx_res = diffcoex.diffcoex_test(data['expr'], data['label'], dcx_pairs, args.diff_coexpression, seed=args.seed)
+        bm = set(biomarkers)
+        is_bm = np.array([g in bm for g in genes], dtype=np.int64)
+        dcx_bm = is_bm[dcx_pairs[:, 0]] + is_bm[dcx_pairs[:, 1]]
+        print('    ' + diffcoex.summary(dcx_res, dcx_in_graph[0], dcx_in_graph[1], dcx_bm))
+
     print(">>> 7. Save results")
     write_biomarkers(args.RESULT_NAME, biomarkers)
     print('    %s_biomarkers.txt' % args.RESULT_NAME)
@@ -661,6 +712,9 @@ def main(argv=None):
     if args.signature_cv:
         write_signature(args.RESULT_NAME, genes, sig_res, biomarkers)
         print('    %s_signature.txt' % args.RESULT_NAME)
+    if args.diff_coexpression:
+        write_diffcoex(args.RESULT_NAME, genes, dcx_res, dcx_in_graph[0], dcx_in_graph[1], dcx_bm)
+        print('    %s_diffcoex.txt' % args.RESULT_NAME)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

@@ -59,17 +59,18 @@ def check_inputs(expr, label, n_perm):
     return x, lab[used]
 
 
-def quantise(x):
+def quantise(x, bits=Q_BITS):
     """float64 [n, G] -> int64 q [n, G]: per gene c = the mean, m = max |x - c|; q = 0 if m = 0, else
-    q = rint((x - c) 2^e) with e = 21 - floor(log2 m), so 2^21 <= max |q| <= 2^22.  Invariant to scaling a gene by a
-    power of two (the scaling is exact) and, where x - c is exact, to shifting it."""
+    q = rint((x - c) 2^e) with e = bits - 1 - floor(log2 m), so 2^(bits-1) <= max |q| <= 2^bits (bits = 22: the
+    permutation test's e = 21 - floor(log2 m)).  Invariant to scaling a gene by a power of two (the scaling is exact)
+    and, where x - c is exact, to shifting it."""
     x = np.asarray(x, dtype=np.float64)
     d = x - x.mean(axis=0)
     m = np.abs(d).max(axis=0) if x.shape[0] else np.zeros(x.shape[1])
     q = np.zeros(x.shape, dtype=np.int64)
     nz = m > 0
     _, ex = np.frexp(m[nz])                             # m = f 2^ex, 0.5 <= f < 1: floor(log2 m) = ex - 1
-    e = 22 - ex.astype(np.int64)                        # up to 1096: scale in two exact power-of-two steps
+    e = int(bits) - ex.astype(np.int64)                 # up to 1096: scale in two exact power-of-two steps
     h = e // 2
     q[:, nz] = np.rint(d[:, nz] * np.ldexp(1.0, h) * np.ldexp(1.0, e - h))
     return q

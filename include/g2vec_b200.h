@@ -756,6 +756,33 @@ int g2v_sig_auc(const double *scores, const uint8_t *y, const int8_t *fold, int3
                 int32_t n_sig, int32_t cap, double *auc, double *acc, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Label-permutation test of differential co-expression for every network pair (DESIGN.md §4.30; g2vec_b200/diffcoex.py
+ * does the host side).  A row is one labelling: an indicator [S_pad] u8 of its selected samples (g2v_perm_labels'
+ * rows, or the all-ones and observed rows), padding 0.  q [G][S_pad] int32, gene-major, |q| <= 2^16, padding 0.
+ * Pairs e = 0 .. E-1 are (pair_i[e], pair_j[e]), genes in [0, G).  1 <= n_b <= G2V_DCX_MAX_ROWS, 1 <= E <=
+ * G2V_DCX_MAX_PAIRS, S_pad a multiple of 32 in [32, G2V_DCX_MAX_SAMPLES].
+ * g2v_dcx_sums: S[r][e] = sum_s M[r][s] q[pair_i[e]][s] q[pair_j[e]][s], exact (FP64 mma.sync m8n8k4, every partial
+ *   sum an integer <= 2^47).  Exactly one of P and D is given:
+ *   P [n_b][E] int64: the sums (A .. P_tot, n and k unused; pairs (g, g) give sum_s q_g^2);
+ *   D [n_b][E] float64: every row has k selected samples of n (4 <= k <= n - 4); group 1 = the selected samples, group
+ *     2 = the others, with A [n_b][G] (g2v_perm_sums' sums of q), Bq [n_b][G] (sums of q^2), and the all-sample totals
+ *     A_tot, B_tot [G] and P_tot [E] giving group 2 by subtraction.  Per group (size m): C = m P - A_i A_j and
+ *     V_g = m B_g - A_g^2 (int64, exact), r = ll2double(C) / sqrt(ll2double(V_i) * ll2double(V_j)) clamped to [-1, 1],
+ *     0 when V_i or V_j is 0; D = 0 when r1 = r2, else |r2 - r1| / (1 - r1 r2), every operation correctly rounded.
+ * g2v_dcx_tally: per row of D, count[e] += D[e] >= D_obs[e];  count_maxt[e] += (max over e' >= e of D[e']) >=
+ *   D_obs[e].  Integer atomics only; the counts do not depend on the grid or on how the rows are chunked.
+ * Out-of-range sizes fail with nothing launched.  One launch each, never synchronises. */
+#define G2V_DCX_MAX_SAMPLES 32768
+#define G2V_DCX_MAX_ROWS (1 << 20)
+#define G2V_DCX_MAX_PAIRS (1 << 26)
+int g2v_dcx_sums(const uint8_t *M, int64_t n_b, int32_t S_pad, const int32_t *q, int32_t G, const int32_t *pair_i,
+                 const int32_t *pair_j, int64_t E, int32_t n, int32_t k, const int64_t *A, const int64_t *Bq,
+                 const int64_t *A_tot, const int64_t *B_tot, const int64_t *P_tot, int64_t *P, double *D,
+                 void *stream);
+int g2v_dcx_tally(const double *D, int64_t n_b, int64_t E, const double *D_obs, int64_t *count, int64_t *count_maxt,
+                  void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Between the two hot paths (SURVEY.md 8f-2): `tuple(sorted(path))` into a set (G2Vec.py:345,351) and
  * the removal of paths common to both groups (G2Vec.py:313).
  * g2v_paths_canonicalise: row i of nodes [n*L] (-1 or INT32_MAX padded) -> sorted [n*L] ascending with
