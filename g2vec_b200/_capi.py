@@ -158,6 +158,8 @@ SIGNATURES = {
     "g2v_dcx_sums": (ctypes.c_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
                                     _vp, _vp, _vp]),
     "g2v_dcx_tally": (ctypes.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "g2v_surv_rows": (ctypes.c_int, [_vp, _i32, _u64, _i64, _i64, _vp, _vp]),
+    "g2v_surv_scores": (ctypes.c_int, [_vp, _i32, _i32, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "g2v_paths_canonicalise":(ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
     "g2v_paths_mark": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "g2v_paths_set_workspace_bytes": (ctypes.c_size_t, [_i64]),

@@ -120,6 +120,21 @@ over the pairs with Q <= 0.05), and step 7 also writes RESULT_NAME_diffcoex.txt:
 positions in _lgroups.txt, R_good, R_poor, Z, P, P_maxT, Q, whether step 3 kept the pair in the good and in the poor
 graph (either direction), and how many of its two genes are biomarkers.  None of these depend on training.
 
+``--survival FILE`` (default off) adds a permutation Cox score test of every gene against patient survival, on the GPU
+(DESIGN.md §4.31).  FILE is tab-delimited with a header line and the columns SAMPLE, TIME (a finite number >= 0, any
+unit) and EVENT (1 for death or relapse, 0 for censored); further columns are ignored, rows of samples not in the
+expression file are ignored, and a sample whose TIME or EVENT is NA or empty is left out of the test.  Each gene's
+statistic is the Cox partial-likelihood score test at beta = 0 with Breslow ties (the log-rank test for a 0/1
+covariate without tied event times); Z > 0 means higher expression goes with higher hazard.
+``--survival-permutations B`` (default 1000, 1 <= B <= 2^20) permutations of the expression against the records, seeded
+by ``--seed`` and drawn as ``--permutations`` draws its rows, give each gene a raw P, Westfall & Young's step-down maxT
+P_maxT over the genes and the Benjamini-Hochberg Q.  The file and the inputs are checked after step 2 (every
+expression sample has exactly one row, at least 3 and at most 32768 samples used, at least one event), where the run
+prints a ``survival:`` line or stops with an ``ERROR``; after step 6 (on rank 0 only under torchrun) it prints a
+``survival:`` line that also gives the score test of the good / poor label itself, and step 7 also writes
+RESULT_NAME_survival.txt: per gene, in the order of _lgroups.txt, its L-group, Z, P_score (the asymptotic
+erfc(|Z| / sqrt(2))), P, P_maxT, Q and whether it is a biomarker.  None of these depend on training.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle`` or ``--class-weight``, at every table size (DESIGN.md §4.13); ``--class-weight 1,1`` writes the
@@ -231,6 +246,13 @@ def parse_arguments(argv=None):
                    help="label-permutation test of differential co-expression (Pearson, Fisher's z) of every gene pair "
                         "of the network with B permutations (1 <= B <= 2^20): raw, step-down maxT and "
                         "Benjamini-Hochberg p-values in RESULT_NAME_diffcoex.txt; 0 (default) = off")
+    p.add_argument('--survival', type=str, default=None, metavar='FILE',
+                   help="permutation Cox score test (Breslow ties) of every gene against the survival times of FILE "
+                        "(tab-delimited SAMPLE, TIME, EVENT with a header line), in RESULT_NAME_survival.txt; default "
+                        "off")
+    p.add_argument('--survival-permutations', type=int, default=1000, metavar='B',
+                   help="with --survival: permutations of the expression against the records, 1 <= B <= 2^20 "
+                        "(default 1000)")
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
@@ -247,6 +269,8 @@ def parse_arguments(argv=None):
     args.gene_set_size = _parse_gene_set_size(args.gene_set_size, p)
     if not 0 <= args.diff_coexpression <= 1 << 20:
         p.error("--diff-coexpression must be an integer in [0, 2^20]")
+    if not 1 <= args.survival_permutations <= 1 << 20:
+        p.error("--survival-permutations must be an integer in [1, 2^20]")
     if not 0 <= args.signature_cv <= 1 << 16:
         p.error("--signature-cv must be an integer in [0, 65536]")
     if not 2 <= args.signature_folds <= 100:
@@ -478,6 +502,16 @@ def write_diffcoex(prefix, genes, res, in_good, in_poor, biomarkers):
                             biomarkers))
 
 
+def write_survival(prefix, genes, lgroup, res, biomarkers):
+    """One row per gene in the order of _lgroups.txt: L-group, Z, P_score, P, P_maxT, Q of a survival.SurvivalResult,
+    biomarker 0/1."""
+    bm = set(biomarkers)
+    with open(prefix + "_survival.txt", 'w') as f:
+        f.write('GeneSymbol\tLgroup(0:good,1:poor,2:other)\tZ\tP_score\tP\tP_maxT\tQ\tBiomarker\n')
+        f.writelines('%s\t%d\t%.6f\t%.6g\t%.6g\t%.6g\t%.6g\t%d\n' % (g, k, z, ps, pv, pm, qv, g in bm)
+                     for g, k, z, ps, pv, pm, qv in zip(genes, lgroup, res.Z, res.P_score, res.P, res.P_maxT, res.Q))
+
+
 def write_vectors(prefix, genes, mat):
     with open(prefix + "_vectors.txt", 'w') as f:
         f.write('GeneSymbol' + ''.join('\tV%d' % i for i in range(mat.shape[1])) + '\n')
@@ -559,6 +593,18 @@ def main(argv=None):
             print('ERROR: --diff-coexpression: %s' % e)
             sys.exit(1)
         dcx_in_graph = []
+    if args.survival is not None:
+        from . import survival
+        try:                                           # fail now rather than after training
+            surv_time, surv_event, surv_used = survival.match_survival(survival.read_survival(args.survival),
+                                                                       data['sample'])
+            survival.check_inputs(data['expr'][surv_used], surv_time[surv_used], surv_event[surv_used],
+                                  args.survival_permutations)
+        except (OSError, ValueError) as e:
+            print('ERROR: --survival: %s' % e)
+            sys.exit(1)
+        print('    survival: %d of %d samples with a record, %d events, in %s'
+              % (int(surv_used.sum()), n_samples, int(surv_event[surv_used].sum()), args.survival))
     if args.kmeans_restarts and n_genes < 3:
         print('ERROR: --kmeans-restarts needs at least 3 common genes, found %d' % n_genes)
         sys.exit(1)
@@ -687,6 +733,14 @@ def main(argv=None):
         dcx_bm = is_bm[dcx_pairs[:, 0]] + is_bm[dcx_pairs[:, 1]]
         print('    ' + diffcoex.summary(dcx_res, dcx_in_graph[0], dcx_in_graph[1], dcx_bm))
 
+    if args.survival is not None:
+        surv_res = survival.survival_test(data['expr'][surv_used], surv_time[surv_used], surv_event[surv_used],
+                                          args.survival_permutations, seed=args.seed)
+        bm = set(biomarkers)
+        label_z, label_p = survival.label_score(data['label'][surv_used], surv_time[surv_used],
+                                                surv_event[surv_used])
+        print('    ' + survival.summary(surv_res, np.array([g in bm for g in genes]), label_z, label_p))
+
     print(">>> 7. Save results")
     write_biomarkers(args.RESULT_NAME, biomarkers)
     print('    %s_biomarkers.txt' % args.RESULT_NAME)
@@ -715,6 +769,9 @@ def main(argv=None):
     if args.diff_coexpression:
         write_diffcoex(args.RESULT_NAME, genes, dcx_res, dcx_in_graph[0], dcx_in_graph[1], dcx_bm)
         print('    %s_diffcoex.txt' % args.RESULT_NAME)
+    if args.survival is not None:
+        write_survival(args.RESULT_NAME, genes, lgroup, surv_res, biomarkers)
+        print('    %s_survival.txt' % args.RESULT_NAME)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

@@ -783,6 +783,33 @@ int g2v_dcx_tally(const double *D, int64_t n_b, int64_t E, const double *D_obs, 
                   void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Permutation Cox score test of every gene against survival (DESIGN.md §4.31; g2vec_b200/survival.py does the host
+ * side).  n samples (3 <= n <= G2V_SURV_MAX_SAMPLES) with survival records; the time order lists them by time
+ * descending and slot [n] int32 is its inverse (slot[s] = the time position of sample s).  Permutations are numbered
+ * b = 1 .. B, B <= G2V_SURV_MAX_PERMUTATIONS.
+ * g2v_surv_rows: idx [n_b][n] uint16, row r = permutation b = b_begin + 1 + r: pi_b is Fisher-Yates on the identity
+ *   with the draws of g2v_perm_labels' row b (for i = n-1 down to 1: j = hi64(draw64(seed, 2^63 + b, n-1-i) * (i+1)),
+ *   swap i and j), and idx[slot[pi_b(s)]] = s: sample s's expression meets sample pi_b(s)'s record.  A row depends
+ *   only on (slot, seed, b).
+ * g2v_surv_scores: T [n_b][G] float64 from q [n][G] int32 (sample-major, |q| <= 2^16) and the rows idx [n_b][n] (the
+ *   time order itself is the observed row).  flags [n] u8 per time position: bit 0 = an event, bit 1 = the last
+ *   position of its group of equal times; a, c [n] float64 at the group ends: a = 1 / S0, c = d / (S0 S0) with S0 =
+ *   the position + 1 and d the group's events.  Scanning the positions p = 0 .. n-1 with x = q[idx[r][p]][g]:
+ *   S1 += x, S2 += x^2, and over the group's events E1 += x, d += 1 (exact int64); at the end of a group with d > 0,
+ *   num_u = S0 E1 - d S1, num_v = S0 S2 - S1^2, U = U + ll2double(num_u) * a[p], V = V + ll2double(num_v) * c[p]
+ *   (each operation correctly rounded, from U = V = +0); then T = (U * U) / V, 0 when V = 0.  UV (may be NULL):
+ *   [2][n_b][G] float64, U then V.
+ * Out-of-range sizes fail with nothing launched.  One launch each, never synchronises; no floating-point atomics.
+ * The counts of T >= T_obs are g2v_dcx_tally's (E = G, the genes in rank order). */
+#define G2V_SURV_MAX_SAMPLES 32768
+#define G2V_SURV_MAX_PERMUTATIONS (1 << 20)
+#define G2V_SURV_MAX_GENES (1 << 20)
+int g2v_surv_rows(const int32_t *slot, int32_t n, uint64_t seed, int64_t b_begin, int64_t n_b, uint16_t *idx,
+                  void *stream);
+int g2v_surv_scores(const int32_t *q, int32_t n, int32_t G, const uint16_t *idx, int64_t n_b, const uint8_t *flags,
+                    const double *a, const double *c, double *T, double *UV, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Between the two hot paths (SURVEY.md 8f-2): `tuple(sorted(path))` into a set (G2Vec.py:345,351) and
  * the removal of paths common to both groups (G2Vec.py:313).
  * g2v_paths_canonicalise: row i of nodes [n*L] (-1 or INT32_MAX padded) -> sorted [n*L] ascending with
