@@ -96,6 +96,10 @@ SIGNATURES = {
     "g2v_cbow_loop_begin": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i64, _vp]),
     "g2v_cbow_loop_tail": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _f32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32,
                                           _vp]),
+    "g2v_cbow_loop_tail_val": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _f32, _vp, _i64, _vp, _vp, _vp, _vp, _vp,
+                                              _vp, _i32, _i32, _i32, _vp]),
+    "g2v_cbow_loop_tail_val_cw": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _f32, _vp, _i64, _vp, _vp, _vp, _vp,
+                                                 _vp, _vp, _i32, _i32, _i32, _f32, _f32, _vp]),
     "g2v_cbow_loop_decide": (ctypes.c_int, [_vp, _vp, _vp, _vp]),
     "g2v_cbow_loop_decide_best": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp]),
     "g2v_cbow_loop_keep_best": (ctypes.c_int, [_vp, _vp, _vp, _i64, _vp]),

@@ -369,6 +369,17 @@ class CbowModel:
             name, cw = self._cw("g2v_cbow_loop_tail")
             self._launch(name, *args, *cw)
 
+    def loop_tail_val(self, ctl, win, n_total, va):
+        """loop_tail(ctl, win, n_total) and evaluate(va, 2) on the certified pass as one window launch
+        (g2v_cbow_loop_tail_val, DESIGN.md §4.32): the same dO, counts and acc[5]; g_ho and acc[4] up to the order of
+        their atomics.  For a carried loop whose training list routes to csc and whose D is in TAIL_VAL_D."""
+        rec = self.prepared(win)
+        name, cw = self._cw("g2v_cbow_loop_tail_val")
+        self._launch(name, ctl.data_ptr(), self.rowptr.data_ptr(), self.gene.data_ptr(), self.label.data_ptr(),
+                     win.data_ptr(), rec.n, 1.0 / float(n_total), va.data_ptr(), int(va.shape[0]),
+                     self.W_ih.data_ptr(), self.W_ho.data_ptr(), self.st.data_ptr(), rec.dO.data_ptr(),
+                     self.g_ho.data_ptr(), self.acc.data_ptr(), self.V, self.D, self.reduce, *cw)
+
     def _lazy_update(self, adev):
         plan, r0, n_rows = self._pending or (None, 0, 0)
         self._pending = None
@@ -490,6 +501,9 @@ class CbowModel:
     def loss_sum(self, acc_host):
         return float(acc_host[:1].view(torch.float64)[0])
 
+
+# the hidden sizes g2v_cbow_loop_tail_val has kernels for
+TAIL_VAL_D = (128, 256, 512)
 
 # what early stopping and the reduce-on-plateau rate can decide on (train_cbow's ``monitor``)
 MONITORS = ("val_acc", "val_loss")
@@ -1023,7 +1037,8 @@ class DeviceLoop:
 
     Carried mode (``self.carried``: one GPU, rows, dense optimizer, fwdbwd on the CSC path of the training list):
     the training-accuracy pass runs on every step as the tail pass (g2v_cbow_loop_tail) and is also the next step's
-    forward, so the next fwdbwd only expands its dO into g_ih.  The training list is gathered once per step instead
+    forward, so the next fwdbwd only expands its dO into g_ih.  On the csc path with the certified validation pass
+    (monitor="val_acc", D in TAIL_VAL_D) the validation pass runs inside the tail's launch (g2v_cbow_loop_tail_val).  The training list is gathered once per step instead
     of twice.  This assumes the training windows do not change between steps: the list is static, and a
     WindowFeeder re-uploads the same windows every step.  The first step after reset() runs the full forward,
     decided on the device, so a graph captured right after reset() is correct from its first replay.
@@ -1120,14 +1135,19 @@ class DeviceLoop:
         m.update()
         if m_upd is not None:
             m_upd.record()
-        if self.n_va_loc:
+        # the carried csc step with the certified validation pass runs both window passes in one launch (§4.32)
+        tail_val = (self.carried and not m.det and not self.loss and self.n_va_loc and m.D in TAIL_VAL_D
+                    and choose_route(m.algo, False, False, m.prepared(self.va_d), 0, self.n_va_loc) in ("csc", "scatter"))
+        if self.n_va_loc and not tail_val:
             if self.loss:
                 m.evaluate(self.va_d, 2, loss=True)
             else:
                 m.evaluate(self.va_d, 2)
         if m_val is not None:
             m_val.record()
-        if self.carried:
+        if tail_val:
+            m.loop_tail_val(self.ctl, self.tr_d, self.n_tr, self.va_d)
+        elif self.carried:
             m.loop_tail(self.ctl, self.tr_d, self.n_tr)
         elif show and self.n_tr_loc:
             m.evaluate(self.tr_d, 3)

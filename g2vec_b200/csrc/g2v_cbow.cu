@@ -46,6 +46,59 @@ namespace g2v {
 // each gene row once.
 constexpr int kRowsEval = 0, kRowsScatter = 1, kRowsCsc = 2;
 
+// One window of cbow_rows_kernel, the whole warp: list position i, window n = win[win_begin + i] (or win_begin + i).
+// Adds the window's correct prediction (and with a backward its loss term) into the lane-0 accumulators, its h*dO
+// into the lanes' g_ho partial gho, and per MODE stores dO*scale at dO_pos[i] or scatters the rows into g_ih.
+// g2v_cbow_loop_tail_val's training items call it as well, so a window's dO and count are the same bits there.
+template <int VEC, int MODE, bool CW>
+__device__ __forceinline__ void rows_window(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
+                                            const uint8_t *__restrict__ label, const int32_t *__restrict__ win,
+                                            int64_t win_begin, int64_t i, float inv_n,
+                                            const float4 *__restrict__ W4, const float4 (&who)[VEC],
+                                            float *__restrict__ g_ih, float *__restrict__ dO_pos, int32_t reduce_mean,
+                                            float2 cw, int lane, float4 (&gho)[VEC], float &loss_acc,
+                                            unsigned &correct_acc) {
+    constexpr bool BACKWARD = MODE != kRowsEval;
+    constexpr int D = 128 * VEC;
+    const int64_t n = win ? (int64_t)__ldg(win + win_begin + i) : win_begin + i;
+    const int32_t b = __ldg(rowptr + n), e = __ldg(rowptr + n + 1);
+    const float y = (float)__ldg(label + n);
+    float4 h[VEC];
+    float scale;
+    const float o = rows_logit<VEC>(gene, W4, b, e, lane, reduce_mean, who, h, scale);
+    if (lane == 0) {
+        correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
+        if (BACKWARD) loss_acc += class_weighted<CW>(fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o))), y, cw);
+    }
+    if (MODE == kRowsCsc) {
+        const float dO = class_weighted<CW>((sigmoid_stable(o) - y) * inv_n, y, cw);
+#pragma unroll
+        for (int v = 0; v < VEC; ++v) {
+            gho[v].x += h[v].x * dO; gho[v].y += h[v].y * dO; gho[v].z += h[v].z * dO; gho[v].w += h[v].w * dO;
+        }
+        if (lane == 0) dO_pos[i] = dO * scale;
+    } else if (MODE == kRowsScatter) {
+        const float dO = class_weighted<CW>((sigmoid_stable(o) - y) * inv_n, y, cw);
+        float4 gv[VEC];
+#pragma unroll
+        for (int v = 0; v < VEC; ++v) {
+            gho[v].x += h[v].x * dO; gho[v].y += h[v].y * dO; gho[v].z += h[v].z * dO; gho[v].w += h[v].w * dO;
+            const float s = dO * scale;
+            gv[v] = make_float4(who[v].x * s, who[v].y * s, who[v].z * s, who[v].w * s);
+        }
+        for (int32_t base = b; base < e; base += 32) {
+            const int cnt = min(32, e - base);
+            const int32_t g = (lane < cnt) ? __ldg(gene + base + lane) : 0;
+            for (int k = 0; k < cnt; ++k) {
+                const int32_t gk = __shfl_sync(0xffffffffu, g, k);
+                float *dst = g_ih + (size_t)gk * D + lane * 4;
+#pragma unroll
+                for (int v = 0; v < VEC; ++v) red_add4(dst + v * 128, gv[v]);
+            }
+        }
+    }
+}
+
 // carried != NULL and set: the loop's tail pass already ran this forward at these weights (g2v_cbow_loop_tail).
 // CW: the training term of a window of label y is weighted by cw.{x,y}[y] (class_weighted, DESIGN.md §4.20).
 template <int VEC, int MODE, bool CW>
@@ -79,45 +132,9 @@ cbow_rows_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__
     float loss_acc = 0.f;
 
     const int64_t warps_total = (int64_t)gridDim.x * kCbowWarps;
-    for (int64_t i = (int64_t)blockIdx.x * kCbowWarps + warp; i < n_win; i += warps_total) {
-        const int64_t n = win ? (int64_t)__ldg(win + win_begin + i) : win_begin + i;
-        const int32_t b = __ldg(rowptr + n), e = __ldg(rowptr + n + 1);
-        const float y = (float)__ldg(label + n);
-        float4 h[VEC];
-        float scale;
-        const float o = rows_logit<VEC>(gene, W4, b, e, lane, reduce_mean, who, h, scale);
-        if (lane == 0) {
-            correct_acc += ((o > 0.f) == (y != 0.f)) ? 1u : 0u;
-            if (BACKWARD) loss_acc += class_weighted<CW>(fmaxf(o, 0.f) - o * y + log1pf(expf(-fabsf(o))), y, cw);
-        }
-        if (MODE == kRowsCsc) {
-            const float dO = class_weighted<CW>((sigmoid_stable(o) - y) * inv_n, y, cw);
-#pragma unroll
-            for (int v = 0; v < VEC; ++v) {
-                gho[v].x += h[v].x * dO; gho[v].y += h[v].y * dO; gho[v].z += h[v].z * dO; gho[v].w += h[v].w * dO;
-            }
-            if (lane == 0) dO_pos[i] = dO * scale;
-        } else if (MODE == kRowsScatter) {
-            const float dO = class_weighted<CW>((sigmoid_stable(o) - y) * inv_n, y, cw);
-            float4 gv[VEC];
-#pragma unroll
-            for (int v = 0; v < VEC; ++v) {
-                gho[v].x += h[v].x * dO; gho[v].y += h[v].y * dO; gho[v].z += h[v].z * dO; gho[v].w += h[v].w * dO;
-                const float s = dO * scale;
-                gv[v] = make_float4(who[v].x * s, who[v].y * s, who[v].z * s, who[v].w * s);
-            }
-            for (int32_t base = b; base < e; base += 32) {
-                const int cnt = min(32, e - base);
-                const int32_t g = (lane < cnt) ? __ldg(gene + base + lane) : 0;
-                for (int k = 0; k < cnt; ++k) {
-                    const int32_t gk = __shfl_sync(0xffffffffu, g, k);
-                    float *dst = g_ih + (size_t)gk * D + lane * 4;
-#pragma unroll
-                    for (int v = 0; v < VEC; ++v) red_add4(dst + v * 128, gv[v]);
-                }
-            }
-        }
-    }
+    for (int64_t i = (int64_t)blockIdx.x * kCbowWarps + warp; i < n_win; i += warps_total)
+        rows_window<VEC, MODE, CW>(rowptr, gene, label, win, win_begin, i, inv_n, W4, who, g_ih, dO_pos, reduce_mean,
+                                   cw, lane, gho, loss_acc, correct_acc);
     cta_epilogue<VEC, BACKWARD, true>(sh_gho, sh_acc, gho, loss_acc, correct_acc, lane, g_ho, loss_sum, n_correct);
 }
 
@@ -200,10 +217,78 @@ __device__ __forceinline__ float certified_tau(float T, float scale, int32_t l, 
     return __fadd_rn(__fmul_rn(rel, T), abs_);
 }
 
-// 8 lanes per window, 4 windows per warp (r1_windows_kernel's layout) for o' and T; then the whole warp gathers the
-// rows of each undecided window of the four in turn.  VEC > 0: D = 128 * VEC; VEC == 0: any D, h in shared memory
-// ([kCbowWarps][D], dynamic).  force_gather: every window takes the row gather (tests).  n_gathered (nullable): the
-// number of windows that took it.
+// One group of the certified pass: windows base .. base + 3 of the list, 8 lanes per window (r1_windows_kernel's
+// layout) for o' and T; then the whole warp gathers the rows of each undecided window of the four in turn.  A is
+// sum_d |W_ho[d]| (certified_tau's underflow term); with VEC > 0 a negative A is computed here from the lanes' who,
+// after the group's st loads are issued, so that the warp does not wait for W_ho before its first window's loads.
+// The group's correct windows are added into correct_acc (any lane; the caller sums the warp), the gathered ones
+// into gathered_acc (lane 0).  cbow_eval_certified_kernel and g2v_cbow_loop_tail_val's validation items call it.
+template <int VEC>
+__device__ __forceinline__ void certified_group(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
+                                                const uint8_t *__restrict__ label, const int32_t *__restrict__ win,
+                                                int64_t win_begin, int64_t n_win, int64_t base,
+                                                const float *__restrict__ W_ih, const float *__restrict__ W_ho,
+                                                const float2 *__restrict__ st, const float4 (&who)[VEC > 0 ? VEC : 1],
+                                                float *h_generic, int32_t D, int32_t reduce_mean,
+                                                int32_t force_gather, int lane, float &A, unsigned &correct_acc,
+                                                unsigned &gathered_acc) {
+    constexpr int NV = VEC > 0 ? VEC : 1;
+    const int sub = lane & 7, slot = lane >> 3;
+    const int64_t i = base + slot;
+    const bool active = i < n_win;
+    int32_t b = 0, e = 0;
+    float y = 0.f;
+    if (active) {
+        const int64_t n = win ? (int64_t)__ldg(win + win_begin + i) : win_begin + i;
+        b = __ldg(rowptr + n); e = __ldg(rowptr + n + 1);
+        y = (float)__ldg(label + n);
+    }
+    float ps = 0.f, pt = 0.f;
+    for (int32_t j = b + sub; j < e; j += 8) {
+        const float2 q = __ldg(st + __ldg(gene + j));
+        ps += q.x; pt += q.y;
+    }
+#pragma unroll
+    for (int o = 4; o > 0; o >>= 1) {
+        ps += __shfl_xor_sync(0xffffffffu, ps, o);
+        pt += __shfl_xor_sync(0xffffffffu, pt, o);
+    }
+    if (VEC > 0 && A < 0.f) {                              // A is warp-uniform: the whole warp takes this branch
+        A = 0.f;
+#pragma unroll
+        for (int v = 0; v < NV; ++v)
+            A += (fabsf(who[v].x) + fabsf(who[v].y)) + (fabsf(who[v].z) + fabsf(who[v].w));
+        A = warp_sum(A);
+    }
+    const float scale = (reduce_mean && e > b) ? 1.f / (float)(e - b) : 1.f;
+    const float o1 = ps * scale;
+    const bool decided = !force_gather && fabsf(o1) <= 0x1.fffffep127f
+                         && fabsf(o1) > certified_tau(pt, scale, e - b, D, A);
+    if (active && sub == 0 && decided) correct_acc += ((o1 > 0.f) == (y != 0.f)) ? 1u : 0u;
+    unsigned todo = __ballot_sync(0xffffffffu, active && sub == 0 && !decided);
+    const float4 *__restrict__ W4 = reinterpret_cast<const float4 *>(W_ih);
+    while (todo) {
+        const int src = __ffs(todo) - 1;
+        todo &= todo - 1;
+        const int32_t wb = __shfl_sync(0xffffffffu, b, src), we = __shfl_sync(0xffffffffu, e, src);
+        const float wy = __shfl_sync(0xffffffffu, y, src);
+        float wscale, o;
+        if (VEC > 0) {
+            float4 h[NV];
+            o = rows_logit<NV>(gene, W4, wb, we, lane, reduce_mean, who, h, wscale);
+        } else {
+            o = rows_generic_logit(gene, W_ih, W_ho, wb, we, lane, D, reduce_mean, h_generic, wscale);
+        }
+        if (lane == 0) {
+            correct_acc += ((o > 0.f) == (wy != 0.f)) ? 1u : 0u;
+            ++gathered_acc;
+        }
+    }
+}
+
+// certified_group over the list, 4 windows per warp and group.  VEC > 0: D = 128 * VEC; VEC == 0: any D, h in shared
+// memory ([kCbowWarps][D], dynamic).  force_gather: every window takes the row gather (tests).  n_gathered
+// (nullable): the number of windows that took it.
 template <int VEC>
 __global__ void __launch_bounds__(kCbowWarps * 32)
 cbow_eval_certified_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
@@ -217,76 +302,26 @@ cbow_eval_certified_kernel(const int32_t *__restrict__ rowptr, const int32_t *__
     extern __shared__ float shf[];
     __shared__ unsigned long long sh_cnt[2];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int sub = lane & 7, slot = lane >> 3;
     if (threadIdx.x < 2) sh_cnt[threadIdx.x] = 0ull;
     __syncthreads();
-    const float4 *__restrict__ W4 = reinterpret_cast<const float4 *>(W_ih);
     float4 who[NV];
     if (VEC > 0) {
 #pragma unroll
         for (int v = 0; v < NV; ++v) who[v] = ldg4(reinterpret_cast<const float4 *>(W_ho) + v * 32 + lane);
     }
     float *h_generic = shf + (size_t)warp * D;
-    // A = sum_d |W_ho[d]| (certified_tau's underflow term).  VEC > 0: from the lanes' who, summed where it is first
-    // needed, so that the warp does not wait for W_ho before its first window's loads are issued
-    float A = 0.f;
+    // VEC > 0: A is left to the first group (certified_group)
+    float A = -1.f;
     if (VEC == 0) {
+        A = 0.f;
         for (int d = lane; d < D; d += 32) A += fabsf(__ldg(W_ho + d));
         A = warp_sum(A);
     }
     unsigned correct_acc = 0, gathered_acc = 0;
     const int64_t stride = (int64_t)gridDim.x * kCbowWarps * 4;
-    for (int64_t base = ((int64_t)blockIdx.x * kCbowWarps + warp) * 4; base < n_win; base += stride) {
-        const int64_t i = base + slot;
-        const bool active = i < n_win;
-        int32_t b = 0, e = 0;
-        float y = 0.f;
-        if (active) {
-            const int64_t n = win ? (int64_t)__ldg(win + win_begin + i) : win_begin + i;
-            b = __ldg(rowptr + n); e = __ldg(rowptr + n + 1);
-            y = (float)__ldg(label + n);
-        }
-        float ps = 0.f, pt = 0.f;
-        for (int32_t j = b + sub; j < e; j += 8) {
-            const float2 q = __ldg(st + __ldg(gene + j));
-            ps += q.x; pt += q.y;
-        }
-#pragma unroll
-        for (int o = 4; o > 0; o >>= 1) {
-            ps += __shfl_xor_sync(0xffffffffu, ps, o);
-            pt += __shfl_xor_sync(0xffffffffu, pt, o);
-        }
-        if (VEC > 0) {
-            A = 0.f;
-#pragma unroll
-            for (int v = 0; v < NV; ++v)
-                A += (fabsf(who[v].x) + fabsf(who[v].y)) + (fabsf(who[v].z) + fabsf(who[v].w));
-            A = warp_sum(A);
-        }
-        const float scale = (reduce_mean && e > b) ? 1.f / (float)(e - b) : 1.f;
-        const float o1 = ps * scale;
-        const bool decided = !force_gather && fabsf(o1) <= 0x1.fffffep127f
-                             && fabsf(o1) > certified_tau(pt, scale, e - b, D, A);
-        if (active && sub == 0 && decided) correct_acc += ((o1 > 0.f) == (y != 0.f)) ? 1u : 0u;
-        unsigned todo = __ballot_sync(0xffffffffu, active && sub == 0 && !decided);
-        while (todo) {
-            const int src = __ffs(todo) - 1;
-            todo &= todo - 1;
-            const int32_t wb = __shfl_sync(0xffffffffu, b, src), we = __shfl_sync(0xffffffffu, e, src);
-            const float wy = __shfl_sync(0xffffffffu, y, src);
-            float wscale, o;
-            if (VEC > 0) {
-                float4 h[NV];
-                o = rows_logit<NV>(gene, W4, wb, we, lane, reduce_mean, who, h, wscale);
-            } else {
-                o = rows_generic_logit(gene, W_ih, W_ho, wb, we, lane, D, reduce_mean, h_generic, wscale);
-            }
-            if (lane == 0) {
-                correct_acc += ((o > 0.f) == (wy != 0.f)) ? 1u : 0u;
-                ++gathered_acc;
-            }
-        }
-    }
+    for (int64_t base = ((int64_t)blockIdx.x * kCbowWarps + warp) * 4; base < n_win; base += stride)
+        certified_group<VEC>(rowptr, gene, label, win, win_begin, n_win, base, W_ih, W_ho, st, who, h_generic, D,
+                             reduce_mean, force_gather, lane, A, correct_acc, gathered_acc);
     correct_acc = __reduce_add_sync(0xffffffffu, correct_acc);
     if (lane == 0) {
         atomicAdd(&sh_cnt[0], (unsigned long long)correct_acc);
@@ -297,6 +332,78 @@ cbow_eval_certified_kernel(const int32_t *__restrict__ rowptr, const int32_t *__
         atomicAdd(n_correct, sh_cnt[0]);
         if (n_gathered) atomicAdd(n_gathered, sh_cnt[1]);
     }
+}
+
+// ---- the carried step's two window passes in one launch (DESIGN.md §4.32) ----------------------------------------
+// Items: the validation list in groups of four windows (certified_group, items 0 .. n_groups-1), then the training
+// list one window per item (rows_window<VEC, kRowsCsc, CW>, item n_groups + i = list position i).  Warps take
+// kTailValChunk consecutive items at a time from the counter *queue, so the cheap validation groups go first and the
+// last warps to finish end within a chunk of each other.  Every warp stops at its first fetch past the end, after its
+// last item, so the fetch that returns (chunks + warps - 1) * kTailValChunk is the launch's last access to the
+// counter, and that warp sets it back to 0 for the next launch.  The validation count goes to n_correct_va; the
+// training count, loss and g_ho partial go through cta_epilogue as in cbow_rows_kernel.
+constexpr int kTailValChunk = 2;
+// The CTAs per SM of cbow_rows_kernel<VEC, kRowsCsc> at its register count, given to ptxas as the kernel's minimum:
+// without it ptxas fits this kernel in fewer registers by issuing the row gather's loads a few at a time.
+constexpr int tail_val_min_ctas(int vec) { return vec == 1 ? 4 : vec == 2 ? 3 : 2; }
+
+template <int VEC, bool CW>
+__global__ void __launch_bounds__(kCbowWarps * 32, tail_val_min_ctas(VEC))
+cbow_tail_val_kernel(const int32_t *__restrict__ rowptr, const int32_t *__restrict__ gene,
+                     const uint8_t *__restrict__ label, const int32_t *__restrict__ tr_win, int64_t n_tr, float inv_n,
+                     const int32_t *__restrict__ va_win, int64_t n_va, const float *__restrict__ W_ih,
+                     const float *__restrict__ W_ho, const float2 *__restrict__ st, float *__restrict__ dO_pos,
+                     float *__restrict__ g_ho, double *__restrict__ loss_sum,
+                     unsigned long long *__restrict__ n_correct_tr, unsigned long long *__restrict__ n_correct_va,
+                     int32_t reduce_mean, unsigned long long *__restrict__ queue, const int32_t *__restrict__ skip,
+                     float2 cw) {
+    G2V_SKIP_IF_STOPPED(skip);
+    constexpr int D = 128 * VEC;
+    __shared__ float sh_gho[D];
+    __shared__ CtaAcc sh_acc;
+    __shared__ unsigned long long sh_va;
+    const int lane = threadIdx.x & 31;
+    for (int i = threadIdx.x; i < D; i += blockDim.x) sh_gho[i] = 0.f;
+    if (threadIdx.x == 0) { sh_acc.loss = 0.0; sh_acc.correct = 0ull; sh_va = 0ull; }
+    __syncthreads();
+
+    const float4 *__restrict__ W4 = reinterpret_cast<const float4 *>(W_ih);
+    float4 who[VEC], gho[VEC];
+#pragma unroll
+    for (int v = 0; v < VEC; ++v) {
+        who[v] = ldg4(reinterpret_cast<const float4 *>(W_ho) + v * 32 + lane);
+        gho[v] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    unsigned correct_acc = 0, va_acc = 0, gathered_acc = 0;
+    float loss_acc = 0.f, A = -1.f;                        // A: computed by the warp's first validation group
+
+    const int64_t n_groups = (n_va + 3) / 4, n_items = n_groups + n_tr;
+    const unsigned long long last =
+        (unsigned long long)((n_items + kTailValChunk - 1) / kTailValChunk + (int64_t)gridDim.x * kCbowWarps - 1)
+        * kTailValChunk;
+    for (;;) {
+        unsigned long long first = 0;
+        if (lane == 0) first = atomicAdd(queue, (unsigned long long)kTailValChunk);
+        first = __shfl_sync(0xffffffffu, first, 0);
+        if (first >= (unsigned long long)n_items) {
+            if (lane == 0 && first == last) atomicExch(queue, 0ull);
+            break;
+        }
+        const int64_t end = min((int64_t)first + kTailValChunk, n_items);
+        for (int64_t it = (int64_t)first; it < end; ++it) {
+            if (it < n_groups)
+                certified_group<VEC>(rowptr, gene, label, va_win, 0, n_va, it * 4, W_ih, W_ho, st, who, nullptr, D,
+                                     reduce_mean, 0, lane, A, va_acc, gathered_acc);
+            else
+                rows_window<VEC, kRowsCsc, CW>(rowptr, gene, label, tr_win, 0, it - n_groups, inv_n, W4, who, nullptr,
+                                               dO_pos, reduce_mean, cw, lane, gho, loss_acc, correct_acc);
+        }
+    }
+    va_acc = __reduce_add_sync(0xffffffffu, va_acc);
+    if (lane == 0 && va_acc) atomicAdd(&sh_va, (unsigned long long)va_acc);
+    // its barrier orders the sh_va adds before thread 0 reads it
+    cta_epilogue<VEC, true, true>(sh_gho, sh_acc, gho, loss_acc, correct_acc, lane, g_ho, loss_sum, n_correct_tr);
+    if (threadIdx.x == 0 && sh_va) atomicAdd(n_correct_va, sh_va);
 }
 
 // Second half of the CSC backward.  The model is linear, so every window adds the same row W_ho to its genes,
@@ -897,7 +1004,7 @@ static int launch_rows_det(const int32_t *rowptr, const int32_t *gene, const uin
 //   [6] carried      1 once a tail pass (g2v_cbow_loop_tail) has run the training forward of the current weights:
 //                    dO per list position, the g_ho partial and the carry counters acc[4..5] are pending, and the
 //                    forward of g2v_cbow_fwdbwd_csc returns at once while the loop is attached
-//   [7] unused
+//   [7] queue        the work counter of g2v_cbow_loop_tail_val, 0 between its launches (cbow_tail_val_kernel)
 // acc (int64): [0] loss sum (f64 bits)  [1] pre-update train correct  [2] validation correct  [3] train correct;
 //   with tail passes also [4] carried loss sum (f64 bits)  [5] carried train correct (this rank's own count, kept
 //   out of [1..3], the range a multi-GPU step sums over the ranks).
@@ -1462,6 +1569,63 @@ extern "C" int g2v_cbow_loop_tail_cw(int64_t *ctl, const int32_t *rowptr, const 
     G2V_CW_CHECK("g2v_cbow_loop_tail_cw");
     return loop_tail_impl<true>("g2v_cbow_loop_tail_cw", ctl, rowptr, gene, label, win, n_win, inv_n_total, W_ih,
                                 W_ho, dO, g_ho, acc, V, D, reduce, float2{w0, w1}, stream);
+}
+
+template <bool CW>
+static int loop_tail_val_impl(const char *name, int64_t *ctl, const int32_t *rowptr, const int32_t *gene,
+                              const uint8_t *label, const int32_t *tr_win, int64_t n_tr, float inv_n_total,
+                              const int32_t *va_win, int64_t n_va, const float *W_ih, const float *W_ho, float *st,
+                              float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D, int32_t reduce, float2 cw,
+                              void *stream) {
+    G2V_REQUIRE(ctl && acc, "%s: null loop state", name);
+    G2V_REQUIRE(V > 0 && D > 0 && n_tr >= 0 && n_va >= 0, "%s: bad sizes (V=%d D=%d n_tr=%lld n_va=%lld)", name, V, D,
+                (long long)n_tr, (long long)n_va);
+    G2V_REQUIRE(D == 128 || D == 256 || D == 512, "%s: needs D = 128, 256 or 512 (D=%d)", name, D);
+    G2V_REQUIRE(rowptr && label && W_ih && W_ho && st && dO && g_ho, "%s: null pointer", name);
+    G2V_REQUIRE(reduce == G2V_REDUCE_SUM || reduce == G2V_REDUCE_MEAN, "%s: unknown reduce %d", name, reduce);
+    cudaStream_t s = (cudaStream_t)stream;
+    int rc;
+    // st complete before any warp of the window pass reads it: a launch of its own, no grid-wide wait
+    if (n_va > 0 && (rc = launch_r1_prepare(W_ih, W_ho, st, V, D, true, s))) return rc;
+    const int64_t n_items = (n_va + 3) / 4 + n_tr;
+    if (n_items > 0) {
+        auto kern = D == 128 ? cbow_tail_val_kernel<1, CW> : D == 256 ? cbow_tail_val_kernel<2, CW>
+                                                                      : cbow_tail_val_kernel<4, CW>;
+        int grid = 0;
+        if ((rc = rows_grid((const void *)kern, 0, n_items, &grid))) return rc;
+        kern<<<grid, kCbowWarps * 32, 0, s>>>(rowptr, gene, label, tr_win, n_tr, inv_n_total, va_win, n_va, W_ih, W_ho,
+                                              reinterpret_cast<const float2 *>(st), dO, g_ho,
+                                              reinterpret_cast<double *>(acc + 4),
+                                              reinterpret_cast<unsigned long long *>(acc + 5),
+                                              reinterpret_cast<unsigned long long *>(acc + 2),
+                                              reduce == G2V_REDUCE_MEAN,
+                                              reinterpret_cast<unsigned long long *>(ctl + 7), loop_skip_flag(), cw);
+        G2V_CUDA_OK(cudaGetLastError());
+        count_launch();
+    }
+    loop_carry_kernel<<<1, 1, 0, s>>>(reinterpret_cast<long long *>(ctl), reinterpret_cast<long long *>(acc));
+    G2V_CUDA_OK(cudaGetLastError());
+    count_launch();
+    return 0;
+}
+
+extern "C" int g2v_cbow_loop_tail_val(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                                      const int32_t *tr_win, int64_t n_tr, float inv_n_total, const int32_t *va_win,
+                                      int64_t n_va, const float *W_ih, const float *W_ho, float *st, float *dO,
+                                      float *g_ho, int64_t *acc, int32_t V, int32_t D, int32_t reduce, void *stream) {
+    return loop_tail_val_impl<false>("g2v_cbow_loop_tail_val", ctl, rowptr, gene, label, tr_win, n_tr, inv_n_total,
+                                     va_win, n_va, W_ih, W_ho, st, dO, g_ho, acc, V, D, reduce, float2{1.f, 1.f},
+                                     stream);
+}
+
+extern "C" int g2v_cbow_loop_tail_val_cw(int64_t *ctl, const int32_t *rowptr, const int32_t *gene,
+                                         const uint8_t *label, const int32_t *tr_win, int64_t n_tr, float inv_n_total,
+                                         const int32_t *va_win, int64_t n_va, const float *W_ih, const float *W_ho,
+                                         float *st, float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D,
+                                         int32_t reduce, float w0, float w1, void *stream) {
+    G2V_CW_CHECK("g2v_cbow_loop_tail_val_cw");
+    return loop_tail_val_impl<true>("g2v_cbow_loop_tail_val_cw", ctl, rowptr, gene, label, tr_win, n_tr, inv_n_total,
+                                    va_win, n_va, W_ih, W_ho, st, dO, g_ho, acc, V, D, reduce, float2{w0, w1}, stream);
 }
 
 extern "C" size_t g2v_cbow_det_workspace_bytes(int64_t n_win, int32_t D) {

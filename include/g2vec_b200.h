@@ -292,6 +292,10 @@ int g2v_cbow_loop_tail_cw(int64_t *ctl, const int32_t *rowptr, const int32_t *ge
                           const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
                           float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D, int32_t reduce, float w0,
                           float w1, void *stream);
+int g2v_cbow_loop_tail_val_cw(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                              const int32_t *tr_win, int64_t n_tr, float inv_n_total, const int32_t *va_win,
+                              int64_t n_va, const float *W_ih, const float *W_ho, float *st, float *dO, float *g_ho,
+                              int64_t *acc, int32_t V, int32_t D, int32_t reduce, float w0, float w1, void *stream);
 int g2v_cbow_loop_tail_det_cw(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
                               const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih,
                               const float *W_ho, float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D,
@@ -359,8 +363,8 @@ int g2v_cbow_eval_certified(const int32_t *rowptr, const int32_t *gene, const ui
 /* ---------------------------------------------------------------------------------------
  * Device-side control of the training loop (SURVEY.md 8f-4; G2Vec.py:262-283), so that several iterations of
  * the reference's loop can be enqueued -- or replayed as ONE CUDA graph -- without a host decision in between.
- *   ctl  [8] int64 in device memory: {stopped, step, stop_step, before_val, max_steps, early_stop, carried, -}
- *        g2v_cbow_loop_init sets {0, 0, -1, -1, max_steps, early_stop, 0}.
+ *   ctl  [8] int64 in device memory: {stopped, step, stop_step, before_val, max_steps, early_stop, carried, queue}
+ *        g2v_cbow_loop_init sets {0, 0, -1, -1, max_steps, early_stop, 0, 0}.
  *   g2v_cbow_loop_attach(ctl): from now on every CBOW kernel launched by THIS host thread first reads
  *        ctl.stopped and returns at once if it is set (attach(NULL) detaches); the forward of
  *        g2v_cbow_fwdbwd_csc also returns at once while ctl.carried is set (its per-gene expansion still runs).
@@ -385,6 +389,15 @@ int g2v_cbow_loop_begin(const int64_t *ctl, int64_t *acc, const float *W_ih, flo
 int g2v_cbow_loop_tail(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
                        const int32_t *win, int64_t n_win, float inv_n_total, const float *W_ih, const float *W_ho,
                        float *dO, float *g_ho, int64_t *acc, int32_t V, int32_t D, int32_t reduce, void *stream);
+/* g2v_cbow_loop_tail_val (DESIGN.md §4.32): the validation pass g2v_cbow_eval_certified(va_win[0..n_va-1]) into
+ * acc[2] and the tail pass g2v_cbow_loop_tail(tr_win[0..n_tr-1]) in one window launch, after st's own launch: the same
+ * validation count, the same dO and acc[5]; g_ho and acc[4] differ only by the order of their atomics.  Warps take
+ * validation groups of four windows, then training windows, from the counter in ctl[7], which the launch leaves at 0
+ * (g2v_cbow_loop_init sets it so).  D = 128, 256 or 512.  Both window launches and the carry test `stopped`. */
+int g2v_cbow_loop_tail_val(int64_t *ctl, const int32_t *rowptr, const int32_t *gene, const uint8_t *label,
+                           const int32_t *tr_win, int64_t n_tr, float inv_n_total, const int32_t *va_win, int64_t n_va,
+                           const float *W_ih, const float *W_ho, float *st, float *dO, float *g_ho, int64_t *acc,
+                           int32_t V, int32_t D, int32_t reduce, void *stream);
 int g2v_cbow_loop_decide(int64_t *ctl, const int64_t *acc, int64_t *hist, void *stream);
 /* Early stopping with patience (DESIGN.md §4.15): the loop keeps the weights of its best step instead of a snapshot.
  *   best [4] int64 in device memory: {patience, best_step, bad_steps, improved}; the caller sets {K, -1, 0, 0}
