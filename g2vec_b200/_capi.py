@@ -159,6 +159,10 @@ SIGNATURES = {
     "g2v_sig_fit": (ctypes.c_int, [_vp, _i32, _i32, _i64, _vp, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp,
                                    _i32, _vp]),
     "g2v_sig_auc": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "g2v_cox_fit_smem_bytes": (ctypes.c_size_t, [_i32]),
+    "g2v_cox_fit": (ctypes.c_int, [_vp, _i32, _i32, _i64, _vp, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp,
+                                   _vp, _i32, _vp]),
+    "g2v_cox_concordance": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp]),
     "g2v_dcx_sums": (ctypes.c_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
                                     _vp, _vp, _vp]),
     "g2v_dcx_tally": (ctypes.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp]),

@@ -135,6 +135,24 @@ prints a ``survival:`` line or stops with an ``ERROR``; after step 6 (on rank 0 
 RESULT_NAME_survival.txt: per gene, in the order of _lgroups.txt, its L-group, Z, P_score (the asymptotic
 erfc(|Z| / sqrt(2))), P, P_maxT, Q and whether it is a biomarker.  None of these depend on training.
 
+``--survival-cv R`` (default 0: off; 0 <= R <= 65536, needs ``--survival``) adds a cross-validated test of whether the
+biomarkers predict survival, on the GPU (DESIGN.md §4.33), over the samples ``--survival`` uses: ridge Cox regression
+(Breslow ties, penalty |beta|^2 / 2 on the summed partial likelihood, features standardised on each training fold)
+over ``--survival-cv-repeats K`` (default 10, 1 <= K <= 100) repeats of ``--survival-cv-folds F``-fold splits (default
+5, 2 <= F <= 100, F at most the number of events and at most half the samples) stratified by event status, scored on
+each test fold with Harrell's C.  The biomarkers are compared with the same number of genes of largest |t| (``top_t``,
+as ``--signature-cv`` picks them), of largest Cox score statistic (``top_z``, the ranking of ``--survival``) and with
+R random signatures of that size (the random signatures of ``--signature-cv`` for the same ``--seed``); P_random =
+(1 + #{random C >= C}) / (R + 1).  Each sample's out-of-fold risk, averaged over the repeats, splits the samples at the
+median into a high- and a low-risk group (pre-validation), with a log-rank test and the hazard ratio of the high-risk
+group.  It needs ``-n`` <= 64.  The inputs are checked after step 2, where the run stops with an ``ERROR`` if they are
+refused; after step 6 (on rank 0 only under torchrun) it prints a ``survival CV:`` line, and step 7 also writes
+RESULT_NAME_survival_cv.txt: per signature (biomarkers, top_t, top_z, random_1 .. random_R) its size, mean C over the
+fits, the SD of the K per-repeat means, P_random, the log-rank Z and P and the hazard ratio with its 95 % CI of the
+risk groups (``nan`` on random rows) and how many of its genes are biomarkers; and RESULT_NAME_risk.txt: per sample
+used, in the expression file's order, its time, event, the biomarkers' pre-validated risk and group (1 = high risk),
+ready for a Kaplan-Meier plot.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle`` or ``--class-weight``, at every table size (DESIGN.md §4.13); ``--class-weight 1,1`` writes the
@@ -253,6 +271,15 @@ def parse_arguments(argv=None):
     p.add_argument('--survival-permutations', type=int, default=1000, metavar='B',
                    help="with --survival: permutations of the expression against the records, 1 <= B <= 2^20 "
                         "(default 1000)")
+    p.add_argument('--survival-cv', type=int, default=0, metavar='R',
+                   help="with --survival: cross-validated Harrell's C of ridge Cox fits of the biomarkers against the "
+                        "top-|t| genes, the top-|Z| genes and R random signatures of the same size (0 <= R <= 65536), "
+                        "in RESULT_NAME_survival_cv.txt, and the biomarkers' pre-validated risk groups in "
+                        "RESULT_NAME_risk.txt; 0 (default) = off")
+    p.add_argument('--survival-cv-folds', type=int, default=5, metavar='F',
+                   help="with --survival-cv: folds per repeat, stratified by event, 2 <= F <= 100 (default 5)")
+    p.add_argument('--survival-cv-repeats', type=int, default=10, metavar='K',
+                   help="with --survival-cv: repeats of the fold split, 1 <= K <= 100 (default 10)")
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
@@ -279,6 +306,16 @@ def parse_arguments(argv=None):
         p.error("--signature-repeats must be an integer in [1, 100]")
     if args.signature_cv and args.numBiomarker > 64:
         p.error("--signature-cv needs -n <= 64: a signature has at most 128 genes")
+    if not 0 <= args.survival_cv <= 1 << 16:
+        p.error("--survival-cv must be an integer in [0, 65536]")
+    if not 2 <= args.survival_cv_folds <= 100:
+        p.error("--survival-cv-folds must be an integer in [2, 100]")
+    if not 1 <= args.survival_cv_repeats <= 100:
+        p.error("--survival-cv-repeats must be an integer in [1, 100]")
+    if args.survival_cv and args.survival is None:
+        p.error("--survival-cv needs --survival FILE")
+    if args.survival_cv and args.numBiomarker > 64:
+        p.error("--survival-cv needs -n <= 64: a signature has at most 128 genes")
     if not 0 <= args.neighbors <= 64:
         p.error("--neighbors must be an integer in [0, 64]")
     if not 0 <= args.kmeans_restarts <= 1024:
@@ -512,6 +549,30 @@ def write_survival(prefix, genes, lgroup, res, biomarkers):
                      for g, k, z, ps, pv, pm, qv in zip(genes, lgroup, res.Z, res.P_score, res.P, res.P_maxT, res.Q))
 
 
+def write_survival_cv(prefix, genes, res, biomarkers):
+    """One row per signature of a survival_cv.SurvivalCVResult: size, C, C_SD, P_random, the log-rank Z and P and the
+    hazard ratio with its 95 % CI of the risk groups (nan on the random rows), and how many of its genes are
+    biomarkers."""
+    bm = set(biomarkers)
+    nan = [float("nan")] * (len(res.names) - 3)
+    cols = [list(a) + nan for a in (res.p_random, res.logrank_z, res.logrank_p, res.hr, res.hr_low, res.hr_high)]
+    with open(prefix + "_survival_cv.txt", 'w') as f:
+        f.write('Signature\tSize\tC\tC_SD\tP_random\tLogRank_Z\tLogRank_P\tHR\tHR_Low\tHR_High\tBiomarkers\n')
+        for i, name in enumerate(res.names):
+            f.write('%s\t%d\t%.6f\t%.6f\t%.6g\t%.6f\t%.6g\t%.6g\t%.6g\t%.6g\t%d\n'
+                    % ((name, res.genes.shape[1], res.c_mean[i], res.c_sd[i]) + tuple(c[i] for c in cols)
+                       + (sum(genes[g] in bm for g in res.genes[i]),)))
+
+
+def write_risk(prefix, samples, time, event, res):
+    """One row per sample of the survival CV, in expression order: time, event, the biomarkers' pre-validated risk and
+    risk group (1 = high)."""
+    with open(prefix + "_risk.txt", 'w') as f:
+        f.write('SAMPLE\tTIME\tEVENT\tRISK\tGROUP\n')
+        f.writelines('%s\t%.10g\t%d\t%.6f\t%d\n' % (s, t, e, r, g)
+                     for s, t, e, r, g in zip(samples, time, event, res.risk[0], res.group[0]))
+
+
 def write_vectors(prefix, genes, mat):
     with open(prefix + "_vectors.txt", 'w') as f:
         f.write('GeneSymbol' + ''.join('\tV%d' % i for i in range(mat.shape[1])) + '\n')
@@ -605,6 +666,15 @@ def main(argv=None):
             sys.exit(1)
         print('    survival: %d of %d samples with a record, %d events, in %s'
               % (int(surv_used.sum()), n_samples, int(surv_event[surv_used].sum()), args.survival))
+        if args.survival_cv:
+            from . import survival_cv
+            try:
+                survival_cv.check_inputs(data['expr'], surv_time, surv_event, data['label'],
+                                         min(2 * args.numBiomarker, n_genes), args.survival_cv,
+                                         args.survival_cv_folds, args.survival_cv_repeats)
+            except ValueError as e:
+                print('ERROR: --survival-cv: %s' % e)
+                sys.exit(1)
     if args.kmeans_restarts and n_genes < 3:
         print('ERROR: --kmeans-restarts needs at least 3 common genes, found %d' % n_genes)
         sys.exit(1)
@@ -741,6 +811,14 @@ def main(argv=None):
                                                 surv_event[surv_used])
         print('    ' + survival.summary(surv_res, np.array([g in bm for g in genes]), label_z, label_p))
 
+    if args.survival_cv:
+        pos = {g: i for i, g in enumerate(genes)}
+        scv_res = survival_cv.survival_cv(data['expr'], surv_time, surv_event, data['label'],
+                                          np.array([pos[g] for g in biomarkers]), args.survival_cv,
+                                          folds=args.survival_cv_folds, repeats=args.survival_cv_repeats,
+                                          seed=args.seed)
+        print('    ' + survival_cv.summary(scv_res))
+
     print(">>> 7. Save results")
     write_biomarkers(args.RESULT_NAME, biomarkers)
     print('    %s_biomarkers.txt' % args.RESULT_NAME)
@@ -772,6 +850,12 @@ def main(argv=None):
     if args.survival is not None:
         write_survival(args.RESULT_NAME, genes, lgroup, surv_res, biomarkers)
         print('    %s_survival.txt' % args.RESULT_NAME)
+    if args.survival_cv:
+        write_survival_cv(args.RESULT_NAME, genes, scv_res, biomarkers)
+        print('    %s_survival_cv.txt' % args.RESULT_NAME)
+        write_risk(args.RESULT_NAME, [s for s, u in zip(data['sample'], surv_used) if u], surv_time[surv_used],
+                   surv_event[surv_used], scv_res)
+        print('    %s_risk.txt' % args.RESULT_NAME)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

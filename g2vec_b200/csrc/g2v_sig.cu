@@ -13,7 +13,7 @@
 //                     counts of the (positive, negative) pairs ordered and tied, and of the correct predictions.
 // Every floating-point sum is in a fixed order (per-thread chains, xor shuffle trees, fixed accumulator ownership);
 // the only atomics are integer ones, so the results are the same bits whatever the grid or the chunking.
-#include "g2v_common.cuh"
+#include "g2v_fit.cuh"
 
 namespace g2v {
 
@@ -76,49 +76,15 @@ sig_draw_kernel(int32_t G, int32_t p, uint64_t seed, int64_t r_begin, int64_t co
     }
 }
 
-// ---- fits ---------------------------------------------------------------------------------------------------
-constexpr int kFitThreads = 512, kFitWarps = kFitThreads / 32;
-constexpr int kTileS = 32;                             // samples per tile
-constexpr int kPerSample = kFitThreads / kTileS;      // threads per sample in the logit sums
-constexpr int kTS = kTileS + 4;                        // row stride of the tiles in doubles (conflict-free DMMA loads)
-constexpr int kMaxPad = ((G2V_SIG_MAX_SIZE + 1 + 7) / 8) * 8;            // 136
-constexpr int kMaxTiles = (kMaxPad / 8) * (kMaxPad / 8 + 1) / 2;           // 153 lower-triangle 8 x 8 tiles
-constexpr int kTilesPerWarp = (kMaxTiles + kFitWarps - 1) / kFitWarps;     // 10
-constexpr int kMaxIter = 100, kMaxHalvings = 40;
-constexpr double kStepTol = 1e-10, kArmijo = 1e-4;
-// The Armijo test allows the rounding of the loss sum: near the minimum the decrease it asks for falls below the
-// loss's last bits, and without the slack the search would halve 40 times and the tiny step t d would meet the stop
-// rule with the minimiser still a full Newton step away.
-constexpr double kLossSlack = 0x1p-40;
-
-__device__ __forceinline__ void dmma_8x8x4(double c[2], double a, double b) {
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                 : "+d"(c[0]), "+d"(c[1]) : "d"(a), "d"(b));
-}
-
-__host__ __device__ __forceinline__ int fit_pad(int p) { return ((p + 1 + 7) / 8) * 8; }
-__host__ __device__ __forceinline__ int tri(int i) { return i * (i + 1) / 2; }
+// ---- fits (the shared Newton machinery is in g2v_fit.cuh) ---------------------------------------------------
 __host__ __device__ __forceinline__ size_t fit_smem_doubles(int p) {
     const int P = fit_pad(p), P1 = p + 1;
     const int big = 2 * P * kTS > tri(P1) ? 2 * P * kTS : tri(P1);
     return (size_t)big + 7 * (size_t)P;
 }
 
-struct Fit {
-    const double *X;
-    int64_t n_pad;
-    int n, p, P1, P, f, n_tiles;
-    const uint8_t *y;
-    const int8_t *fold;                                // this repeat's row
-    const int32_t *genes;                              // this signature's row
-    double *Zs, *WZs, *Hp;                             // Hp aliases Zs / WZs once a pass is over
-    double *mu, *sd, *g;
-};
-
-// Per-CTA scratch of a fit at fixed size: one tile's weights, residuals and loss terms, the scalars the threads share,
-// and the 8 x 8 tiles of H's lower triangle as (I << 8) | J, I >= J.
-__shared__ double fit_w[kTileS], fit_r[kTileS], fit_lt[kTileS], fit_scal[4];
-__shared__ uint16_t fit_tiles[kMaxTiles];
+// Per-CTA scratch of a fit: one tile's weights, residuals and loss terms.
+__shared__ double fit_w[kTileS], fit_r[kTileS], fit_lt[kTileS];
 
 enum { kPassGram = 0, kPassLoss = 1, kPassScore = 2 };
 
@@ -224,81 +190,11 @@ __device__ double fit_pass(const Fit &c, const double *b, double *score_row) {
     return fit_scal[0];
 }
 
-// Training-fold mean and population SD of every feature, in fixed order; a feature constant over the training fold
-// (min == max) gets mu = that value and sd = 1, so its z is exactly 0.
-__device__ void fit_standardise(const Fit &c) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int j = 1 + warp; j <= c.p; j += kFitWarps) {
-        const double *xr = c.X + (int64_t)__ldg(c.genes + j - 1) * c.n_pad;
-        double s = 0.0, mn = INFINITY, mx = -INFINITY;
-        int cnt = 0;
-        for (int i = lane; i < c.n; i += 32)
-            if (c.fold[i] != c.f) {
-                const double v = __ldg(xr + i);
-                s += v; mn = fmin(mn, v); mx = fmax(mx, v); ++cnt;
-            }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            s += __shfl_xor_sync(0xffffffffu, s, o);
-            mn = fmin(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-            mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-            cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-        }
-        double mu = mn, sd = 1.0;
-        if (mn != mx) {
-            mu = s / cnt;
-            double ss = 0.0;
-            for (int i = lane; i < c.n; i += 32)
-                if (c.fold[i] != c.f) {
-                    const double d = __ldg(xr + i) - mu;
-                    ss = fma(d, d, ss);
-                }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-            sd = sqrt(ss / cnt);
-        }
-        if (lane == 0) { c.mu[j] = mu; c.sd[j] = sd; }
-    }
-    if (threadIdx.x == 0) { c.mu[0] = 0.0; c.sd[0] = 1.0; }
-    __syncthreads();
-}
-
-// Solves H d = g in place of the packed lower triangle Hp (Cholesky, right-looking, one barrier per column), then
-// L y = g and L^T d = y in one warp.  y and d go through tmp.
-__device__ void fit_solve(const Fit &c, double *d, double *tmp) {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    double *H = c.Hp;
-    for (int j = 0; j < c.P1; ++j) {
-        const double inv = 1.0 / sqrt(H[tri(j) + j]);
-        for (int i = j + 1 + warp; i < c.P1; i += kFitWarps) {
-            const double lij = H[tri(i) + j] * inv;
-            for (int k = j + 1 + lane; k <= i; k += 32) H[tri(i) + k] = fma(-lij, H[tri(k) + j] * inv, H[tri(i) + k]);
-        }
-        __syncthreads();                               // every thread has read column j and the diagonal
-        for (int i = j + tid; i < c.P1; i += kFitThreads) H[tri(i) + j] = i == j ? sqrt(H[tri(j) + j]) : H[tri(i) + j] * inv;
-        // column j is not read again before the next barrier: step j+1 reads columns j+1.. only
-    }
-    __syncthreads();
-    if (warp == 0) {
-        for (int j = lane; j < c.P1; j += 32) tmp[j] = c.g[j];
-        __syncwarp();
-        for (int j = 0; j < c.P1; ++j) {
-            const double yj = tmp[j] / H[tri(j) + j];
-            for (int i = j + 1 + lane; i < c.P1; i += 32) tmp[i] = fma(-H[tri(i) + j], yj, tmp[i]);
-            __syncwarp();
-            if (lane == 0) tmp[j] = yj;
-            __syncwarp();
-        }
-        for (int j = c.P1 - 1; j >= 0; --j) {
-            const double dj = tmp[j] / H[tri(j) + j];
-            for (int i = lane; i < j; i += 32) tmp[i] = fma(-H[tri(j) + i], dj, tmp[i]);
-            __syncwarp();
-            if (lane == 0) d[j] = dj;
-            __syncwarp();
-        }
-    }
-    __syncthreads();
-}
+struct LogisticModel {
+    const Fit &c;
+    __device__ double gram(const double *b) { return fit_pass<kPassGram>(c, b, nullptr); }
+    __device__ double loss(const double *b) { return fit_pass<kPassLoss>(c, b, nullptr); }
+};
 
 __global__ void __launch_bounds__(kFitThreads, 1)
 sig_fit_kernel(const double *__restrict__ X, int64_t n_pad, int32_t n, const uint8_t *__restrict__ y,
@@ -318,40 +214,13 @@ sig_fit_kernel(const double *__restrict__ X, int64_t n_pad, int32_t n, const uin
     c.Zs = sm; c.WZs = sm + c.P * kTS; c.Hp = sm;
     double *bt = sm + big, *bc = bt + c.P, *d = bc + c.P, *tmp = d + c.P;
     c.mu = tmp + c.P; c.sd = c.mu + c.P; c.g = c.sd + c.P;
-    for (int t = threadIdx.x; t < c.n_tiles; t += kFitThreads) {
-        int I = 0;
-        while (tri(I + 1) <= t) ++I;
-        fit_tiles[t] = (uint16_t)((I << 8) | (t - tri(I)));
-    }
+    fit_init_tiles(c.n_tiles);
     for (int j = threadIdx.x; j < c.P; j += kFitThreads) bt[j] = 0.0;
     fit_standardise(c);                                // ends with a barrier
-    double L = fit_pass<kPassGram>(c, bt, nullptr);
-    int it = 0;
-    bool conv = false;
-    while (it < kMaxIter) {
-        fit_solve(c, d, tmp);
-        if (threadIdx.x == 0) {
-            double gd = 0.0, dmax = 0.0;
-            for (int j = 0; j < c.P1; ++j) { gd = fma(c.g[j], d[j], gd); dmax = fmax(dmax, fabs(d[j])); }
-            fit_scal[1] = gd; fit_scal[2] = dmax;
-        }
-        __syncthreads();
-        const double gd = fit_scal[1], dmax = fit_scal[2];
-        double t = 1.0;
-        for (int h = 0;; ++h) {
-            for (int j = threadIdx.x; j < c.P1; j += kFitThreads) bc[j] = bt[j] - t * d[j];
-            __syncthreads();
-            const double Lc = fit_pass<kPassLoss>(c, bc, nullptr);
-            if (Lc <= L - kArmijo * t * gd + kLossSlack * fabs(L) || h == kMaxHalvings) break;
-            t *= 0.5;
-        }
-        for (int j = threadIdx.x; j < c.P1; j += kFitThreads) bt[j] = bc[j];
-        __syncthreads();
-        ++it;
-        if (t * dmax <= kStepTol) { conv = true; break; }
-        if (it == kMaxIter) break;
-        L = fit_pass<kPassGram>(c, bt, nullptr);
-    }
+    LogisticModel model{c};
+    int it;
+    bool conv;
+    fit_newton(c, model, bt, bc, d, tmp, it, conv);
     fit_pass<kPassScore>(c, bt, scores + (s * K + k) * (int64_t)n);
     if (threadIdx.x == 0) { n_iter[fit] = it; converged[fit] = conv ? 1 : 0; }
     if (s < beta_rows)

@@ -224,39 +224,61 @@ def chunk_rows(n, G, n_perm, max_chunk_bytes):
     return int(max(1, min(int(n_perm), int(max_chunk_bytes) // (2 * n + 8 * G))))
 
 
-def survival_test(expr, time, event, n_perm, seed=0, max_chunk_bytes=None):
-    """Permutation Cox score test of every gene against survival on the GPU.
-
-    expr: host float array [samples, genes]; time: one finite time >= 0 per sample (any unit); event: 1 for an event
-    (death or relapse), 0 for censored.  n_perm: B, 1 <= B <= 2^20 permutations of the expression against the
-    records (the observed pairing is not among them), with the Fisher-Yates draws of perm.perm_test's rows for the same
-    seed and sample count; seed: the Philox key (--seed).  max_chunk_bytes: bound on the device memory of one chunk's
-    rows and statistics (default: half the free device memory).  Makes 1 launch, then 3 per chunk.  Returns a
-    SurvivalResult; ValueError (before anything is uploaded) on inputs check_inputs refuses."""
-    prep = prepare(expr, time, event, n_perm)
+def _device():
+    """The torch device and stream of a run, and the upload helper; RuntimeError without a GPU."""
     import torch
     from . import _capi
     lib = _capi.load()
     if not torch.cuda.is_available():
         raise RuntimeError("g2vec_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     dev = torch.device("cuda", torch.cuda.current_device())
-    n, B, q = prep["n"], int(n_perm), prep["q"]
-    G = q.shape[1]
     up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    return lib, dev, torch.cuda.current_stream(dev).cuda_stream, up
+
+
+def _observed(prep, lib, dev, st, up):
+    """One g2v_surv_scores launch on the time order itself: (T_obs, U, V float64 [G], order, (flags_d, a_d, c_d)),
+    with order the genes by T descending, ties by gene index."""
+    import torch
+    from . import _capi
+    n, q = prep["n"], prep["q"]
+    G = q.shape[1]
     q_d = up(q.astype(np.int32))
-    flags_d, a_d, c_d, slot_d = up(prep["flags"]), up(prep["a"]), up(prep["c"]), up(prep["slot"])
+    flags_d, a_d, c_d = up(prep["flags"]), up(prep["a"]), up(prep["c"])
     ident_d = up(prep["order"].astype(np.uint16))
     T1 = torch.empty((1, G), dtype=torch.float64, device=dev)
     UV = torch.empty((2, 1, G), dtype=torch.float64, device=dev)
-    st = torch.cuda.current_stream(dev).cuda_stream
-    scores = lambda qq, idx, nb, T, uv: _capi.check(lib.g2v_surv_scores(
-        qq.data_ptr(), n, G, idx.data_ptr(), nb, flags_d.data_ptr(), a_d.data_ptr(), c_d.data_ptr(), T.data_ptr(),
-        uv, st), "g2v_surv_scores")
-    scores(q_d, ident_d, 1, T1, UV.data_ptr())
+    _capi.check(lib.g2v_surv_scores(q_d.data_ptr(), n, G, ident_d.data_ptr(), 1, flags_d.data_ptr(), a_d.data_ptr(),
+                                    c_d.data_ptr(), T1.data_ptr(), UV.data_ptr(), st), "g2v_surv_scores")
     T_obs, UVh = T1[0].cpu().numpy(), UV.cpu().numpy()
-    order = np.argsort(-T_obs, kind="stable")
+    return T_obs, UVh[0, 0], UVh[1, 0], np.argsort(-T_obs, kind="stable"), (flags_d, a_d, c_d)
+
+
+def rank_genes(expr, time, event):
+    """The genes by their observed Cox score statistic T, descending, ties by gene index: survival_test's `order`,
+    from the same device scan (one launch).  ValueError on inputs check_inputs refuses, RuntimeError without a GPU."""
+    prep = prepare(expr, time, event)
+    return _observed(prep, *_device())[3]
+
+
+def survival_test(expr, time, event, n_perm, seed=0, max_chunk_bytes=None):
+    """Permutation Cox score test of every gene against survival on the GPU.
+
+    expr: host float array [samples, genes]; time: one finite time >= 0 per sample (any unit); event: 1 for an event
+    (death or relapse), 0 for censored.  n_perm: B, 1 <= B <= 2^20 permutations of the expression against the
+    records (the observed pairing is not among them), with the Fisher-Yates draws of perm.perm_test's rows for the
+    same seed and sample count; seed: the Philox key (--seed).  max_chunk_bytes: bound on the device memory of one
+    chunk's rows and statistics (default: half the free device memory).  Makes 1 launch, then 3 per chunk.  Returns a
+    SurvivalResult; ValueError (before anything is uploaded) on inputs check_inputs refuses."""
+    prep = prepare(expr, time, event, n_perm)
+    import torch
+    from . import _capi
+    lib, dev, st, up = _device()
+    n, B, q = prep["n"], int(n_perm), prep["q"]
+    G = q.shape[1]
+    T_obs, U, V, order, (flags_d, a_d, c_d) = _observed(prep, lib, dev, st, up)
+    slot_d = up(prep["slot"])
     # the permutations run over the genes in rank order, so the tally reads every row of T front to back
-    del q_d
     qr_d = up(q[:, order].astype(np.int32))
     Tobs_d = up(T_obs[order])
     cnt = torch.zeros(G, dtype=torch.int64, device=dev)
@@ -270,10 +292,11 @@ def survival_test(expr, time, event, n_perm, seed=0, max_chunk_bytes=None):
     for b0 in range(0, B, rows):
         nb = min(rows, B - b0)
         _capi.check(lib.g2v_surv_rows(slot_d.data_ptr(), n, seed, b0, nb, idx.data_ptr(), st), "g2v_surv_rows")
-        scores(qr_d, idx, nb, T, None)
+        _capi.check(lib.g2v_surv_scores(qr_d.data_ptr(), n, G, idx.data_ptr(), nb, flags_d.data_ptr(),
+                                        a_d.data_ptr(), c_d.data_ptr(), T.data_ptr(), None, st), "g2v_surv_scores")
         _capi.check(lib.g2v_dcx_tally(T.data_ptr(), nb, G, Tobs_d.data_ptr(), cnt.data_ptr(), cmax.data_ptr(), st),
                     "g2v_dcx_tally")
-    return finish(prep, T_obs, UVh[0, 0], UVh[1, 0], order, cnt.cpu().numpy(), cmax.cpu().numpy(), B)
+    return finish(prep, T_obs, U, V, order, cnt.cpu().numpy(), cmax.cpu().numpy(), B)
 
 
 def label_score(label, time, event):

@@ -769,6 +769,34 @@ int g2v_sig_auc(const double *scores, const uint8_t *y, const int8_t *fold, int3
                 int32_t n_sig, int32_t cap, double *auc, double *acc, void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Cross-validated survival prediction from a gene signature: ridge Cox regression (DESIGN.md §4.33;
+ * g2vec_b200/survival_cv.py does the host side).  The sizes are bounded as for g2v_sig_*: 3 <= n <=
+ * G2V_SIG_MAX_SAMPLES, 1 <= K <= G2V_SIG_MAX_REPEATS, 2 <= F <= min(G2V_SIG_MAX_FOLDS, n / 2), 1 <= p <=
+ * min(G2V_SIG_MAX_SIZE, G), 1 <= n_sig and n_sig K F <= G2V_SIG_MAX_FITS.  Samples are in time positions (time
+ * descending, ties by sample index); flags [n] uint8 per position: bit 0 event, bit 1 last position of its time group.
+ * fold [K][n] int8 over the positions (g2v_sig_folds with y = the event bits).  A fit is (s, k, f), numbered
+ * (s K + k) F + f.
+ * g2v_cox_fit: one fit per CTA.  X [G][n_pad] float64 (gene-major over the positions, n_pad >= n); genes [n_sig][p].
+ *   Per fit, on the positions outside fold f: each feature standardised as g2v_sig_fit does (no intercept), then the
+ *   Breslow negative log partial likelihood plus |beta|^2 / 2 minimised by g2v_sig_fit's damped Newton.  ell
+ *   [n_sig * K * F][n] float64 is scratch.  scores [n_sig][K][n] = the out-of-fold eta of every position; n_iter and
+ *   converged [n_sig * K * F]; beta [beta_rows][K][F][p] for the first beta_rows signatures (beta may be NULL when
+ *   0).  g2v_cox_fit_smem_bytes(p): the fit kernel's dynamic shared memory (0 for p out of range).
+ * g2v_cox_concordance: counts [n_sig * K * F][3] int64 over the test fold of each fit: the pairs (i, j) with
+ *   grp[i] > grp[j] (grp [n] int32: the time group of each position, numbered in descending time) and i an event, and
+ *   of those the ones with score_i > score_j and score_i == score_j.  A test fold of at most cap positions (0 <= cap
+ *   <= min(n, G2V_COX_MAX_STAGED)) is staged in cap * 12 bytes of shared memory; a larger one is read from global
+ *   memory.
+ * Out-of-range sizes fail with nothing launched.  Never synchronises; no floating-point atomics. */
+#define G2V_COX_MAX_STAGED 18432
+size_t g2v_cox_fit_smem_bytes(int32_t p);
+int g2v_cox_fit(const double *X, int32_t G, int32_t n, int64_t n_pad, const uint8_t *flags, const int8_t *fold,
+                int32_t K, int32_t F, const int32_t *genes, int32_t n_sig, int32_t p, double *ell, double *scores,
+                int32_t *n_iter, uint8_t *converged, double *beta, int32_t beta_rows, void *stream);
+int g2v_cox_concordance(const double *scores, const uint8_t *flags, const int32_t *grp, const int8_t *fold, int32_t n,
+                        int32_t K, int32_t F, int32_t n_sig, int32_t cap, int64_t *counts, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Label-permutation test of differential co-expression for every network pair (DESIGN.md §4.30; g2vec_b200/diffcoex.py
  * does the host side).  A row is one labelling: an indicator [S_pad] u8 of its selected samples (g2v_perm_labels'
  * rows, or the all-ones and observed rows), padding 0.  q [G][S_pad] int32, gene-major, |q| <= 2^16, padding 0.
