@@ -100,8 +100,8 @@ at most the number of samples of either label), the same splits for every signat
 the same number of genes of largest |t| (``top_t``) and with R random signatures of that size (Floyd's sampling, seeded
 by ``--seed``).  The biomarkers and ``top_t`` were both chosen with every sample's label, so their AUCs are optimistic
 and comparable with each other; the random signatures are not selected, and P_random = (1 + #{random AUC >= AUC}) /
-(R + 1) says how often one does at least as well.  Nested re-selection (the walks and the training rerun inside every
-fold) is not done.  It needs ``-n`` <= 64 (at most 128 biomarkers).  The inputs are checked after step 2, where the run
+(R + 1) says how often one does at least as well.  For the AUC of the selection itself, rerun inside every fold, see
+``--nested-cv``, which scores on the same splits for the same F, K and ``--seed``.  It needs ``-n`` <= 64 (at most 128 biomarkers).  The inputs are checked after step 2, where the run
 stops with an ``ERROR`` if they are refused; after step 6 (on rank 0 only under torchrun) it prints a ``signature CV:``
 line, and step 7 also writes RESULT_NAME_signature.txt: per signature (biomarkers, top_t, random_1 .. random_R) its
 size, mean AUC over the K F fits, the SD of the K per-repeat AUCs, mean accuracy, P_random (``nan`` on random rows)
@@ -151,7 +151,28 @@ RESULT_NAME_survival_cv.txt: per signature (biomarkers, top_t, top_z, random_1 .
 fits, the SD of the K per-repeat means, P_random, the log-rank Z and P and the hazard ratio with its 95 % CI of the
 risk groups (``nan`` on random rows) and how many of its genes are biomarkers; and RESULT_NAME_risk.txt: per sample
 used, in the expression file's order, its time, event, the biomarkers' pre-validated risk and group (1 = high risk),
-ready for a Kaplan-Meier plot.
+ready for a Kaplan-Meier plot.  The biomarkers were chosen with every sample's label, so their C is optimistic;
+nested re-selection is done for the good / poor label only (``--nested-cv``), not for survival.
+
+``--nested-cv F`` (default 0: off; 2 <= F <= 100, F at most the number of samples of either label) adds nested
+cross-validation of the selection itself, on one GPU (DESIGN.md §4.34): over ``--nested-cv-repeats K`` (default 1,
+1 <= K <= 100) repeats of stratified F-fold splits of the samples with label 0 or 1 -- the splits ``--signature-cv``
+uses for the same F, K and ``--seed``; repeat k's split depends only on the labels, F, the seed and k -- steps 3 to 6
+run again on every outer training fold alone, with every option of the run, and the fit's list (``nested
+biomarkers``, at most 2 ``-n`` genes) and the same number of genes of largest |t| over those training samples
+(``nested top_t``) are scored on the held-out fold by ``--signature-cv``'s ridge logistic regression.  The test fold's
+expression and labels reach neither the selection nor the fit, so the nested AUC is the honest estimate of how well
+the selection generalises (Ambroise & McLachlan 2002); the run's own biomarkers and ``top_t`` are scored on the same
+splits, and the optimism is AUC(biomarkers) - AUC(nested biomarkers).  With ``--signature-cv R`` at the same F and K,
+P_random = (1 + #{random AUC >= nested AUC}) / (R + 1).  It needs ``-n`` <= 64 and refuses torchrun.  The inputs are
+checked after step 2, where the run stops with an ``ERROR`` if they are refused; after step 6 every outer fit prints
+one line (repeat, fold, training samples, windows, stop epoch, its two AUCs; its steps 3 and 4 print nothing), an
+outer fit that cannot train stops the run with an ``ERROR`` naming it, and the run prints a ``nested CV:`` line.  Step
+7 also writes RESULT_NAME_nested_cv.txt: per outer fit its repeat, fold, N_train, N_test, N_windows, Stop_epoch,
+Size, AUC and accuracy of the nested biomarkers and of nested top_t, the AUC of the biomarkers and of top_t, the
+Jaccard overlap with the biomarkers and its list, then the ``nested CV:`` line; and RESULT_NAME_nested_selection.txt:
+per gene, in the order of _lgroups.txt, its L-group, whether it is a biomarker, how many outer fits selected it, that
+count's share of the K F fits, and how many selected it from the good and from the poor L-group.
 
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
@@ -280,6 +301,12 @@ def parse_arguments(argv=None):
                    help="with --survival-cv: folds per repeat, stratified by event, 2 <= F <= 100 (default 5)")
     p.add_argument('--survival-cv-repeats', type=int, default=10, metavar='K',
                    help="with --survival-cv: repeats of the fold split, 1 <= K <= 100 (default 10)")
+    p.add_argument('--nested-cv', type=int, default=0, metavar='F',
+                   help="nested cross-validation of the selection: steps 3-6 rerun on every training fold of "
+                        "stratified F-fold splits (2 <= F <= 100) and the list's ridge logistic AUC on the held-out "
+                        "fold, in RESULT_NAME_nested_cv.txt and RESULT_NAME_nested_selection.txt; 0 (default) = off")
+    p.add_argument('--nested-cv-repeats', type=int, default=1, metavar='K',
+                   help="with --nested-cv: repeats of the fold split, 1 <= K <= 100 (default 1)")
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
@@ -316,6 +343,12 @@ def parse_arguments(argv=None):
         p.error("--survival-cv needs --survival FILE")
     if args.survival_cv and args.numBiomarker > 64:
         p.error("--survival-cv needs -n <= 64: a signature has at most 128 genes")
+    if not (args.nested_cv == 0 or 2 <= args.nested_cv <= 100):
+        p.error("--nested-cv must be 0 (off) or an integer in [2, 100]")
+    if not 1 <= args.nested_cv_repeats <= 100:
+        p.error("--nested-cv-repeats must be an integer in [1, 100]")
+    if args.nested_cv and args.numBiomarker > 64:
+        p.error("--nested-cv needs -n <= 64: a signature has at most 128 genes")
     if not 0 <= args.neighbors <= 64:
         p.error("--neighbors must be an integer in [0, 64]")
     if not 0 <= args.kmeans_restarts <= 1024:
@@ -573,6 +606,36 @@ def write_risk(prefix, samples, time, event, res):
                      for s, t, e, r, g in zip(samples, time, event, res.risk[0], res.group[0]))
 
 
+def write_nested_cv(prefix, genes, res):
+    """One row per outer fit of a nested.NestedResult (repeat-major, 1-based): its sizes, windows, stop epoch, list
+    size, the AUC and accuracy of its list and of top_t at that size, the full run's biomarkers' and top_t's AUC on
+    the same fold, the Jaccard overlap with the full run's list and the list itself; then the nested CV line."""
+    from .nested import summary
+    K, F = res.n_train.shape
+    with open(prefix + "_nested_cv.txt", 'w') as f:
+        f.write('Repeat\tFold\tN_train\tN_test\tN_windows\tStop_epoch\tSize\tAUC_nested\tACC_nested\tAUC_nested_top_t\t'
+                'ACC_nested_top_t\tAUC_biomarkers\tAUC_top_t\tJaccard\tBiomarkers\n')
+        for k in range(K):
+            for j in range(F):
+                bm = res.biomarkers[k][j]
+                f.write('%d\t%d\t%d\t%d\t%d\t%d\t%d\t%.6f\t%.6f\t%.6f\t%.6f\t%.6f\t%.6f\t%.6f\t%s\n'
+                        % (k + 1, j + 1, res.n_train[k, j], res.n_test[k, j], res.n_windows[k, j], res.stop_epoch[k, j],
+                           len(bm), res.auc[0, k, j], res.acc[0, k, j], res.auc[1, k, j], res.acc[1, k, j],
+                           res.auc[2, k, j], res.auc[3, k, j], res.jaccard[k, j], ','.join(genes[g] for g in bm)))
+        f.write(summary(res) + '\n')
+
+
+def write_nested_selection(prefix, genes, lgroup, res, biomarkers):
+    """One row per gene in the order of _lgroups.txt: L-group, biomarker 0/1, how many outer fits selected it, that
+    count over the fits, and how many selected it from the good and from the poor L-group."""
+    bm = set(biomarkers)
+    with open(prefix + "_nested_selection.txt", 'w') as f:
+        f.write('GeneSymbol\tLgroup(0:good,1:poor,2:other)\tBiomarker\tSelected\tFrequency\tSelectedGood\tSelectedPoor\n')
+        f.writelines('%s\t%d\t%d\t%d\t%.6f\t%d\t%d\n' % (g, k, g in bm, n, q, a, b)
+                     for g, k, n, q, a, b in zip(genes, lgroup, res.selected, res.frequency, res.selected_good,
+                                                 res.selected_poor))
+
+
 def write_vectors(prefix, genes, mat):
     with open(prefix + "_vectors.txt", 'w') as f:
         f.write('GeneSymbol' + ''.join('\tV%d' % i for i in range(mat.shape[1])) + '\n')
@@ -599,6 +662,11 @@ def _distributed():
 
 def main(argv=None):
     args = parse_arguments(argv)
+    if args.nested_cv:
+        import os
+        if int(os.environ.get("WORLD_SIZE", "1")) > 1:            # before any process group or device
+            sys.stdout.write('ERROR: --nested-cv: the nested loop runs on one GPU; run without torchrun\n')
+            sys.exit(1)
     rank, world, dist = _distributed()
     import builtins
     print = builtins.print if rank == 0 else (lambda *a, **k: None)   # noqa: A001  every rank computes, rank 0 talks
@@ -675,52 +743,37 @@ def main(argv=None):
             except ValueError as e:
                 print('ERROR: --survival-cv: %s' % e)
                 sys.exit(1)
+    if args.nested_cv:
+        from . import nested
+        try:                                           # fail now rather than after training
+            nested.check_inputs(data['expr'], data['label'], args.nested_cv, args.nested_cv_repeats,
+                                min(2 * args.numBiomarker, n_genes))
+        except ValueError as e:
+            print('ERROR: --nested-cv: %s' % e)
+            sys.exit(1)
     if args.kmeans_restarts and n_genes < 3:
         print('ERROR: --kmeans-restarts needs at least 3 common genes, found %d' % n_genes)
         sys.exit(1)
 
     print('>>> 3. Generate random paths from each group')
     print('    *** most time consuming step ***')
-    from . import graph, paths, walks, cbow           # needs the GPU from here on
+    from . import paths, pipeline, walks              # needs the GPU from here on
     if args.walk_q != 1.0:
         a_near, a_far = walks.walk_bias(args.walk_q)
         print('    walk q  : %g\t(in-out multipliers %d near, %d far: effective q = %.6g)'
               % (args.walk_q, a_near, a_far, walks.effective_q(args.walk_q)))
     if args.correlation != 'pearson' or args.min_corr != 0.5:
         print('    correlation: %s (|r| > %g)' % (args.correlation, args.min_corr))
-    idx = {g: i for i, g in enumerate(data['gene'])}
-    src = np.fromiter((idx[e[0]] for e in network['edge']), dtype=np.int32, count=len(network['edge']))
-    dst = np.fromiter((idx[e[1]] for e in network['edge']), dtype=np.int32, count=len(network['edge']))
-    import torch
-    n_total = n_genes * args.numRepetition                     # walkers per group: w = repetition * n_genes + start gene
-    L = args.lenPath
-    dev = torch.device("cuda", torch.cuda.current_device())
-    rows = torch.empty((2 * n_total, L), dtype=torch.int32, device=dev)
-    lens = torch.empty(2 * n_total, dtype=torch.int32, device=dev)
-    key = torch.empty(2 * n_total, dtype=torch.int64, device=dev)
-    for i, _group in enumerate(['g', 'p']):
-        rp, col, w = graph.group_csr_gpu(data['expr'], data['label'], i, src, dst, threshold=args.min_corr,
-                                         method=args.correlation)
-        if args.diff_coexpression:                     # which pairs this group's graph kept, either direction
-            dcx_in_graph.append(diffcoex.graph_pairs(dcx_pairs, n_genes, rp.cpu().numpy(), col.cpu().numpy()))
-        wg = walks.WalkGraph(rp, col, weights=w)
-        sl = slice(i * n_total, (i + 1) * n_total)
-        if dist is None:
-            # tuple(sorted(path)) is fused into the sampler: sorted rows + their 64-bit keys come back
-            walks.generate_paths(wg, L, args.numRepetition, seed=args.seed, group=i, canonical=True,
-                                 out=(rows[sl], lens[sl], key[sl]), q=args.walk_q)
-        else:
-            # walkers rank, rank+world, ...: no collective during the walk (counter-based RNG); one all_gather after,
-            # rows put back at their walker index so that every rank holds the 1-GPU arrays (same window order,
-            # hence the same --seed split, whatever the number of GPUs)
-            r_, l_, k_ = walks.generate_paths(wg, L, args.numRepetition, seed=args.seed, group=i, canonical=True,
-                                              walker_begin=rank, walker_stride=world, q=args.walk_q)
-            rows[sl], lens[sl], key[sl] = paths.gather_walker_shards(dist, world, n_total, r_, l_, k_)
-    group = torch.cat([torch.zeros(n_total, dtype=torch.uint8, device=dev), torch.ones(n_total, dtype=torch.uint8, device=dev)])
-    w_rowptr, w_gene, w_label, code = paths.build_windows(rows, lens, key, group, n_genes)
-    del rows, lens, key, group
+    src, dst = pipeline.edge_arrays(data['gene'], network['edge'])
+    on_graph = None
+    if args.diff_coexpression:                         # which pairs each group's graph kept, either direction
+        on_graph = lambda i, rp, col: dcx_in_graph.append(diffcoex.graph_pairs(dcx_pairs, n_genes, rp.cpu().numpy(),
+                                                                                col.cpu().numpy()))
+    windows = pipeline.walk_windows(data['expr'], data['label'], src, dst, n_genes, args, dist=dist, rank=rank,
+                                    world=world, on_graph=on_graph)
+    code = windows[3]
     geneFreq = paths.gene_freq_dict(code, data['gene'])
-    print("    n_paths : %d" % int(w_label.shape[0]))
+    print("    n_paths : %d" % int(windows[2].shape[0]))
     print("    n_genes : %d\t(genes in good or poor random paths)" % len(geneFreq))
     if args.neighbors or args.tsne:
         from . import neighbors
@@ -738,12 +791,8 @@ def main(argv=None):
             sys.exit(1)
 
     print(">>> 4. Compute distributed representations using modified CBOW")
-    mat = cbow.train_cbow(w_rowptr, w_gene, w_label, n_genes, args.sizeHiddenlayer, args.learningRate,
-                          max_epoch=args.epoch, seed=args.seed, log=print, algo=args.algo,   # print is silent off rank 0
-                          batch=args.batch, optimizer=args.optimizer, reshuffle=args.reshuffle,
-                          deterministic=args.deterministic, patience=args.patience, lr_patience=args.lr_patience,
-                          lr_factor=args.lr_factor, min_lr=args.min_lr, weight_decay=args.weight_decay,
-                          monitor=args.monitor, class_weight=args.class_weight)
+    mat = pipeline.train(windows, n_genes, args, log=print)   # print is silent off rank 0
+    del windows
     genes = data['gene']
     if rank != 0:
         dist.barrier()
@@ -751,24 +800,13 @@ def main(argv=None):
         return
 
     print('>>> 5. Find L-groups')
+    lgroup, km = pipeline.find_lgroups(mat, args)
     if args.kmeans_restarts:
         from . import kmeans
-        km = kmeans.kmeans_lgroups(mat, args.kmeans_restarts, seed=args.seed)
-        lgroup = km.lgroups
         print('    ' + kmeans.summary(km))
-    else:
-        lgroup = find_lgroups(mat, genes, geneFreq)
 
     print(">>> 6. Select biomarkers with gene scores")
-    biomarkers = []
-    for i in (0, 1):
-        sel = lgroup == i
-        d = minmax(np.linalg.norm(mat[sel], axis=1))
-        t = minmax(tscores(data['expr'][:, sel], data['label']))
-        score = 0.5 * (d + t)
-        ranked = sorted(zip(genes[sel], score), key=lambda gs: gs[1], reverse=True)
-        biomarkers += sorted(g for g, _ in ranked[:args.numBiomarker])
-    biomarkers = sorted(biomarkers)
+    biomarkers = pipeline.select_biomarkers(mat, lgroup, data['expr'], data['label'], genes, args.numBiomarker)
     if args.permutations:
         res = perm.perm_test(data['expr'], data['label'], args.permutations, seed=args.seed)
         sig = res.P_maxT <= 0.05
@@ -819,6 +857,18 @@ def main(argv=None):
                                           seed=args.seed)
         print('    ' + survival_cv.summary(scv_res))
 
+    if args.nested_cv:
+        same_splits = (args.signature_cv and args.signature_folds == args.nested_cv
+                       and args.signature_repeats == args.nested_cv_repeats)
+        try:
+            ncv_res = nested.nested_cv(data['expr'], data['label'], src, dst, genes, args, biomarkers,
+                                       random_auc=sig_res.auc_mean[2:] if same_splits else None,
+                                       log=lambda line: print('    ' + line))
+        except ValueError as e:
+            print('ERROR: --nested-cv: %s' % e)
+            sys.exit(1)
+        print('    ' + nested.summary(ncv_res))
+
     print(">>> 7. Save results")
     write_biomarkers(args.RESULT_NAME, biomarkers)
     print('    %s_biomarkers.txt' % args.RESULT_NAME)
@@ -856,6 +906,11 @@ def main(argv=None):
         write_risk(args.RESULT_NAME, [s for s, u in zip(data['sample'], surv_used) if u], surv_time[surv_used],
                    surv_event[surv_used], scv_res)
         print('    %s_risk.txt' % args.RESULT_NAME)
+    if args.nested_cv:
+        write_nested_cv(args.RESULT_NAME, genes, ncv_res)
+        print('    %s_nested_cv.txt' % args.RESULT_NAME)
+        write_nested_selection(args.RESULT_NAME, genes, lgroup, ncv_res, biomarkers)
+        print('    %s_nested_selection.txt' % args.RESULT_NAME)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

@@ -4,12 +4,14 @@ biomarkers, for the same number of genes of largest |t| (top_t) and for R random
 
 The biomarkers and top_t were both chosen with every sample's label, so their AUCs are optimistic and comparable with
 each other (Ambroise & McLachlan 2002); the random signatures are not selected, and most random gene sets already carry
-some of the outcome (Venet et al. 2011), so P_random says how often a random signature does at least as well.  Nested
-re-selection (rerunning the walks and the training inside every fold) is not done.
+some of the outcome (Venet et al. 2011), so P_random says how often a random signature does at least as well.  The
+honest AUC of the selection itself, with steps 3-6 rerun on every training fold, is nested.nested_cv
+(``--nested-cv``), which scores on these same splits with cv_fits.
 
 Host side (NumPy): the checks, top_t from perm.prepare's exact ranking, X as float64 gene-major, chunking over whole
 signatures and the summaries.  Device side (csrc/g2v_sig.cu): g2v_sig_folds once, then per chunk g2v_sig_draw,
-g2v_sig_fit (one CTA per fit, Newton on the device, Gram matrix on the FP64 tensor cores) and g2v_sig_auc.
+g2v_sig_fit (one CTA per fit, Newton on the device, Gram matrix on the FP64 tensor cores) and g2v_sig_auc, in
+cv_fits.
 """
 from collections import namedtuple
 
@@ -112,9 +114,28 @@ def signature_cv(expr, label, signature, n_random, folds=5, repeats=10, seed=0, 
     G = x.shape[1]
     if sig.dtype.kind not in "iu" or (sig.size and (sig.min() < 0 or sig.max() >= G)) or np.unique(sig).size != sig.size:
         raise ValueError("signature test: the signature must be distinct gene indices in [0, %d)" % G)
-    n, p, R, K, F = x.shape[0], int(sig.shape[0]), int(n_random), int(repeats), int(folds)
-    S = R + 2
+    p, R, K, F = int(sig.shape[0]), int(n_random), int(repeats), int(folds)
     head = np.stack([np.sort(sig).astype(np.int32), top_t(expr, label, p)])
+    genes, fold, auc, acc, n_iter, conv, beta = cv_fits(x, lab, head, R, K, F, seed, max_chunk_bytes=max_chunk_bytes)
+    auc_mean, auc_sd, acc_mean, p_random = summarise(auc, acc, R)
+    return SignatureResult(names=list(NAMES) + ["random_%d" % r for r in range(1, R + 1)], genes=genes, folds=fold,
+                           auc=auc, acc=acc, n_iter=n_iter, converged=int(conv.sum()), beta=beta, auc_mean=auc_mean,
+                           auc_sd=auc_sd, acc_mean=acc_mean, p_random=p_random)
+
+
+def cv_fits(x, lab, head, n_random, repeats, folds, seed, fold=None, cap=None, max_chunk_bytes=None):
+    """The device part of signature_cv, also run by nested.nested_cv: the fits and test-fold scores of S = H + R
+    signatures, the H rows of head [H, p] (sorted distinct gene indices) then random_1 .. random_R (g2v_sig_draw).
+
+    x float64 [n, G] and lab [n] in {0, 1}: the used samples, as check_inputs returns them (not checked here).  fold:
+    None to split with g2v_sig_folds (K repeats of stratified F-fold at seed), or an int8 [K, n] array of test folds
+    0..F-1 to fit on instead.  cap: the largest test fold g2v_sig_auc scores (a larger fold gets NaN); default the
+    largest stratified fold.  Returns (genes int32 [S, p], fold int8 [K, n], auc, acc float64 [S, K, F], n_iter int32
+    [S, K, F], converged uint8 [S, K, F], beta float64 [H, K, F, p + 1])."""
+    n, G = x.shape
+    H, p = head.shape
+    R, K, F = int(n_random), int(repeats), int(folds)
+    S = H + R
     import torch
     from . import _capi
     lib = _capi.load()
@@ -129,18 +150,22 @@ def signature_cv(expr, label, signature, n_random, folds=5, repeats=10, seed=0, 
     del Xt
     y_d = torch.from_numpy(lab.astype(np.uint8)).to(dev)
     seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-    fold_d = torch.empty((K, n), dtype=torch.int8, device=dev)
-    _capi.check(lib.g2v_sig_folds(y_d.data_ptr(), n, K, F, seed, fold_d.data_ptr(), st), "g2v_sig_folds")
-    n0, n1 = int((lab == 0).sum()), int((lab == 1).sum())
-    cap = -(-n0 // F) + -(-n1 // F)                    # the largest test fold
+    if fold is None:
+        fold_d = torch.empty((K, n), dtype=torch.int8, device=dev)
+        _capi.check(lib.g2v_sig_folds(y_d.data_ptr(), n, K, F, seed, fold_d.data_ptr(), st), "g2v_sig_folds")
+    else:
+        fold_d = torch.from_numpy(np.ascontiguousarray(fold, dtype=np.int8)).to(dev)
+    if cap is None:
+        n0, n1 = int((lab == 0).sum()), int((lab == 1).sum())
+        cap = -(-n0 // F) + -(-n1 // F)                # the largest test fold
     if max_chunk_bytes is None:
         max_chunk_bytes = torch.cuda.mem_get_info(dev)[0] // 2
     rows = chunk_signatures(S, n, p, K, F, max_chunk_bytes)
     genes = np.empty((S, p), dtype=np.int32)
-    genes[:2] = head
+    genes[:H] = head
     auc = np.empty((S, K, F)); acc = np.empty((S, K, F))
     n_iter = np.empty((S, K, F), dtype=np.int32); conv = np.empty((S, K, F), dtype=np.uint8)
-    beta = torch.empty((2, K, F, p + 1), dtype=torch.float64, device=dev)
+    beta = torch.empty((H, K, F, p + 1), dtype=torch.float64, device=dev)
     g_d = torch.empty((rows, p), dtype=torch.int32, device=dev)
     sc_d = torch.empty((rows, K, n), dtype=torch.float64, device=dev)
     auc_d, acc_d = (torch.empty((rows, K, F), dtype=torch.float64, device=dev) for _ in range(2))
@@ -148,11 +173,11 @@ def signature_cv(expr, label, signature, n_random, folds=5, repeats=10, seed=0, 
     cv_d = torch.empty((rows, K, F), dtype=torch.uint8, device=dev)
     for s0 in range(0, S, rows):
         ns = min(rows, S - s0)
-        fixed = min(ns, max(0, 2 - s0))                # rows of this chunk that are biomarkers / top_t
+        fixed = min(ns, max(0, H - s0))                # rows of this chunk that come from head
         if fixed:
             g_d[:fixed] = torch.from_numpy(head[s0:s0 + fixed]).to(dev)
         if ns > fixed:
-            _capi.check(lib.g2v_sig_draw(G, p, seed, s0 + fixed - 1, ns - fixed, g_d[fixed].data_ptr(), st),
+            _capi.check(lib.g2v_sig_draw(G, p, seed, s0 + fixed - H + 1, ns - fixed, g_d[fixed].data_ptr(), st),
                         "g2v_sig_draw")
         _capi.check(lib.g2v_sig_fit(X_d.data_ptr(), G, n, n_pad, y_d.data_ptr(), fold_d.data_ptr(), K, F,
                                     g_d.data_ptr(), ns, p, sc_d.data_ptr(), it_d.data_ptr(), cv_d.data_ptr(),
@@ -163,8 +188,4 @@ def signature_cv(expr, label, signature, n_random, folds=5, repeats=10, seed=0, 
         genes[sl] = g_d[:ns].cpu().numpy()
         auc[sl] = auc_d[:ns].cpu().numpy(); acc[sl] = acc_d[:ns].cpu().numpy()
         n_iter[sl] = it_d[:ns].cpu().numpy(); conv[sl] = cv_d[:ns].cpu().numpy()
-    auc_mean, auc_sd, acc_mean, p_random = summarise(auc, acc, R)
-    return SignatureResult(names=list(NAMES) + ["random_%d" % r for r in range(1, R + 1)], genes=genes,
-                           folds=fold_d.cpu().numpy(), auc=auc, acc=acc, n_iter=n_iter,
-                           converged=int(conv.sum()), beta=beta.cpu().numpy(), auc_mean=auc_mean,
-                           auc_sd=auc_sd, acc_mean=acc_mean, p_random=p_random)
+    return genes, fold_d.cpu().numpy(), auc, acc, n_iter, conv, beta.cpu().numpy()

@@ -7,7 +7,8 @@ get pre-validated risk groups (Tibshirani & Efron 2002): each sample's out-of-fo
 split at the median, with a log-rank test and the hazard ratio of the high-risk group.
 
 The biomarkers, top_t and top_z were chosen with every sample, so their C are optimistic and comparable with each
-other; nested re-selection is not done.
+other.  Nested re-selection (steps 3-6 rerun on every training fold) exists for the good / poor label only
+(nested.nested_cv, ``--nested-cv``); a nested survival C is not done.
 
 Host side (NumPy): the checks, top_t (signature.top_t), X as float64 gene-major over the time positions, chunking over
 whole signatures and the summaries.  Device side: g2v_sig_folds once (y = the event flags), g2v_surv_scores once for
