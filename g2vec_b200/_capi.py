@@ -166,6 +166,10 @@ SIGNATURES = {
     "g2v_dcx_sums": (ctypes.c_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
                                     _vp, _vp, _vp]),
     "g2v_dcx_tally": (ctypes.c_int, [_vp, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "g2v_nr_seed": (ctypes.c_int, [_vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _i64, _vp]),
+    "g2v_nr_step": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _i64, ctypes.c_double, _vp]),
+    "g2v_nr_tile_cols": (_i64, [_i32]),
+    "g2v_nr_tally": (ctypes.c_int, [_vp, _i32, _i64, _i64, _vp, _vp, _vp]),
     "g2v_surv_rows": (ctypes.c_int, [_vp, _i32, _u64, _i64, _i64, _vp, _vp]),
     "g2v_surv_scores": (ctypes.c_int, [_vp, _i32, _i32, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "g2v_paths_canonicalise":(ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),

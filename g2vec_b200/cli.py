@@ -174,6 +174,24 @@ Jaccard overlap with the biomarkers and its list, then the ``nested CV:`` line; 
 per gene, in the order of _lgroups.txt, its L-group, whether it is a biomarker, how many outer fits selected it, that
 count's share of the K F fits, and how many selected it from the good and from the poor L-group.
 
+``--netrank B`` (default 0: off; 1 <= B <= 2^20) adds network-propagated gene scores, NetRank (Winter et al. 2012;
+GeneRank, Morrison et al. 2005), with a label-permutation test, on the GPU (DESIGN.md §4.35).  The network is the
+distinct unordered gene pairs of step 2's edges, as ``--diff-coexpression`` takes them, unweighted; each gene's seed is
+its |point-biserial r| with the good / poor label (the |t| of ``--permutations`` on another scale), and the score is
+personalised PageRank of the seeds, x_j = (1 - d) s_j + d sum over the neighbours i of x_i / deg_i, iterated from
+x = s until d^T <= 1e-12, with ``--netrank-damping d`` (default 0.5; finite, 0 <= d <= 0.95; 0 gives the seeds
+themselves).  A gene with little difference of its own can rank high when its neighbourhood differs.  B label
+permutations, seeded by ``--seed`` and the same as ``--permutations`` makes for the same B, give each gene a raw P and
+the Benjamini-Hochberg Q (no maxT: the null spread of a score grows with the gene's degree).  ``top_netrank`` is the
+genes of highest score (ties by position), as many as there are biomarkers.  The inputs are checked after step 2
+(labels 0 and 1 both present, 3 to 32768 samples with label 0 or 1, finite expression values, 1 to 2^26 pairs), where
+the run stops with an ``ERROR`` if they are refused; after step 6 (on rank 0 only under torchrun) it prints a
+``netrank:`` line (how many genes have Q <= 0.05 and how many of those are biomarkers, and the Jaccard overlap of
+``top_netrank`` with the biomarkers; with ``--signature-cv`` also the cross-validated AUC of ``top_netrank`` on the same
+splits, beside the biomarkers'), and step 7 also writes RESULT_NAME_netrank.txt: per gene, in the order of _lgroups.txt, its L-group, degree, seed S, score,
+rank (1 = highest score), P, Q and whether it is a biomarker, followed by the same line.  None of these depend on
+training.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle`` or ``--class-weight``, at every table size (DESIGN.md §4.13); ``--class-weight 1,1`` writes the
@@ -307,6 +325,12 @@ def parse_arguments(argv=None):
                         "fold, in RESULT_NAME_nested_cv.txt and RESULT_NAME_nested_selection.txt; 0 (default) = off")
     p.add_argument('--nested-cv-repeats', type=int, default=1, metavar='K',
                    help="with --nested-cv: repeats of the fold split, 1 <= K <= 100 (default 1)")
+    p.add_argument('--netrank', type=int, default=0, metavar='B',
+                   help="network-propagated gene scores (NetRank: personalised PageRank of each gene's |r| with the "
+                        "label over the network) with a label-permutation test of B permutations (1 <= B <= 2^20): P "
+                        "and Benjamini-Hochberg Q in RESULT_NAME_netrank.txt; 0 (default) = off")
+    p.add_argument('--netrank-damping', type=float, default=0.5, metavar='d',
+                   help="with --netrank: the damping d, a finite number in [0, 0.95] (default 0.5; 0 = no propagation)")
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
@@ -349,6 +373,10 @@ def parse_arguments(argv=None):
         p.error("--nested-cv-repeats must be an integer in [1, 100]")
     if args.nested_cv and args.numBiomarker > 64:
         p.error("--nested-cv needs -n <= 64: a signature has at most 128 genes")
+    if not 0 <= args.netrank <= 1 << 20:
+        p.error("--netrank must be an integer in [0, 2^20]")
+    if not (np.isfinite(args.netrank_damping) and 0.0 <= args.netrank_damping <= 0.95):
+        p.error("--netrank-damping must be a finite number in [0, 0.95]")
     if not 0 <= args.neighbors <= 64:
         p.error("--neighbors must be an integer in [0, 64]")
     if not 0 <= args.kmeans_restarts <= 1024:
@@ -636,6 +664,20 @@ def write_nested_selection(prefix, genes, lgroup, res, biomarkers):
                                                  res.selected_poor))
 
 
+def write_netrank(prefix, genes, lgroup, res, biomarkers, line):
+    """One row per gene in the order of _lgroups.txt: L-group, degree, seed S, score, rank (1 = highest score), P and Q
+    of a netrank.NetRankResult, biomarker 0/1; then the netrank line."""
+    bm = set(biomarkers)
+    rank = np.empty(res.order.shape[0], dtype=np.int64)
+    rank[res.order] = np.arange(1, res.order.shape[0] + 1)
+    with open(prefix + "_netrank.txt", 'w') as f:
+        f.write('GeneSymbol\tLgroup(0:good,1:poor,2:other)\tDegree\tS\tScore\tRank\tP\tQ\tBiomarker\n')
+        f.writelines('%s\t%d\t%d\t%.6f\t%.6f\t%d\t%.6g\t%.6g\t%d\n' % (g, k, dg, sv, sc, r, pv, qv, g in bm)
+                     for g, k, dg, sv, sc, r, pv, qv in zip(genes, lgroup, res.degree, res.S, res.score, rank, res.P,
+                                                          res.Q))
+        f.write(line + '\n')
+
+
 def write_vectors(prefix, genes, mat):
     with open(prefix + "_vectors.txt", 'w') as f:
         f.write('GeneSymbol' + ''.join('\tV%d' % i for i in range(mat.shape[1])) + '\n')
@@ -722,6 +764,16 @@ def main(argv=None):
             print('ERROR: --diff-coexpression: %s' % e)
             sys.exit(1)
         dcx_in_graph = []
+    if args.netrank:
+        from . import diffcoex, netrank
+        try:                                           # fail now rather than after training
+            gi = {g: i for i, g in enumerate(data['gene'])}
+            nr_pairs = diffcoex.pairs_from_edges([gi[e[0]] for e in network['edge']],
+                                                 [gi[e[1]] for e in network['edge']])
+            netrank.check_inputs(data['expr'], data['label'], nr_pairs, args.netrank, args.netrank_damping)
+        except ValueError as e:
+            print('ERROR: --netrank: %s' % e)
+            sys.exit(1)
     if args.survival is not None:
         from . import survival
         try:                                           # fail now rather than after training
@@ -841,6 +893,21 @@ def main(argv=None):
         dcx_bm = is_bm[dcx_pairs[:, 0]] + is_bm[dcx_pairs[:, 1]]
         print('    ' + diffcoex.summary(dcx_res, dcx_in_graph[0], dcx_in_graph[1], dcx_bm))
 
+    if args.netrank:
+        nr_res = netrank.netrank_test(data['expr'], data['label'], nr_pairs, args.netrank, damping=args.netrank_damping,
+                                      seed=args.seed)
+        bm = set(biomarkers)
+        nr_bm = np.array([g in bm for g in genes])
+        nr_auc = None
+        if args.signature_cv:                          # top_netrank on --signature-cv's splits, beside the biomarkers
+            from .perm import check_inputs as used_samples
+            head = netrank.top_netrank(nr_res, len(biomarkers))[None, :]
+            auc = signature.cv_fits(*used_samples(data['expr'], data['label'], 1), head, 0, args.signature_repeats,
+                                    args.signature_folds, args.seed)[2]
+            nr_auc = (float(auc[0].reshape(-1).mean()), float(sig_res.auc_mean[0]))
+        nr_line = netrank.summary(nr_res, args.netrank_damping, nr_pairs.shape[0], nr_bm, nr_auc)
+        print('    ' + nr_line)
+
     if args.survival is not None:
         surv_res = survival.survival_test(data['expr'][surv_used], surv_time[surv_used], surv_event[surv_used],
                                           args.survival_permutations, seed=args.seed)
@@ -897,6 +964,9 @@ def main(argv=None):
     if args.diff_coexpression:
         write_diffcoex(args.RESULT_NAME, genes, dcx_res, dcx_in_graph[0], dcx_in_graph[1], dcx_bm)
         print('    %s_diffcoex.txt' % args.RESULT_NAME)
+    if args.netrank:
+        write_netrank(args.RESULT_NAME, genes, lgroup, nr_res, biomarkers, nr_line)
+        print('    %s_netrank.txt' % args.RESULT_NAME)
     if args.survival is not None:
         write_survival(args.RESULT_NAME, genes, lgroup, surv_res, biomarkers)
         print('    %s_survival.txt' % args.RESULT_NAME)

@@ -824,6 +824,34 @@ int g2v_dcx_tally(const double *D, int64_t n_b, int64_t E, const double *D_obs, 
                   void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Network-propagated gene scores with a label-permutation test, NetRank (DESIGN.md §4.35; g2vec_b200/netrank.py does
+ * the host side).  A labelling is the observed one or a row of g2v_perm_labels, with its exact sums A [n_b][G] from
+ * g2v_perm_sums over the genes in their input order; n, k, Q, W as for g2v_perm_tally.  Columns: S and x are gene-major
+ * [G][ld] float64, column b = labelling b of the launch, 1 <= n_b <= ld <= G2V_NR_MAX_ROWS.  1 <= G <=
+ * G2V_NR_MAX_GENES.  The network is CSR over the genes: rowptr [G + 1] and col [rowptr[G]] int32, each row's
+ * neighbours ascending; w [G] float64 = 1 / deg (any value for a gene without neighbours).
+ * g2v_nr_seed: S[g][b] = sqrt(rho), rho = (double) N * (double) N / W[g] with N = n A[b][g] - k Q[g] (0 when W = 0).
+ * g2v_nr_step: one power iteration on the columns c0 .. c0 + n_cols - 1: for every gene j (rows [G] int32 lists each
+ *   gene once, in the order the warps take them), acc = +0, then acc = acc + x_in[i][b] * w[i] over the neighbours i
+ *   of j in CSR order, and x_out[j][b] = (1 - d) * S[j][b] + d * acc, with 1 - d computed on the host, every operation
+ *   correctly rounded (no fma).  0 <= d <= G2V_NR_MAX_DAMPING; x_in may be S, x_out must be neither.
+ * g2v_nr_tile_cols: the columns of a tile whose S and two x buffers fit in half the L2 of the current device (a
+ *   multiple of 32, at least 32); 0 for G out of range.
+ * g2v_nr_tally: count [G] int64 += #{b < n_b : x[j][b] >= score_obs[j]} (integer adds, one warp per gene).
+ * Out-of-range sizes fail with nothing launched.  One launch each, never synchronises; no floating-point atomics. */
+#define G2V_NR_MAX_GENES (1 << 24)
+#define G2V_NR_MAX_ROWS (1 << 20)
+#define G2V_NR_MAX_DAMPING 0.95
+int g2v_nr_seed(const int64_t *A, int64_t n_b, int32_t G, int32_t n, int32_t k, const int64_t *Q, const double *W,
+                double *S, int64_t ld, void *stream);
+int g2v_nr_step(const int32_t *rowptr, const int32_t *col, const double *w, const int32_t *rows, const double *S,
+                const double *x_in, double *x_out, int32_t G, int64_t ld, int64_t c0, int64_t n_cols, double damping,
+                void *stream);
+int64_t g2v_nr_tile_cols(int32_t G);
+int g2v_nr_tally(const double *x, int32_t G, int64_t n_b, int64_t ld, const double *score_obs, int64_t *count,
+                 void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Permutation Cox score test of every gene against survival (DESIGN.md §4.31; g2vec_b200/survival.py does the host
  * side).  n samples (3 <= n <= G2V_SURV_MAX_SAMPLES) with survival records; the time order lists them by time
  * descending and slot [n] int32 is its inverse (slot[s] = the time position of sample s).  Permutations are numbered
