@@ -152,7 +152,7 @@ fits, the SD of the K per-repeat means, P_random, the log-rank Z and P and the h
 risk groups (``nan`` on random rows) and how many of its genes are biomarkers; and RESULT_NAME_risk.txt: per sample
 used, in the expression file's order, its time, event, the biomarkers' pre-validated risk and group (1 = high risk),
 ready for a Kaplan-Meier plot.  The biomarkers were chosen with every sample's label, so their C is optimistic;
-nested re-selection is done for the good / poor label only (``--nested-cv``), not for survival.
+nested re-selection is ``--nested-cv`` for the good / poor label and ``--nested-survival-cv`` for survival.
 
 ``--nested-cv F`` (default 0: off; 2 <= F <= 100, F at most the number of samples of either label) adds nested
 cross-validation of the selection itself, on one GPU (DESIGN.md §4.34): over ``--nested-cv-repeats K`` (default 1,
@@ -173,6 +173,28 @@ Size, AUC and accuracy of the nested biomarkers and of nested top_t, the AUC of 
 Jaccard overlap with the biomarkers and its list, then the ``nested CV:`` line; and RESULT_NAME_nested_selection.txt:
 per gene, in the order of _lgroups.txt, its L-group, whether it is a biomarker, how many outer fits selected it, that
 count's share of the K F fits, and how many selected it from the good and from the poor L-group.
+
+``--nested-survival-cv F`` (default 0: off; 2 <= F <= 100, F at most the number of events and at most half the samples
+with a record; needs ``--survival``) is the same nested cross-validation against survival, on one GPU (DESIGN.md
+§4.36): over ``--nested-survival-cv-repeats K`` (default 1, 1 <= K <= 100) repeats of F-fold splits of the samples
+``--survival`` uses, stratified by event status -- the splits ``--survival-cv`` uses for the same F, K and ``--seed`` --
+steps 3 to 6 run again, with every option of the run, on every expression sample outside the test fold (samples
+without a record and of other labels included, as the main run takes them), and the fit's list, the same number of
+genes of largest |t| (``nested top_t``) and of largest Cox score statistic (``nested top_z``) over those training
+samples are scored on the held-out fold by ``--survival-cv``'s ridge Cox regression and Harrell's C.  The test fold's
+expression, labels and records reach neither the selection nor the fit.  The run's own biomarkers, ``top_t`` and
+``top_z`` are scored on the same splits, and the optimism is C(biomarkers) - C(nested biomarkers); with
+``--survival-cv R`` at the same F and K, P_random = (1 + #{random C >= nested C}) / (R + 1).  Each sample's
+out-of-fold risk from the nested biomarkers, averaged over the repeats, splits the samples at the median into
+pre-validated risk groups, with a log-rank test and a hazard ratio: the Kaplan-Meier split to report.  It needs ``-n``
+<= 64 and refuses torchrun.  The inputs are checked after step 2, where the run stops with an ``ERROR`` if they are
+refused; after step 6 (and after ``--nested-cv``'s lines) every outer fit prints one line, an outer fit that cannot
+train stops the run with an ``ERROR`` naming it, and the run prints a ``nested survival CV:`` line.  Step 7 also writes
+RESULT_NAME_nested_survival_cv.txt: per outer fit its repeat, fold, N_train, N_test, N_test_events, N_windows,
+Stop_epoch, Size, the C of the nested biomarkers, nested top_t and nested top_z, the C of the biomarkers, top_t and
+top_z, the Jaccard overlap with the biomarkers and its list, then the ``nested survival CV:`` line;
+RESULT_NAME_nested_survival_risk.txt, laid out as _risk.txt, with the nested biomarkers' pre-validated risk; and
+RESULT_NAME_nested_survival_selection.txt, laid out as _nested_selection.txt.
 
 ``--netrank B`` (default 0: off; 1 <= B <= 2^20) adds network-propagated gene scores, NetRank (Winter et al. 2012;
 GeneRank, Morrison et al. 2005), with a label-permutation test, on the GPU (DESIGN.md §4.35).  The network is the
@@ -325,6 +347,14 @@ def parse_arguments(argv=None):
                         "fold, in RESULT_NAME_nested_cv.txt and RESULT_NAME_nested_selection.txt; 0 (default) = off")
     p.add_argument('--nested-cv-repeats', type=int, default=1, metavar='K',
                    help="with --nested-cv: repeats of the fold split, 1 <= K <= 100 (default 1)")
+    p.add_argument('--nested-survival-cv', type=int, default=0, metavar='F',
+                   help="with --survival: nested cross-validation of the selection against survival: steps 3-6 rerun "
+                        "without every test fold of F-fold splits stratified by event (2 <= F <= 100) and the list's "
+                        "ridge Cox C on the held-out fold, in RESULT_NAME_nested_survival_cv.txt, "
+                        "RESULT_NAME_nested_survival_risk.txt and RESULT_NAME_nested_survival_selection.txt; 0 "
+                        "(default) = off")
+    p.add_argument('--nested-survival-cv-repeats', type=int, default=1, metavar='K',
+                   help="with --nested-survival-cv: repeats of the fold split, 1 <= K <= 100 (default 1)")
     p.add_argument('--netrank', type=int, default=0, metavar='B',
                    help="network-propagated gene scores (NetRank: personalised PageRank of each gene's |r| with the "
                         "label over the network) with a label-permutation test of B permutations (1 <= B <= 2^20): P "
@@ -373,6 +403,14 @@ def parse_arguments(argv=None):
         p.error("--nested-cv-repeats must be an integer in [1, 100]")
     if args.nested_cv and args.numBiomarker > 64:
         p.error("--nested-cv needs -n <= 64: a signature has at most 128 genes")
+    if not (args.nested_survival_cv == 0 or 2 <= args.nested_survival_cv <= 100):
+        p.error("--nested-survival-cv must be 0 (off) or an integer in [2, 100]")
+    if not 1 <= args.nested_survival_cv_repeats <= 100:
+        p.error("--nested-survival-cv-repeats must be an integer in [1, 100]")
+    if args.nested_survival_cv and args.survival is None:
+        p.error("--nested-survival-cv needs --survival FILE")
+    if args.nested_survival_cv and args.numBiomarker > 64:
+        p.error("--nested-survival-cv needs -n <= 64: a signature has at most 128 genes")
     if not 0 <= args.netrank <= 1 << 20:
         p.error("--netrank must be an integer in [0, 2^20]")
     if not (np.isfinite(args.netrank_damping) and 0.0 <= args.netrank_damping <= 0.95):
@@ -625,10 +663,11 @@ def write_survival_cv(prefix, genes, res, biomarkers):
                        + (sum(genes[g] in bm for g in res.genes[i]),)))
 
 
-def write_risk(prefix, samples, time, event, res):
-    """One row per sample of the survival CV, in expression order: time, event, the biomarkers' pre-validated risk and
-    risk group (1 = high)."""
-    with open(prefix + "_risk.txt", 'w') as f:
+def write_risk(prefix, samples, time, event, res, suffix="_risk.txt"):
+    """One row per sample of the survival CV, in expression order: time, event, the pre-validated risk and risk group
+    (1 = high) of res's first row (the biomarkers of a survival_cv.SurvivalCVResult, the nested biomarkers of a
+    nested_survival.NestedSurvivalResult)."""
+    with open(prefix + suffix, 'w') as f:
         f.write('SAMPLE\tTIME\tEVENT\tRISK\tGROUP\n')
         f.writelines('%s\t%.10g\t%d\t%.6f\t%d\n' % (s, t, e, r, g)
                      for s, t, e, r, g in zip(samples, time, event, res.risk[0], res.group[0]))
@@ -653,15 +692,36 @@ def write_nested_cv(prefix, genes, res):
         f.write(summary(res) + '\n')
 
 
-def write_nested_selection(prefix, genes, lgroup, res, biomarkers):
+def write_nested_selection(prefix, genes, lgroup, res, biomarkers, suffix="_nested_selection.txt"):
     """One row per gene in the order of _lgroups.txt: L-group, biomarker 0/1, how many outer fits selected it, that
-    count over the fits, and how many selected it from the good and from the poor L-group."""
+    count over the fits, and how many selected it from the good and from the poor L-group (a nested.NestedResult or a
+    nested_survival.NestedSurvivalResult)."""
     bm = set(biomarkers)
-    with open(prefix + "_nested_selection.txt", 'w') as f:
+    with open(prefix + suffix, 'w') as f:
         f.write('GeneSymbol\tLgroup(0:good,1:poor,2:other)\tBiomarker\tSelected\tFrequency\tSelectedGood\tSelectedPoor\n')
         f.writelines('%s\t%d\t%d\t%d\t%.6f\t%d\t%d\n' % (g, k, g in bm, n, q, a, b)
                      for g, k, n, q, a, b in zip(genes, lgroup, res.selected, res.frequency, res.selected_good,
                                                  res.selected_poor))
+
+
+def write_nested_survival_cv(prefix, genes, res):
+    """One row per outer fit of a nested_survival.NestedSurvivalResult (repeat-major, 1-based): its sample counts, test
+    events, windows, stop epoch, list size, the C of its list and of top_t and top_z at that size, the full run's
+    biomarkers', top_t's and top_z's C on the same fold, the Jaccard overlap with the full run's list and the list
+    itself; then the nested survival CV line."""
+    from .nested_survival import summary
+    K, F = res.n_train.shape
+    with open(prefix + "_nested_survival_cv.txt", 'w') as f:
+        f.write('Repeat\tFold\tN_train\tN_test\tN_test_events\tN_windows\tStop_epoch\tSize\tC_nested\t'
+                'C_nested_top_t\tC_nested_top_z\tC_biomarkers\tC_top_t\tC_top_z\tJaccard\tBiomarkers\n')
+        for k in range(K):
+            for j in range(F):
+                bm = res.biomarkers[k][j]
+                f.write('%d\t%d\t%d\t%d\t%d\t%d\t%d\t%d\t%.6f\t%.6f\t%.6f\t%.6f\t%.6f\t%.6f\t%.6f\t%s\n'
+                        % ((k + 1, j + 1, res.n_train[k, j], res.n_test[k, j], res.n_test_events[k, j],
+                            res.n_windows[k, j], res.stop_epoch[k, j], len(bm)) + tuple(res.c[:, k, j])
+                           + (res.jaccard[k, j], ','.join(genes[g] for g in bm))))
+        f.write(summary(res) + '\n')
 
 
 def write_netrank(prefix, genes, lgroup, res, biomarkers, line):
@@ -704,10 +764,11 @@ def _distributed():
 
 def main(argv=None):
     args = parse_arguments(argv)
-    if args.nested_cv:
+    nested_flag = '--nested-cv' if args.nested_cv else '--nested-survival-cv' if args.nested_survival_cv else None
+    if nested_flag:
         import os
         if int(os.environ.get("WORLD_SIZE", "1")) > 1:            # before any process group or device
-            sys.stdout.write('ERROR: --nested-cv: the nested loop runs on one GPU; run without torchrun\n')
+            sys.stdout.write('ERROR: %s: the nested loop runs on one GPU; run without torchrun\n' % nested_flag)
             sys.exit(1)
     rank, world, dist = _distributed()
     import builtins
@@ -802,6 +863,14 @@ def main(argv=None):
                                 min(2 * args.numBiomarker, n_genes))
         except ValueError as e:
             print('ERROR: --nested-cv: %s' % e)
+            sys.exit(1)
+    if args.nested_survival_cv:
+        from . import nested_survival
+        try:                                           # fail now rather than after training
+            nested_survival.check_inputs(data['expr'], surv_time, surv_event, data['label'], args.nested_survival_cv,
+                                         args.nested_survival_cv_repeats, min(2 * args.numBiomarker, n_genes))
+        except ValueError as e:
+            print('ERROR: --nested-survival-cv: %s' % e)
             sys.exit(1)
     if args.kmeans_restarts and n_genes < 3:
         print('ERROR: --kmeans-restarts needs at least 3 common genes, found %d' % n_genes)
@@ -936,6 +1005,19 @@ def main(argv=None):
             sys.exit(1)
         print('    ' + nested.summary(ncv_res))
 
+    if args.nested_survival_cv:
+        same_splits = (args.survival_cv and args.survival_cv_folds == args.nested_survival_cv
+                       and args.survival_cv_repeats == args.nested_survival_cv_repeats)
+        try:
+            nscv_res = nested_survival.nested_survival_cv(data['expr'], data['label'], surv_time, surv_event, src, dst,
+                                                          genes, args, biomarkers,
+                                                          random_c=scv_res.c_mean[3:] if same_splits else None,
+                                                          log=lambda line: print('    ' + line))
+        except ValueError as e:
+            print('ERROR: --nested-survival-cv: %s' % e)
+            sys.exit(1)
+        print('    ' + nested_survival.summary(nscv_res))
+
     print(">>> 7. Save results")
     write_biomarkers(args.RESULT_NAME, biomarkers)
     print('    %s_biomarkers.txt' % args.RESULT_NAME)
@@ -981,6 +1063,15 @@ def main(argv=None):
         print('    %s_nested_cv.txt' % args.RESULT_NAME)
         write_nested_selection(args.RESULT_NAME, genes, lgroup, ncv_res, biomarkers)
         print('    %s_nested_selection.txt' % args.RESULT_NAME)
+    if args.nested_survival_cv:
+        write_nested_survival_cv(args.RESULT_NAME, genes, nscv_res)
+        print('    %s_nested_survival_cv.txt' % args.RESULT_NAME)
+        write_risk(args.RESULT_NAME, [s for s, u in zip(data['sample'], surv_used) if u], surv_time[surv_used],
+                   surv_event[surv_used], nscv_res, suffix="_nested_survival_risk.txt")
+        print('    %s_nested_survival_risk.txt' % args.RESULT_NAME)
+        write_nested_selection(args.RESULT_NAME, genes, lgroup, nscv_res, biomarkers,
+                               suffix="_nested_survival_selection.txt")
+        print('    %s_nested_survival_selection.txt' % args.RESULT_NAME)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

@@ -138,6 +138,34 @@ def score_fit(x, lab, fold, k, f, head, seed=0):
     return auc[:, 0, 0], acc[:, 0, 0], conv[:, 0, 0]
 
 
+def run_list(genes, biomarkers):
+    """The full run's list (gene names) as sorted int32 indices into genes; ValueError unless it holds 1 to 128."""
+    pos = {g: i for i, g in enumerate(genes)}
+    bm = np.array(sorted(pos[g] for g in biomarkers), dtype=np.int32)
+    if not 1 <= bm.shape[0] <= MAX_SIZE:
+        raise ValueError("the run selected %d biomarkers, must be 1 to %d" % (bm.shape[0], MAX_SIZE))
+    return bm
+
+
+def select_fit(expr, label, rows, src, dst, genes, args, k, f, on_fit=None):
+    """Steps 3-6 of outer fit (k, f) on the expression rows `rows` alone (pipeline.select with every option of args):
+    (its pipeline.Selection, its list as sorted int32 indices into genes).  on_fit(k, f, selection) is called before
+    the list is checked.  ValueError naming the fit when it cannot train or selects no biomarkers."""
+    from . import pipeline
+    try:
+        sel = pipeline.select(expr[rows], label[rows], src, dst, genes, args)
+    except ValueError as e:
+        raise ValueError("outer fit repeat %d fold %d (%d training samples): %s"
+                         % (k + 1, f + 1, rows.shape[0], e)) from e
+    if on_fit is not None:
+        on_fit(k, f, sel)
+    pos = {g: i for i, g in enumerate(genes)}
+    mine = np.array(sorted(pos[g] for g in sel.biomarkers), dtype=np.int32)
+    if mine.shape[0] == 0:
+        raise ValueError("outer fit repeat %d fold %d selected no biomarkers" % (k + 1, f + 1))
+    return sel, mine
+
+
 def nested_cv(expr, label, src, dst, genes, args, biomarkers, random_auc=None, fold=None, log=None, on_fit=None):
     """Nested cross-validation of the selection, on one GPU.
 
@@ -148,16 +176,12 @@ def nested_cv(expr, label, src, dst, genes, args, biomarkers, random_auc=None, f
     outer splits int8 [K, n] over the used samples (default: g2v_sig_folds at the seed).  log(line): the progress line
     of every outer fit.  on_fit(k, f, selection): called with each outer fit's pipeline.Selection.  Returns a
     NestedResult; ValueError naming (k, f) when an outer fit cannot train."""
-    from . import pipeline
     F, K = int(args.nested_cv), int(args.nested_cv_repeats)
     x, lab, used = check_inputs(expr, label, F, K)
     genes = np.asarray(genes)
     G = len(genes)
-    pos = {g: i for i, g in enumerate(genes)}
-    bm = np.array(sorted(pos[g] for g in biomarkers), dtype=np.int32)
+    bm = run_list(genes, biomarkers)
     p = len(bm)
-    if not 1 <= p <= MAX_SIZE:
-        raise ValueError("the run selected %d biomarkers, must be 1 to %d" % (p, MAX_SIZE))
     head = np.stack([bm, signature.top_t(x, lab, p)])
     cap = None
     if fold is not None:
@@ -178,17 +202,7 @@ def nested_cv(expr, label, src, dst, genes, args, biomarkers, random_auc=None, f
     for k in range(K):
         for f in range(F):
             train = fold[k] != f
-            rows = idx[train]
-            try:
-                sel = pipeline.select(expr[rows], lab_all[rows], src, dst, genes, args)
-            except ValueError as e:
-                raise ValueError("outer fit repeat %d fold %d (%d training samples): %s"
-                                 % (k + 1, f + 1, rows.shape[0], e)) from e
-            if on_fit is not None:
-                on_fit(k, f, sel)
-            mine = np.array(sorted(pos[g] for g in sel.biomarkers), dtype=np.int32)
-            if mine.shape[0] == 0:
-                raise ValueError("outer fit repeat %d fold %d selected no biomarkers" % (k + 1, f + 1))
+            sel, mine = select_fit(expr, lab_all, idx[train], src, dst, genes, args, k, f, on_fit)
             pair = np.stack([mine, signature.top_t(x[train], lab[train], mine.shape[0])])
             a, c, cv = score_fit(x, lab, fold, k, f, pair, seed=args.seed)
             auc[:2, k, f], acc[:2, k, f] = a, c

@@ -7,13 +7,14 @@ get pre-validated risk groups (Tibshirani & Efron 2002): each sample's out-of-fo
 split at the median, with a log-rank test and the hazard ratio of the high-risk group.
 
 The biomarkers, top_t and top_z were chosen with every sample, so their C are optimistic and comparable with each
-other.  Nested re-selection (steps 3-6 rerun on every training fold) exists for the good / poor label only
-(nested.nested_cv, ``--nested-cv``); a nested survival C is not done.
+other.  Nested re-selection (steps 3-6 rerun on every training fold) is nested.nested_cv (``--nested-cv``) for the
+good / poor label and nested_survival.nested_survival_cv (``--nested-survival-cv``) for survival; the latter scores
+on these same splits with cox_fits.
 
 Host side (NumPy): the checks, top_t (signature.top_t), X as float64 gene-major over the time positions, chunking over
 whole signatures and the summaries.  Device side: g2v_sig_folds once (y = the event flags), g2v_surv_scores once for
 the top_z ranking (survival.rank_genes), then per chunk g2v_sig_draw, g2v_cox_fit (one CTA per fit, Newton on the
-device) and g2v_cox_concordance (csrc/g2v_sig.cu, csrc/g2v_surv.cu, csrc/g2v_cox.cu).
+device) and g2v_cox_concordance (csrc/g2v_sig.cu, csrc/g2v_surv.cu, csrc/g2v_cox.cu), in cox_fits.
 """
 import math
 from collections import namedtuple
@@ -226,20 +227,48 @@ def survival_cv(expr, time, event, label, signature_genes, n_random, folds=5, re
     G = x.shape[1]
     if sig.dtype.kind not in "iu" or (sig.size and (sig.min() < 0 or sig.max() >= G)) or np.unique(sig).size != sig.size:
         raise ValueError("the signature must be distinct gene indices in [0, %d)" % G)
-    n, p, R, K, F = x.shape[0], int(sig.shape[0]), int(n_random), int(repeats), int(folds)
-    S = R + 3
+    p, R, K, F = int(sig.shape[0]), int(n_random), int(repeats), int(folds)
     tt = signature.top_t(expr, label, p)
+    tz = np.sort(survival.rank_genes(x, t, e)[:p]).astype(np.int32)          # RuntimeError without a GPU
+    head = np.stack([np.sort(sig).astype(np.int32), tt, tz])
+    genes, folds_s, counts, n_iter, conv, beta, scores = cox_fits(x, t, e, head, R, K, F, seed,
+                                                                  max_chunk_bytes=max_chunk_bytes)
+    c = concordance(counts)
+    c_mean, c_sd, p_random = summarise(c, 3, R)
+    rg = [risk_groups(scores[s], t, e) for s in range(3)]
+    col = lambda j: np.array([r[j] for r in rg], dtype=np.float64)
+    return SurvivalCVResult(names=list(NAMES) + ["random_%d" % r for r in range(1, R + 1)], genes=genes,
+                            folds=folds_s, counts=counts, c=c, n_iter=n_iter, converged=int(conv.sum()),
+                            beta=beta, scores=scores, c_mean=c_mean, c_sd=c_sd, p_random=p_random,
+                            risk=np.stack([r[0] for r in rg]), group=np.stack([r[1] for r in rg]),
+                            logrank_z=col(2), logrank_p=col(3), hr=col(4), hr_low=col(5), hr_high=col(6))
+
+
+def cox_fits(x, time, event, head, n_random, repeats, folds, seed, fold=None, cap=None, max_chunk_bytes=None):
+    """The device part of survival_cv, also run by nested_survival.nested_survival_cv: the ridge Cox fits and test-fold
+    concordance counts of S = H + R signatures, the H rows of head [H, p] (sorted distinct gene indices) then
+    random_1 .. random_R (g2v_sig_draw, the random signatures of survival_cv at the same seed).
+
+    x float64 [n, G], time [n] and event [n]: the samples with a record, as check_inputs returns them (not checked
+    here).  fold: None to split with g2v_sig_folds (K repeats of F-fold stratified by event status at seed), or an
+    int8 [K, n] array of test folds 0..F-1 over the samples to fit on instead.  cap: the largest test fold
+    g2v_cox_concordance stages in shared memory (a larger fold is read from global memory, with the same counts);
+    default the largest stratified fold.  Returns (genes int32 [S, p], fold int8 [K, n], counts int64 [S, K, F, 3],
+    n_iter int32 [S, K, F], converged uint8 [S, K, F], beta float64 [H, K, F, p], scores float64 [H, K, n]: the
+    out-of-fold eta of every sample for the head rows), every per-sample array in the samples' order."""
+    n, G = x.shape
+    H, p = head.shape
+    R, K, F = int(n_random), int(repeats), int(folds)
+    S = H + R
     import torch
     from . import _capi
     lib = _capi.load()
     if not torch.cuda.is_available():
         raise RuntimeError("g2vec_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
-    tz = np.sort(survival.rank_genes(x, t, e)[:p]).astype(np.int32)
-    head = np.stack([np.sort(sig).astype(np.int32), tt, tz])
     dev = torch.device("cuda", torch.cuda.current_device())
     st = torch.cuda.current_stream(dev).cuda_stream
     up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-    order, _, flags, _, _ = survival.time_groups(t, e)
+    order, _, flags, _, _ = survival.time_groups(time, event)
     end = (flags & 2).astype(bool)
     grp = np.cumsum(np.r_[0, end[:-1]]).astype(np.int32)
     n_pad = -(-n // 32) * 32
@@ -250,20 +279,24 @@ def survival_cv(expr, time, event, label, signature_genes, n_random, folds=5, re
     flags_d, grp_d = up(flags), up(grp)
     ev_d = up((flags & 1).astype(np.uint8))
     seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-    fold_d = torch.empty((K, n), dtype=torch.int8, device=dev)
-    _capi.check(lib.g2v_sig_folds(ev_d.data_ptr(), n, K, F, seed, fold_d.data_ptr(), st), "g2v_sig_folds")
-    n_ev = int(e.sum())
-    cap = -(-n_ev // F) + -(-(n - n_ev) // F)          # the largest test fold
+    if fold is None:
+        fold_d = torch.empty((K, n), dtype=torch.int8, device=dev)
+        _capi.check(lib.g2v_sig_folds(ev_d.data_ptr(), n, K, F, seed, fold_d.data_ptr(), st), "g2v_sig_folds")
+    else:
+        fold_d = up(np.asarray(fold, dtype=np.int8)[:, order])       # samples -> time positions
+    if cap is None:
+        n_ev = int(np.asarray(event).sum())
+        cap = -(-n_ev // F) + -(-(n - n_ev) // F)      # the largest test fold
     cap = cap if cap <= MAX_STAGED else 0
     if max_chunk_bytes is None:
         max_chunk_bytes = torch.cuda.mem_get_info(dev)[0] // 2
     rows = chunk_signatures(S, n, p, K, F, max_chunk_bytes)
     genes = np.empty((S, p), dtype=np.int32)
-    genes[:3] = head
+    genes[:H] = head
     counts = np.empty((S, K, F, 3), dtype=np.int64)
     n_iter = np.empty((S, K, F), dtype=np.int32); conv = np.empty((S, K, F), dtype=np.uint8)
-    beta = torch.empty((3, K, F, p), dtype=torch.float64, device=dev)
-    named = np.empty((3, K, n))
+    beta = torch.empty((H, K, F, p), dtype=torch.float64, device=dev)
+    named = np.empty((H, K, n))
     g_d = torch.empty((rows, p), dtype=torch.int32, device=dev)
     sc_d = torch.empty((rows, K, n), dtype=torch.float64, device=dev)
     ell_d = torch.empty((rows * K * F, n), dtype=torch.float64, device=dev)
@@ -272,11 +305,11 @@ def survival_cv(expr, time, event, label, signature_genes, n_random, folds=5, re
     cv_d = torch.empty((rows, K, F), dtype=torch.uint8, device=dev)
     for s0 in range(0, S, rows):
         ns = min(rows, S - s0)
-        fixed = min(ns, max(0, 3 - s0))                # rows of this chunk that are named signatures
+        fixed = min(ns, max(0, H - s0))                # rows of this chunk that come from head
         if fixed:
             g_d[:fixed] = up(head[s0:s0 + fixed])
         if ns > fixed:
-            _capi.check(lib.g2v_sig_draw(G, p, seed, s0 + fixed - 2, ns - fixed, g_d[fixed].data_ptr(), st),
+            _capi.check(lib.g2v_sig_draw(G, p, seed, s0 + fixed - H + 1, ns - fixed, g_d[fixed].data_ptr(), st),
                         "g2v_sig_draw")
         _capi.check(lib.g2v_cox_fit(X_d.data_ptr(), G, n, n_pad, flags_d.data_ptr(), fold_d.data_ptr(), K, F,
                                     g_d.data_ptr(), ns, p, ell_d.data_ptr(), sc_d.data_ptr(), it_d.data_ptr(),
@@ -289,16 +322,8 @@ def survival_cv(expr, time, event, label, signature_genes, n_random, folds=5, re
         n_iter[sl] = it_d[:ns].cpu().numpy(); conv[sl] = cv_d[:ns].cpu().numpy()
         if fixed:
             named[s0:s0 + fixed] = sc_d[:fixed].cpu().numpy()
-    c = concordance(counts)
-    c_mean, c_sd, p_random = summarise(c, 3, R)
     scores = np.empty_like(named)
     scores[:, :, order] = named                        # time positions -> samples
     folds_s = np.empty((K, n), dtype=np.int8)
     folds_s[:, order] = fold_d.cpu().numpy()
-    rg = [risk_groups(scores[s], t, e) for s in range(3)]
-    col = lambda j: np.array([r[j] for r in rg], dtype=np.float64)
-    return SurvivalCVResult(names=list(NAMES) + ["random_%d" % r for r in range(1, R + 1)], genes=genes,
-                            folds=folds_s, counts=counts, c=c, n_iter=n_iter, converged=int(conv.sum()),
-                            beta=beta.cpu().numpy(), scores=scores, c_mean=c_mean, c_sd=c_sd, p_random=p_random,
-                            risk=np.stack([r[0] for r in rg]), group=np.stack([r[1] for r in rg]),
-                            logrank_z=col(2), logrank_p=col(3), hr=col(4), hr_low=col(5), hr_high=col(6))
+    return genes, folds_s, counts, n_iter, conv, beta.cpu().numpy(), scores
