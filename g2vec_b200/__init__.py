@@ -13,6 +13,7 @@ from .gsea import gsea, read_gmt  # noqa: F401
 from .signature import signature_cv  # noqa: F401
 from .diffcoex import diffcoex_test  # noqa: F401
 from .netrank import netrank_test  # noqa: F401
+from .lasso import lasso_cv  # noqa: F401
 from .survival import survival_test, read_survival  # noqa: F401
 from . import survival_cv  # noqa: F401  (the module: g2vec_b200.survival_cv.survival_cv runs the test)
 from . import graph, paths  # noqa: F401

@@ -170,6 +170,14 @@ SIGNATURES = {
     "g2v_nr_step": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i64, _i64, _i64, ctypes.c_double, _vp]),
     "g2v_nr_tile_cols": (_i64, [_i32]),
     "g2v_nr_tally": (ctypes.c_int, [_vp, _i32, _i64, _i64, _vp, _vp, _vp]),
+    "g2v_lasso_workspace_bytes": (ctypes.c_size_t, [_i32, _i64, _i32]),
+    "g2v_lasso_standardise": (ctypes.c_int, [_vp, _i32, _i32, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp,
+                                             _vp]),
+    "g2v_lasso_grad": (ctypes.c_int, [_vp, _i32, _i32, _i64, _i32, _vp, ctypes.c_double, ctypes.c_double, _vp]),
+    "g2v_lasso_lambda_max": (ctypes.c_int, [_i32, _i64, _i32, _vp, ctypes.c_double, _vp, _vp]),
+    "g2v_lasso_cd": (ctypes.c_int, [_vp, _i32, _i32, _i64, _vp, _i32, _vp, _i32, ctypes.c_double, ctypes.c_double,
+                                    ctypes.c_double, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "g2v_lasso_score": (ctypes.c_int, [_vp, _vp, _i32, _i64, _i32, _i32, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp]),
     "g2v_surv_rows": (ctypes.c_int, [_vp, _i32, _u64, _i64, _i64, _vp, _vp]),
     "g2v_surv_scores": (ctypes.c_int, [_vp, _i32, _i32, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "g2v_paths_canonicalise":(ctypes.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),

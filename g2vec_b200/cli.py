@@ -214,6 +214,26 @@ splits, beside the biomarkers'), and step 7 also writes RESULT_NAME_netrank.txt:
 rank (1 = highest score), P, Q and whether it is a biomarker, followed by the same line.  None of these depend on
 training.
 
+``--lasso F`` (default 0: off; 2 <= F <= 100, F at most the number of samples of either label) adds the lasso /
+elastic-net logistic baseline on the GPU (DESIGN.md §4.37): glmnet's path of the good / poor label on every gene (the
+samples with label 0 or 1, the matrix ``top_t`` uses), each gene standardised over the fit's training samples, with
+mixing ``--lasso-alpha α`` (default 1 = the lasso; finite, 0 < α <= 1), on the full cohort and on every training fold
+of ``--lasso-repeats K`` (default 1, 1 <= K <= 100) repeats of stratified F-fold splits (``--signature-cv``'s splits
+for the same F, K and ``--seed``).  The 100 lambdas are glmnet's; the path stops at a deviance ratio of 0.999, a rise
+below 1e-5 of it, or 512 genes entered.  Every solution is checked against the KKT conditions in float64.  The
+held-out binomial deviance gives cv.glmnet's lambda_min and lambda_1se; ``top_lasso`` is the genes in the order they
+enter the full-cohort path.  The inputs are checked after step 2, where the run stops with an ``ERROR`` if they are
+refused.  After step 6 (and after ``--nested-cv``'s lines) it prints a ``lasso:`` line: α, F x K, the path length,
+lambda_min and lambda_1se with their gene counts, CV deviance and CV AUC, the Jaccard overlap of ``top_lasso`` at the
+biomarkers' size with the biomarkers, how many biomarkers are nonzero at lambda_1se; with ``--signature-cv`` the AUC
+of ``top_lasso`` on its splits beside the biomarkers'; with ``--nested-cv`` at the same F and K the mean AUC of
+``nested_lasso`` (``top_lasso`` of each training fold at the size of that fold's nested list, scored as the nested
+lists are) beside ``nested_biomarkers``; and how many solutions did not certify.  Step 7 also writes
+RESULT_NAME_lasso.txt: per gene, in the order of _lgroups.txt, its L-group, entry index on the full-cohort path (-1 if
+never), beta at lambda_min and at lambda_1se, the fraction of fold fits in which it had entered by lambda_1se's index
+and whether it is a biomarker, followed by the line; and RESULT_NAME_lasso_path.txt: per lambda index its lambda, df,
+deviance ratio, CV deviance and SE, mean CV AUC and the marks of lambda_min and lambda_1se.
+
 Which runs are bit-reproducible (same input, same seed, one GPU: the same three output files):
 - ``--deterministic`` with ``--algo rows``: every optimizer, full batch or ``--batch``, with or without
   ``--reshuffle`` or ``--class-weight``, at every table size (DESIGN.md §4.13); ``--class-weight 1,1`` writes the
@@ -361,6 +381,14 @@ def parse_arguments(argv=None):
                         "and Benjamini-Hochberg Q in RESULT_NAME_netrank.txt; 0 (default) = off")
     p.add_argument('--netrank-damping', type=float, default=0.5, metavar='d',
                    help="with --netrank: the damping d, a finite number in [0, 0.95] (default 0.5; 0 = no propagation)")
+    p.add_argument('--lasso', type=int, default=0, metavar='F',
+                   help="lasso / elastic-net logistic baseline on every gene: glmnet's path on the cohort and on every "
+                        "training fold of F-fold splits (2 <= F <= 100), lambda_min and lambda_1se by CV deviance, in "
+                        "RESULT_NAME_lasso.txt and RESULT_NAME_lasso_path.txt; 0 (default) = off")
+    p.add_argument('--lasso-repeats', type=int, default=1, metavar='K',
+                   help="with --lasso: repeats of the fold split, 1 <= K <= 100 (default 1)")
+    p.add_argument('--lasso-alpha', type=float, default=1.0, metavar='ALPHA',
+                   help="with --lasso: the elastic-net mixing, a finite number in (0, 1] (default 1 = the lasso)")
     args = p.parse_args(argv)
     if not (np.isfinite(args.walk_q) and 1.0 / 256.0 <= args.walk_q <= 256.0):
         p.error("--walk-q must be a finite number in [1/256, 256]")
@@ -411,6 +439,12 @@ def parse_arguments(argv=None):
         p.error("--nested-survival-cv needs --survival FILE")
     if args.nested_survival_cv and args.numBiomarker > 64:
         p.error("--nested-survival-cv needs -n <= 64: a signature has at most 128 genes")
+    if not (args.lasso == 0 or 2 <= args.lasso <= 100):
+        p.error("--lasso must be 0 (off) or an integer in [2, 100]")
+    if not 1 <= args.lasso_repeats <= 100:
+        p.error("--lasso-repeats must be an integer in [1, 100]")
+    if not (np.isfinite(args.lasso_alpha) and 0.0 < args.lasso_alpha <= 1.0):
+        p.error("--lasso-alpha must be a finite number in (0, 1]")
     if not 0 <= args.netrank <= 1 << 20:
         p.error("--netrank must be an integer in [0, 2^20]")
     if not (np.isfinite(args.netrank_damping) and 0.0 <= args.netrank_damping <= 0.95):
@@ -738,6 +772,32 @@ def write_netrank(prefix, genes, lgroup, res, biomarkers, line):
         f.write(line + '\n')
 
 
+def write_lasso(prefix, genes, lgroup, res, biomarkers, line):
+    """One row per gene in the order of _lgroups.txt: L-group, entry index on fit 0's path (-1 never), beta at
+    lambda_min and lambda_1se, the fraction of fold fits in which the gene had entered by lambda_1se's index, biomarker
+    0/1 (a lasso.LassoResult); then the lasso line."""
+    bm = set(biomarkers)
+    ent = res.entry[1:].astype(np.int64)
+    frac = ((ent >= 0) & (ent <= res.i_1se)).mean(axis=0)
+    with open(prefix + "_lasso.txt", 'w') as f:
+        f.write('GeneSymbol\tLgroup(0:good,1:poor,2:other)\tEntry\tBeta_min\tBeta_1se\tFold_entered\tBiomarker\n')
+        f.writelines('%s\t%d\t%d\t%.6g\t%.6g\t%.6f\t%d\n' % (g, k, e, b0, b1, fr, g in bm)
+                     for g, k, e, b0, b1, fr in zip(genes, lgroup, res.entry[0], res.beta[res.i_min],
+                                                  res.beta[res.i_1se], frac))
+        f.write(line + '\n')
+
+
+def write_lasso_path(prefix, res):
+    """One row per lambda index of a lasso.LassoResult: lambda, df and deviance ratio of fit 0, CV deviance and its SE,
+    mean CV AUC, and the marks of lambda_min and lambda_1se."""
+    with open(prefix + "_lasso_path.txt", 'w') as f:
+        f.write('Index\tLambda\tDf\tDev_ratio\tCV_deviance\tCV_SE\tCV_AUC\tMark\n')
+        for k in range(res.n_lambda):
+            mark = ','.join(m for m, i in (("min", res.i_min), ("1se", res.i_1se)) if i == k)
+            f.write('%d\t%.6g\t%d\t%.6f\t%.6f\t%.6f\t%.6f\t%s\n' % (k, res.lambdas[k], res.df[k], res.dev_ratio[k],
+                                                                      res.cvm[k], res.cvsd[k], res.auc_mean[k], mark))
+
+
 def write_vectors(prefix, genes, mat):
     with open(prefix + "_vectors.txt", 'w') as f:
         f.write('GeneSymbol' + ''.join('\tV%d' % i for i in range(mat.shape[1])) + '\n')
@@ -871,6 +931,13 @@ def main(argv=None):
                                          args.nested_survival_cv_repeats, min(2 * args.numBiomarker, n_genes))
         except ValueError as e:
             print('ERROR: --nested-survival-cv: %s' % e)
+            sys.exit(1)
+    if args.lasso:
+        from . import lasso
+        try:
+            lasso.check_inputs(data['expr'], data['label'], args.lasso, args.lasso_repeats, args.lasso_alpha)
+        except ValueError as e:
+            print('ERROR: --lasso: %s' % e)
             sys.exit(1)
     if args.kmeans_restarts and n_genes < 3:
         print('ERROR: --kmeans-restarts needs at least 3 common genes, found %d' % n_genes)
@@ -1018,6 +1085,27 @@ def main(argv=None):
             sys.exit(1)
         print('    ' + nested_survival.summary(nscv_res))
 
+    if args.lasso:
+        ls_res = lasso.lasso_cv(data['expr'], data['label'], folds=args.lasso, repeats=args.lasso_repeats,
+                                alpha=args.lasso_alpha, seed=args.seed)
+        pos = {g: i for i, g in enumerate(genes)}
+        bm_idx = np.array(sorted(pos[g] for g in biomarkers), dtype=np.int64)
+        ls_x, ls_lab = lasso.check_inputs(data['expr'], data['label'], args.lasso, args.lasso_repeats,
+                                          args.lasso_alpha)
+        extra = ""
+        top = np.sort(lasso.top_lasso(ls_res.entry[0], ls_res.entry_abs[0], len(biomarkers)))
+        if args.signature_cv and top.size:             # top_lasso on --signature-cv's splits, beside the biomarkers
+            auc = signature.cv_fits(ls_x, ls_lab, top[None, :].astype(np.int32), 0, args.signature_repeats,
+                                    args.signature_folds, args.seed)[2]
+            extra += "; top_lasso AUC %.3f vs biomarkers %.3f on the signature splits" % (
+                float(auc[0].reshape(-1).mean()), float(sig_res.auc_mean[0]))
+        if args.nested_cv == args.lasso and args.nested_cv_repeats == args.lasso_repeats:
+            nl = lasso.nested_lasso(ls_x, ls_lab, ls_res, ncv_res.biomarkers, args.seed)
+            extra += "; nested_lasso AUC %.3f vs nested_biomarkers %.3f" % (float(np.nanmean(nl)),
+                                                                            float(ncv_res.auc_mean[0]))
+        ls_line = lasso.summary(ls_res, bm_idx, extra)
+        print('    ' + ls_line)
+
     print(">>> 7. Save results")
     write_biomarkers(args.RESULT_NAME, biomarkers)
     print('    %s_biomarkers.txt' % args.RESULT_NAME)
@@ -1072,6 +1160,11 @@ def main(argv=None):
         write_nested_selection(args.RESULT_NAME, genes, lgroup, nscv_res, biomarkers,
                                suffix="_nested_survival_selection.txt")
         print('    %s_nested_survival_selection.txt' % args.RESULT_NAME)
+    if args.lasso:
+        write_lasso(args.RESULT_NAME, genes, lgroup, ls_res, biomarkers, ls_line)
+        print('    %s_lasso.txt' % args.RESULT_NAME)
+        write_lasso_path(args.RESULT_NAME, ls_res)
+        print('    %s_lasso_path.txt' % args.RESULT_NAME)
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()

@@ -852,6 +852,52 @@ int g2v_nr_tally(const double *x, int32_t G, int64_t n_b, int64_t ld, const doub
                  void *stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Cross-validated lasso / elastic-net logistic regression over every gene, the glmnet path (DESIGN.md §4.37;
+ * g2vec_b200/lasso.py does the host side).  n samples (3 <= n <= G2V_SIG_MAX_SAMPLES) with y [n] in {0, 1}, X [G][n_pad]
+ * float64 gene-major (n_pad >= n, a multiple of 4), fold [K][n] from g2v_sig_folds.  Global fit 0 uses every sample,
+ * fit 1 + k F + f the samples outside fold f of repeat k; a launch covers fits fit0 .. fit0 + fits - 1 (a chunk) whose
+ * state lives in ws (g2v_lasso_workspace_bytes(G, n_pad, fits) bytes, 0 for sizes out of range).  Per fit and lambda
+ * the objective is  -(1/n_fit) sum [y eta - log(1 + e^eta)] + lambda [alpha |beta|_1 + (1 - alpha)/2 |beta|^2],
+ * eta = b0 + z^T beta, z each gene standardised over the fit's training samples (population SD; a constant gene gets
+ * z = 0 and never enters), b0 unpenalised, 0 < alpha <= 1.
+ * g2v_lasso_standardise: the standardisation, the null model and a cleared state; entry [fits][G] int16 = -1 and
+ *   entry_abs [fits][G] = 0 (both offset to the chunk's first fit).
+ * g2v_lasso_grad: the gradient of the smooth part of every fit of the chunk at its current solution (one DGEMM on the
+ *   FP64 tensor cores).  g2v_lasso_lambda_max: lam_max [1] (device) = max_j |g_j| / max(alpha, 1e-3) of the chunk's
+ *   first fit (call it after standardise and one grad).
+ * g2v_lasso_cd: round r of lambda index k (lam_prev = lambda_{k-1}, lambda_0 at k = 0).  Per fit not yet done: the
+ *   largest KKT violation of the current solution (|g_0|, |g_j| - lambda alpha at beta_j = 0, |g_j + lambda alpha
+ *   sign beta_j| otherwise); at most G2V_LASSO_EPS, or after 100 Newton steps at this lambda, the fit records lambda k:
+ *   df, dev_ratio, n_iter, kkt [fits][G2V_LASSO_N_LAMBDA] at [f][k], entry / entry_abs of genes entering, path [k][G + 1]
+ *   (intercept then beta of the chunk's first fit, may be NULL) and its stop rules; else it extends its working set (the sequential strong
+ *   rule at r = 0, KKT violators after) and runs proximal Newton with coordinate descent.  ctl [2] int32: ctl[0] = the
+ *   fits still pending after the call, ctl[1] = the chunk's first fit's path length once it stopped (-1 before).  A fit
+ *   whose ever-active genes would exceed G2V_LASSO_MAX_ACTIVE keeps its previous solution and stops with path length
+ *   k; one whose deviance ratio exceeds 0.999, or at k >= 4 rose by less than 1e-5 of itself, stops with k + 1.  A
+ *   stopped fit reports its last solution at later lambdas.
+ * g2v_lasso_score: for each fold fit of the chunk and each sample i of its test fold, scores [L][K][n] at [k][rep][i] =
+ *   eta_i and dev the binomial deviance -2 log p(y_i) with p clamped to [1e-5, 1 - 1e-5].
+ * Out-of-range sizes fail with nothing launched.  Never synchronises; no floating-point atomics. */
+#define G2V_LASSO_N_LAMBDA 100
+#define G2V_LASSO_MAX_ACTIVE 512
+#define G2V_LASSO_MAX_GENES (1 << 20)
+#define G2V_LASSO_EPS 1e-7
+size_t g2v_lasso_workspace_bytes(int32_t G, int64_t n_pad, int32_t fits);
+int g2v_lasso_standardise(const double *X, int32_t G, int32_t n, int64_t n_pad, const uint8_t *y, const int8_t *fold,
+                          int32_t K, int32_t F, int32_t fit0, int32_t fits, void *ws, int16_t *entry,
+                          double *entry_abs, void *stream);
+int g2v_lasso_grad(const double *X, int32_t G, int32_t n, int64_t n_pad, int32_t fits, void *ws, double lam,
+                   double alpha, void *stream);
+int g2v_lasso_lambda_max(int32_t G, int64_t n_pad, int32_t fits, void *ws, double alpha, double *lam_max,
+                         void *stream);
+int g2v_lasso_cd(const double *X, int32_t G, int32_t n, int64_t n_pad, const uint8_t *y, int32_t fits, void *ws,
+                 int32_t k, double lam, double lam_prev, double alpha, int32_t round, int32_t *df, double *dev_ratio,
+                 int32_t *n_iter, double *kkt, int16_t *entry, double *entry_abs, double *path, int32_t *ctl,
+                 void *stream);
+int g2v_lasso_score(const uint8_t *y, const int8_t *fold, int32_t n, int64_t n_pad, int32_t K, int32_t F, int32_t fit0,
+                    int32_t fits, void *ws, int32_t G, int32_t k, double *scores, double *dev, void *stream);
+
+/* ---------------------------------------------------------------------------------------
  * Permutation Cox score test of every gene against survival (DESIGN.md §4.31; g2vec_b200/survival.py does the host
  * side).  n samples (3 <= n <= G2V_SURV_MAX_SAMPLES) with survival records; the time order lists them by time
  * descending and slot [n] int32 is its inverse (slot[s] = the time position of sample s).  Permutations are numbered
