@@ -139,3 +139,36 @@ def predict(fit, x_test, k):
     k = min(k, len(fit["b0"]) - 1)
     zt = np.where(fit["const"], 0.0, (x_test - fit["mu"]) / fit["sd"])
     return fit["b0"][k] + zt @ fit["beta"][k]
+
+
+P_MIN = 1e-5                                           # glmnet's clamp of a held-out probability
+
+
+def heldout_deviance(eta, y):
+    """Each sample's binomial deviance -2 log p (y = 1) or -2 log(1 - p) (y = 0), p = sigmoid(eta) clamped to
+    [1e-5, 1 - 1e-5]."""
+    eta, y = np.asarray(eta, dtype=np.float64), np.asarray(y)
+    p = np.clip(1.0 / (1.0 + np.exp(-eta)), P_MIN, 1.0 - P_MIN)
+    return np.where(y == 1, -2.0 * np.log(p), -2.0 * np.log(1.0 - p))
+
+
+def cv_glmnet(dev, folds, F):
+    """cv.glmnet's grouped rule over the K F folds as one set (DESIGN.md §4.37), from the held-out deviances dev
+    [L, K, n] and the folds [K, n]: (cvm, cvsd, i_min, i_1se).  cvm is the fold-size-weighted mean of the fold means,
+    which is the plain mean over every held-out (repeat, sample); cvsd = sqrt(sum_f N_f (m_f - cvm)^2 / N / (K F - 1));
+    i_min the first argmin of cvm; i_1se the first (largest-lambda) index with cvm <= cvm[i_min] + cvsd[i_min]."""
+    dev = np.asarray(dev, dtype=np.float64)
+    L, K, n = dev.shape
+    group = (np.arange(K)[:, None] * F + np.asarray(folds, dtype=np.int64)).ravel()     # fold id of (k, i)
+    N = np.bincount(group, minlength=K * F).astype(np.float64)
+    cvm = np.empty(L)
+    cvsd = np.empty(L)
+    for li in range(L):
+        d = dev[li].ravel()
+        cvm[li] = d.mean()
+        m = np.bincount(group, weights=d, minlength=K * F) / N
+        cvsd[li] = np.sqrt((N * (m - cvm[li]) ** 2).sum() / N.sum() / (K * F - 1))
+    best = cvm.min()
+    i_min = next(li for li in range(L) if cvm[li] == best)
+    i_1se = next(li for li in range(L) if cvm[li] <= cvm[i_min] + cvsd[i_min])
+    return cvm, cvsd, i_min, i_1se

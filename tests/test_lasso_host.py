@@ -104,6 +104,54 @@ def test_lambda_min_and_1se_rule():
     assert cvm2.tolist() == [1.0, 0.5, 1.0] and i_min == 1 and not cvsd2.any()
 
 
+def unequal_folds(rs, K, F, n):
+    """[K, n] folds with every fold non-empty and sizes that differ."""
+    folds = np.empty((K, n), dtype=np.int8)
+    for k in range(K):
+        f = np.concatenate([np.arange(F), rs.randint(0, F, n - F)])
+        rs.shuffle(f)
+        folds[k] = f
+    return folds
+
+
+@pytest.mark.parametrize("L,K,F,n", [(7, 1, 2, 5), (30, 1, 5, 23), (20, 3, 4, 17), (12, 10, 10, 101)])
+def test_cv_summary_matches_independent_cv_glmnet(L, K, F, n):
+    rs = np.random.RandomState(L * 1000 + K * 100 + n)
+    folds = unequal_folds(rs, K, F, n)
+    sizes = [np.bincount(folds[k], minlength=F) for k in range(K)]
+    assert all(s.min() >= 1 for s in sizes) and (K * F == 2 or len(np.unique(np.concatenate(sizes))) > 1)
+    dev = rs.gamma(2.0, 0.6, (L, K, n))
+    # ties in cvm: equal rows have equal cvm bit for bit, so both rules must take the first of them
+    dev[3] = dev[5] = dev[:].min(axis=0)
+    dev[4] = dev[3]
+    got = lasso.cv_summary(dev, folds, F)
+    want = orc.cv_glmnet(dev, folds, F)
+    np.testing.assert_allclose(got[0], want[0], rtol=1e-13)
+    np.testing.assert_allclose(got[1], want[1], rtol=1e-12)
+    assert got[2:] == want[2:] == (3, want[3])
+    assert want[3] <= 3 and want[0][want[3]] <= want[0][3] + want[1][3]
+    assert want[3] == 0 or want[0][want[3] - 1] > want[0][3] + want[1][3]
+    # cvsd at K F = 2 from its definition: two fold means, weights N_0 and N_1
+    if K * F == 2:
+        m = np.array([dev[:, 0, folds[0] == f].mean(axis=1) for f in range(2)])       # [2, L]
+        N = np.bincount(folds[0], minlength=2).astype(np.float64)
+        cvm = (N[:, None] * m).sum(axis=0) / n
+        np.testing.assert_allclose(want[1], np.sqrt((N[:, None] * (m - cvm) ** 2).sum(axis=0) / n), rtol=1e-12)
+
+
+def test_heldout_deviance_clamps_at_glmnet_bound():
+    eta = np.array([-40.0, -3.0, 0.0, 2.5, 40.0, 11.6, -11.6])
+    y = np.array([1, 0, 1, 1, 0, 1, 0])
+    d = orc.heldout_deviance(eta, y)
+    p = 1 / (1 + np.exp(-eta))
+    assert d[0] == pytest.approx(-2 * np.log(1e-5), rel=1e-15)         # clamped from below
+    # y = 0, p clamped to 1 - 1e-5: 1 - (1 - 1e-5) is 1e-5 to 7e-12 relative in float64
+    assert d[4] == pytest.approx(-2 * np.log(1e-5), rel=1e-11)
+    np.testing.assert_allclose(d[[1, 2, 3]], [-2 * np.log(1 - p[1]), 2 * np.log(2), -2 * np.log(p[3])], rtol=1e-14)
+    assert d[5] == pytest.approx(-2 * np.log(1 - 1e-5), rel=1e-12)     # sigmoid(11.6) > 1 - 1e-5
+    assert d[6] == pytest.approx(-2 * np.log(1 - 1e-5), rel=1e-12)
+
+
 @pytest.mark.parametrize("kw,msg", [(dict(folds=1), "number of folds F"), (dict(folds=101), "number of folds F"),
                                     (dict(repeats=0), "number of repeats K"), (dict(repeats=101), "repeats K"),
                                     (dict(alpha=0.0), "alpha"), (dict(alpha=1.5), "alpha"),
